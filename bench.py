@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — QR GFLOP/s (fp64) of qr! on the BASELINE workload, one JSON line on rank 0.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 3|2] [--m M --n N --nb NB]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 3|2] [--m M --n N --nb NB] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -20,6 +20,10 @@ the N GPUs (strong scaling: total work fixed).  A "step" is one full factorisati
              whole sweep) and LAPACK dgeqrf, the reference tests' own normaliser (test/runtests.jl:49,53-54).
 --config 2 measures BASELINE configs[1] (8192 x 1024, nb = 1: the unblocked column loop) with an HBM roofline instead.
 --impl reference times the CPU restatement alone (the reference is Julia; Julia is not installed) on the same config.
+--dump-outputs DIR writes what the last timed qr! returned, before anything else touches it: DIR/alpha.npy (all n entries of
+alpha, float64) and DIR/H_sample.npy (float64: DUMP_SAMPLES entries of the factored matrix H at positions drawn by
+numpy.random.default_rng(DUMP_SEED), all rows first and then all columns, gathered from every rank).  The inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -33,6 +37,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 METRIC = "QR GFLOP/s (fp64)"
+DUMP_SAMPLES, DUMP_SEED = 1 << 20, 20240601    # 8 MiB sample of H: the whole matrix is 1 GiB at 32768 x 4096
 ORACLE_PIN = ("oracle = line-cited C restatement of the reference's recurrences; parity with the Julia binary itself is UNPINNED "
               "(no Julia in the image, no golden vectors upstream): pinned by LAPACK dgeqrf through the storage-format identity "
               "and by the reference's own test properties")
@@ -204,7 +209,25 @@ def hbm_peak():
     try:
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s of B200_PROFILING.md (of fallback: MEASURED_PEAKS.json absent on this box)"
+        return 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured: MEASURED_PEAKS.json absent)"
+
+
+def dump_outputs(torch, dist, A, alpha, m, n, c0, nl, world, rank, dev, out_dir):
+    """alpha and a seeded sample of H from the last timed step (see --dump-outputs); rank 0 writes the files."""
+    import numpy as np
+    rng = np.random.default_rng(DUMP_SEED)
+    rows = rng.integers(0, m, DUMP_SAMPLES)
+    cols = rng.integers(0, n, DUMP_SAMPLES)
+    r, c = torch.from_numpy(rows).to(dev), torch.from_numpy(cols).to(dev)
+    mine = (c >= c0) & (c < c0 + nl)
+    vals = torch.zeros(DUMP_SAMPLES, dtype=torch.float64, device=dev)
+    vals[mine] = A[r[mine], c[mine] - c0]
+    if world > 1:
+        dist.all_reduce(vals)                     # every position is owned by exactly one rank, the others contribute 0
+    if rank == 0:
+        os.makedirs(out_dir, exist_ok=True)
+        np.save(os.path.join(out_dir, "alpha.npy"), alpha.cpu().numpy().astype(np.float64))
+        np.save(os.path.join(out_dir, "H_sample.npy"), vals.cpu().numpy())
 
 
 def run_ours(args):
@@ -291,6 +314,8 @@ def run_ours(args):
     value = flops / (ms_per_step * 1e-3) / 1e9
     launches_all = int(sumover(float(launches)))
     last = pool[(K - 1) % pool_n]                 # the last timed factorisation (alpha belongs to it)
+    if args.dump_outputs:
+        dump_outputs(torch, dist, last, alpha, m, n, c0, nl, world, rank, dev, args.dump_outputs)
 
     # ---- parity of the last timed factorisation ------------------------------------------------------------------------
     parity = {"tolerance": 1e-13, "oracle_pin": ORACLE_PIN}
@@ -372,22 +397,15 @@ def run_ours(args):
                             "one-launch-per-column path the profiler needs)") if m <= 8192 and world == 1 else dom
             roof = {"bound": "hbm", "kernel": timed_kernel, "achieved": gbs, "peak": hp, "unit": "GB/s", "frac": gbs / hp, "traffic": None,
                     "algorithmic_bytes_per_step": 16.0 * E, "peak_source": hsrc,
-                    "note": "whole-factorisation algorithmic bytes / ms_per_step; the 64 MiB matrix is L2-resident (126 MB L2), so DRAM traffic is far below the algorithmic bytes and the fraction can exceed what HBM alone would allow",
+                    "note": "whole-factorisation algorithmic bytes / ms_per_step; the 64 MiB matrix exceeds the 50 MB L2, but the trailing matrix fits it after about a quarter of the column steps, so DRAM traffic is below the algorithmic bytes and the fraction can exceed what HBM alone would allow",
                     "share_of_step": prof[dom]["ms"] / tot if tot else None, "classes": classes}
         else:
             peak = dgemm_peak(torch, dev)
             dom = max((k for k in prof if k.startswith("k_gemm")), key=lambda k: prof[k]["ms"], default=None)
             if dom:
                 ach = prof[dom]["work"] / (prof[dom]["ms"] * 1e-3) / 1e12
-                traffic, tnote = None, None
-                try:
-                    tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))[dom]
-                    traffic, tnote = tj["dram_bytes_per_launch"], f"dram bytes of the largest launch ({tj['captured_launch']}), ncu --set full, {tj['source']}"
-                except Exception:
-                    pass
                 roof = {"bound": "tensor", "kernel": dom, "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-                        "traffic": traffic, "traffic_note": tnote,
-                        "peak_source": "cuBLAS DGEMM 8192^3 burst measured in this run (MEASURED_PEAKS.json has no fp64 entry); tcgen05 has no f64 kind, the fp64 tensor pipe is DMMA",
+                        "peak_source": "cuBLAS DGEMM 8192^3 burst measured in this run (MEASURED_PEAKS.json has no fp64 entry); the fp64 tensor pipe is DMMA (mma.sync f64)",
                         "launches": prof[dom]["count"], "avg_launch_ms": prof[dom]["ms"] / max(1, prof[dom]["count"]),
                         "share_of_step": prof[dom]["ms"] / tot if tot else None,
                         "whole_qr_frac_of_peak": value / 1e3 / peak / world, "classes": classes}
@@ -412,7 +430,7 @@ def run_ours(args):
         Ke = max(1, args.e2e_steps)
         tot_s = 0.0
         # Host-side analogue of the L2 flush between device-timed iterations: after the CPU has rewritten the pinned buffer a good part of
-        # it sits dirty in the CPU caches, and DMA reads of such lines are slower and noisy (3-8 ms per step, profiles/r02b_host_pipeline.txt).
+        # it sits dirty in the CPU caches, and DMA reads of such lines are slower and noisy.
         # Writing a scratch buffer larger than the last-level caches puts the input where a matrix that did not just come out of this
         # process's own memcpy would be: in DRAM.  Outside the timed region; the dirty-cache case is reported next to the headline.
         flush = torch.empty(1 << 27, dtype=torch.float64)
@@ -575,6 +593,8 @@ def main():
     ap.add_argument("--no-solve", action="store_true")
     ap.add_argument("--split", default="even", choices=["even", "balanced"],
                     help="column blocks: DArray default (even) or the reference's load-balanced contiguous split (T:35), rounded to panels")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write alpha and a seeded sample of H of the last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     dm, dn, dnb = (8192, 1024, 1) if args.config == 2 else (32768, 4096, 0)
     args.m, args.n = args.m or dm, args.n or dn

@@ -1,4 +1,4 @@
-"""dhqr_b200 — B200-native blocked Householder QR behind DistributedHouseholderQR.jl's qr! / \\.
+"""dhqr_b200 — H100-native (sm_90a) blocked Householder QR behind DistributedHouseholderQR.jl's qr! / \\.
 
 Import as ``import dhqr_b200`` (repo-root shim) — the directory keeps the name the task fixes
 (``distributedhouseholderqr.jl_b200``), which is not a valid Python identifier.

@@ -1,6 +1,6 @@
 // dhqr_api.cu — context, workspace, panel/update drivers and the C-ABI of libdhqr.so.
 // See include/dhqr.h for the contract; each entry point names the reference method it replaces
-// (S:n = /root/reference/src/DistributedHouseholderQR.jl:n).
+// (S:n = line n of the reference's src/DistributedHouseholderQR.jl).
 #include "../../include/dhqr.h"
 
 #include <cuda_runtime.h>
@@ -145,7 +145,7 @@ struct dhqr_context {
     int unblocked_wave = 1;                                             // nb = 1, m <= 8192: the column loop as one persistent launch
     unsigned int* uw_flags = nullptr; size_t uw_flags_n = 0; unsigned int uw_epoch = 0;
     int fuse_house = 1;                                                 // nb = 1: next reflector formed inside the apply kernel (one launch per column)
-    int cvy_persist = 1;                                                // 128-wide gemm_cvy: consecutive tiles per CTA (0: one-tile kernel)
+    int cvy_persist = 4;                                                // 128-wide gemm_cvy: consecutive tiles per CTA (0: one-tile kernel); 4 is fastest on an H100 at one CTA per SM
     int cvy_defer = 1;                                                  // 128-wide gemm_cvy: C tile read in batches behind the k-stages
     int cvy_warps = 8;                                                  // MMA warps per gemm_cvy CTA (4: 64x32 warp tiles, 8: 32x32)
     int tail_cols = 0;                                                  // trailing width below which the chain is considered critical
@@ -1254,7 +1254,8 @@ static int create_common(dhqr_handle* h, int device) {
     CU(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return set_err(5001, "libdhqr is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    // sm_90a code runs on compute capability 9.0 only (architecture-specific features do not carry forward)
+    if (prop.major != 9 || prop.minor != 0) return set_err(5001, "libdhqr is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
     dhqr_context* c = new dhqr_context();
     c->device = device;
     c->sms = prop.multiProcessorCount;

@@ -1,4 +1,4 @@
-# DistributedHouseholderQRB200.jl — drop-in for DistributedHouseholderQR.qr! / \ on B200 GPUs.
+# DistributedHouseholderQRB200.jl — drop-in for DistributedHouseholderQR.qr! / \ on H100 GPUs.
 #
 # UNEXECUTED in this repository's CI image (no Julia there); it documents the reference-side binding a
 # maintainer adds.  Every method names the reference method it replaces

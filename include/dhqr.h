@@ -1,5 +1,5 @@
 /*
- * dhqr.h — C-ABI of libdhqr.so: B200-native (sm_100a) blocked Householder QR behind
+ * dhqr.h — C-ABI of libdhqr.so: H100-native (sm_90a) blocked Householder QR behind
  * DistributedHouseholderQR.jl's qr! / \ entry points.
  *
  * The reference (pure Julia) has no FFI of its own; each entry point below names the Julia

@@ -6,7 +6,7 @@
  * (libdhqr.so) never links, loads or falls back to anything in oracle/.
  *
  * Every function cites the reference lines it follows, with
- *   S:n = /root/reference/src/DistributedHouseholderQR.jl line n.
+ *   S:n = line n of the reference's src/DistributedHouseholderQR.jl.
  *
  * Parity status: the reference ships no golden vectors (its tests draw from Julia's
  * Xoshiro stream, test/runtests.jl:6,45-46) and Julia is not installed, so this

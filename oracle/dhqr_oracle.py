@@ -4,7 +4,7 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl refere
 this module; the product path (libdhqr.so + the dhqr_b200 host package) never does.
 
 Four things live here, each citing the reference lines it follows
-(S:n = /root/reference/src/DistributedHouseholderQR.jl:n, T:n = test/runtests.jl:n):
+(S:n = line n of the reference's src/DistributedHouseholderQR.jl, T:n = test/runtests.jl:n):
 
 * ``COracle``  — ctypes binding of oracle/dhqr_oracle.c (the C restatement, OpenMP threads over
   trailing-column chunks like S:203-211).

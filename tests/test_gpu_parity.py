@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C-ABI
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C-ABI
 (dhqr_b200 -> ctypes -> libdhqr.so), against the CPU oracle, the committed golden fixtures, LAPACK, and —
 at BASELINE's full sizes — size-independent properties.
 
@@ -54,7 +54,7 @@ def gpu_residual(D, A, alpha, A0):
 
 # ---------------------------------------------------------------------------------------------
 def test_native_library_is_what_runs(D):
-    # the .so must be loaded in-tree and be the sm_100a build; no fallback exists
+    # the .so must be loaded in-tree and be the sm_90a build; no fallback exists
     assert os.path.exists(D._lib.LIB_PATH)
     h = D.default_handle(0)
     assert h.get_option("sms") > 0

@@ -88,7 +88,7 @@ def test_plan_invariants(mnb):
 def test_default_plan_of_the_bench_workload():
     b, j = D.plan_host_upload(32768, 4096)
     assert b == [0, 384, 768, 1280, 1792, 2304, 2816, 3328, 3840, 4096]
-    assert j == [0, 0, 3, 7, 11, 15, 19, 23, 27]                       # deadline joins (profiles/r02b_host_pipeline.txt)
+    assert j == [0, 0, 3, 7, 11, 15, 19, 23, 27]                       # deadline joins
 
 
 @pytest.mark.parametrize("mnb", [(700, 640, 32), (900, 768, 64), (1300, 1152, 96), (1100, 1024, 128)])

@@ -9,7 +9,7 @@ rows = 32768
 vp = lambda t: C.c_void_p(t.data_ptr()); sp = lambda: C.c_void_p(torch.cuda.current_stream().cuda_stream)
 P = D.colmajor_empty(rows, 32, dev); al = torch.zeros(32, dtype=torch.float64, device=dev)
 names = ["", "gram1+exch", "chol1", "trsm1", "gram2+exch", "chol2", "trsm2", "Rt+topLU+exch", "rows+top write"]
-for pc in (64, 148):
+for pc in (64, 132):
     h.set_option("panel_ctas", pc); h.set_option("panel_trace", 1)
     for rep in range(3):
         D.fill_uniform_(P, 1); torch.cuda.synchronize()

@@ -7,7 +7,7 @@ import dhqr_b200 as D
 dev = torch.device("cuda:0"); h = D.default_handle(0)
 m, n = 32768, 4096
 A = D.colmajor_empty(m, n, dev); al = torch.zeros(n, dtype=torch.float64, device=dev)
-for tag, opts in (("default", {}), ("panel_ctas=96", {"panel_ctas": 96}), ("panel_ctas=148", {"panel_ctas": 148})):
+for tag, opts in (("default", {}), ("panel_ctas=96", {"panel_ctas": 96}), ("panel_ctas=132", {"panel_ctas": 132})):
     for k, v in opts.items(): h.set_option(k, v)
     for rep in range(2):
         D.fill_uniform_(A, 0); torch.cuda.synchronize()

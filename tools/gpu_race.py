@@ -14,7 +14,7 @@ def experiment(rows, nbp, ncols, iters):
     P = co.fill_uniform(3, rows, nbp); Hp, _ = co.qr(P)
     V = D.to_colmajor(np.tril(Hp), dev)
     C0 = D.colmajor_empty(rows, ncols, dev); D.fill_uniform_(C0, 5)
-    nw = min(64 * 1024 * 1024 // 8, 3 * 148 * 128 * 128)
+    nw = min(64 * 1024 * 1024 // 8, 3 * 132 * 128 * 128)
     ny = 4 * 64 * 36 * ((ncols + 63) // 64)
     ref = None; bad = 0
     for it in range(iters):

@@ -16,7 +16,7 @@ def timeit(reps=3):
         best = min(best, e0.elapsed_time(e1))
     return best
 base = {"hp_max_ctas": 0, "panel_ctas": 0, "vta_max_chunks": 0}
-sweep = ({}, {"panel_ctas": 32}, {"panel_ctas": 48}, {"panel_ctas": 64}, {"panel_ctas": 96}, {"panel_ctas": 128}, {"panel_ctas": 148})
+sweep = ({}, {"panel_ctas": 32}, {"panel_ctas": 48}, {"panel_ctas": 64}, {"panel_ctas": 96}, {"panel_ctas": 128}, {"panel_ctas": 132})
 for opts in sweep:
     for k, v in {**base, **opts}.items(): h.set_option(k, v)
     t = timeit(); print(f"{opts}: {t:.2f} ms  {fl / t / 1e9:.2f} TFLOP/s", flush=True)

@@ -1,9 +1,9 @@
-// fp64 tensor pipe (DMMA.8x8x4) issue-rate microbenchmark for sm_100a:
+// fp64 tensor pipe (DMMA.8x8x4) issue-rate microbenchmark for sm_90a:
 //   mode 0: registers only, ILP independent accumulators per warp, W warps per CTA, one CTA per SM
 //   mode 1: the gemm_cvy inner step (4 A + 4 B fragment LDS.64, then 16 DMMA), fragments loaded right before use
 //   mode 2: the same with the next k-step's fragments loaded before the current step's DMMAs (software pipelined)
 //   mode 3: 64x32 warp tile (8 A + 4 B fragments, 32 DMMA per k-step), software pipelined
-// build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o build/dmma_rate tools/micro/dmma_rate.cu
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o build/dmma_rate tools/micro/dmma_rate.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {

@@ -70,10 +70,10 @@ __global__ void k_lat(double* out, long long* cyc, double seed) {
 }
 int main() {
     double* out; long long* cyc;
-    cudaMalloc(&out, 8 * 148 * 1024); cudaMalloc(&cyc, 8 * 64);
+    cudaMalloc(&out, 8 * 132 * 1024); cudaMalloc(&cyc, 8 * 64);
     const char* names[] = {"dep DFMA", "dep DMUL", "dep DADD", "dep rsqrt+add", "dep div+add", "dep sqrt+add", "dep shfl64", "8 indep DFMA chains (per 8 ops)", "dep rcp.approx+2 Newton+add"};
     for (int threads : {32, 128, 512}) {
-        for (int rep = 0; rep < 2; ++rep) k_lat<<<148, threads>>>(out, cyc, 1.5);
+        for (int rep = 0; rep < 2; ++rep) k_lat<<<132, threads>>>(out, cyc, 1.5);
         cudaDeviceSynchronize();
         long long h[16]; cudaMemcpy(h, cyc, sizeof(long long) * 9, cudaMemcpyDeviceToHost);
         printf("threads per CTA = %d (one CTA per SM)\n", threads);
