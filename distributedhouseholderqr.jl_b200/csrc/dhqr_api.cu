@@ -1450,6 +1450,18 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
     else if (!strcmp(key, "lookahead")) *value = c->lookahead;
     else if (!strcmp(key, "panel_fast")) *value = c->panel_fast;
     else if (!strcmp(key, "wide_panel")) *value = c->wide_panel;
+    else if (!strcmp(key, "cvy_warps")) *value = c->cvy_warps;
+    else if (!strcmp(key, "cvy_persist")) *value = c->cvy_persist;
+    else if (!strcmp(key, "cvy_defer")) *value = c->cvy_defer;
+    else if (!strcmp(key, "gram_sym")) *value = c->gram_sym;
+    else if (!strcmp(key, "wide_trecon")) *value = c->wide_trecon;
+    else if (!strcmp(key, "wide_aux")) *value = c->wide_aux;
+    else if (!strcmp(key, "hp2")) *value = c->hp2;
+    else if (!strcmp(key, "qt_vec")) *value = c->qt_vec;
+    else if (!strcmp(key, "bs_wave")) *value = c->bs_wave;
+    else if (!strcmp(key, "unblocked_wave")) *value = c->unblocked_wave;
+    else if (!strcmp(key, "fuse_house")) *value = c->fuse_house;
+    else if (!strcmp(key, "host_chunk")) *value = c->host_chunk;
     else if (!strcmp(key, "wide_panels")) *value = c->wide_panels;
     else if (!strcmp(key, "wide_redone")) *value = c->wide_redone;
     else if (!strcmp(key, "panel_variant")) *value = PANEL_VARIANT;

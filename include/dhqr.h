@@ -82,6 +82,8 @@ int dhqr_destroy(dhqr_handle h);
  *                 "host_trace" 1: stage timeline on stderr.  A wrong assumption costs idle time, never correctness
  *   "sync"        1: cudaStreamSynchronize + error check after every kernel launch (debugging; implies serial)
  *   "profile"     1: CUDA-event bracket per launch (implies serial), read with dhqr_profile_get
+ *   also readable: "cvy_persist", "cvy_defer", "wide_trecon", "wide_aux", "hp2", "bs_wave", "unblocked_wave", "fuse_house"
+ *                 (kernel and schedule variants, see dhqr_api.cu), so that a caller can put back what it changed
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
  *                 "panel_variant" (compile-time DHQR_PANEL_VARIANT of the panel kernel's fast path)

@@ -21,6 +21,7 @@
  * A "column block" is the localpart of the reference's DArray with a (1,P) process grid
  * (test/runtests.jl:71): all m rows of a contiguous global column range (S:33).
  */
+#include <float.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -269,6 +270,191 @@ int dhqr_oracle_ldiv(int64_t m, int64_t n, const double *a, int64_t lda, const d
     if (!rc) memcpy(x, w, (size_t)n * sizeof(double));             /* S:320 */
     free(w);
     return rc;
+}
+
+/* ---------------------------------------------------------------------------------------------------------------------
+ * Extended-precision reference.  The same recurrences as above (S:127-135 column step, S:208-209 trailing update,
+ * S:232-242 Q'b sweep, S:256-282 back-substitution, S:317-321 ldiv) carried out in long double and rounded to double only
+ * when written out.  Its forward error against exact arithmetic is about kappa * 2^-LDBL_MANT_DIG instead of
+ * kappa * 2^-53, so it can measure the fp64 oracle's error and the library's error on the same input, also on inputs
+ * where kappa * 1e-16 is large.  Each trailing column is updated by one thread with a sequential sum, so the result does
+ * not depend on the thread count.
+ * --------------------------------------------------------------------------------------------------------------------- */
+typedef long double ldbl;
+
+int dhqr_oracle_ext_mant_dig(void) { return LDBL_MANT_DIG; }
+
+/* S:127-135 + S:208-209 on an m x n long double matrix (leading dimension m) */
+static void ext_factor(int64_t m, int64_t n, ldbl *w, ldbl *alpha, int nthreads) {
+    for (int64_t j = 0; j < n; ++j) {
+        ldbl *col = w + j * m;
+        ldbl s = 0.0L;
+        for (int64_t i = j; i < m; ++i) s += col[i] * col[i];
+        s = sqrtl(s);                                                  /* S:129 */
+        const ldbl x = col[j];
+        alpha[j] = s * (x > 0.0L ? -1.0L : (x < 0.0L ? 1.0L : -0.0L * 0.0L));   /* S:130, S:8 */
+        const ldbl f = 1.0L / sqrtl(s * (s + fabsl(x)));             /* S:131 */
+        col[j] -= alpha[j];                                            /* S:132 */
+        for (int64_t i = j; i < m; ++i) col[i] *= f;                   /* S:133-135 */
+#pragma omp parallel for schedule(static) num_threads(nthreads)
+        for (int64_t jj = j + 1; jj < n; ++jj) {
+            ldbl *d = w + jj * m;
+            ldbl t = 0.0L;
+            for (int64_t i = j; i < m; ++i) t += col[i] * d[i];        /* S:208 */
+            for (int64_t i = j; i < m; ++i) d[i] -= col[i] * t;        /* S:209 */
+        }
+    }
+}
+
+/* b <- Q'b (S:232-242) or b <- Qb (the same reflectors in reverse order) */
+static void ext_apply(int64_t m, int64_t n, const ldbl *w, ldbl *b, int trans) {
+    for (int64_t q = 0; q < n; ++q) {
+        const int64_t j = trans ? q : n - 1 - q;
+        const ldbl *col = w + j * m;
+        ldbl s = 0.0L;
+        for (int64_t i = j; i < m; ++i) s += col[i] * b[i];           /* S:237 */
+        for (int64_t i = j; i < m; ++i) b[i] -= col[i] * s;            /* S:238-240 */
+    }
+}
+
+/* S:256-282: b[i] = (b[i] - sum_{k>i} R[i,k] b[k]) / alpha[i], i = n..1 */
+static void ext_backsolve(int64_t m, int64_t n, const ldbl *w, const ldbl *alpha, ldbl *b) {
+    for (int64_t i = n - 1; i >= 0; --i) {
+        ldbl sum = 0.0L;
+        for (int64_t k = i + 1; k < n; ++k) sum += w[i + k * m] * b[k];
+        b[i] = (b[i] - sum) / alpha[i];
+    }
+}
+
+/* qr!(A) in long double; a (lda) is overwritten with H, alpha with diag(R), both rounded to double.  With nrhs > 0 the
+ * right-hand sides b (m x nrhs, ldb) go through the long double factorisation too: qtb = Q'b (m x nrhs, leading dimension m),
+ * qb = Qb (same shape) and x = H \ b (S:317-321; n x nrhs, leading dimension n).  Any of qtb, qb, x may be NULL. */
+int dhqr_oracle_qr_ext(int64_t m, int64_t n, double *a, int64_t lda, double *alpha, int nrhs, const double *b, int64_t ldb,
+                       double *qtb, double *qb, double *x, int nthreads) {
+    if (m < 0) return -1;
+    if (n < 0 || n > m) return -2;
+    if (lda < (m > 1 ? m : 1)) return -4;
+    if (nrhs > 0 && (!b || ldb < m)) return -5;
+    if (nthreads < 1) nthreads = dhqr_oracle_max_threads();
+    ldbl *w = (ldbl *)malloc(sizeof(ldbl) * (size_t)(m > 0 ? m : 1) * (size_t)(n > 0 ? n : 1));
+    ldbl *al = (ldbl *)malloc(sizeof(ldbl) * (size_t)(n > 0 ? n : 1));
+    ldbl *v = (ldbl *)malloc(sizeof(ldbl) * (size_t)(m > 0 ? m : 1));
+    if (!w || !al || !v) { free(w); free(al); free(v); return -100; }
+    for (int64_t j = 0; j < n; ++j)
+        for (int64_t i = 0; i < m; ++i) w[i + j * m] = a[i + j * lda];
+    ext_factor(m, n, w, al, nthreads);
+    for (int64_t j = 0; j < n; ++j) {
+        alpha[j] = (double)al[j];
+        for (int64_t i = 0; i < m; ++i) a[i + j * lda] = (double)w[i + j * m];
+    }
+    for (int r = 0; r < nrhs; ++r) {
+        const double *br = b + (int64_t)r * ldb;
+        if (qb) {
+            for (int64_t i = 0; i < m; ++i) v[i] = br[i];
+            ext_apply(m, n, w, v, 0);
+            for (int64_t i = 0; i < m; ++i) qb[i + (int64_t)r * m] = (double)v[i];
+        }
+        for (int64_t i = 0; i < m; ++i) v[i] = br[i];
+        ext_apply(m, n, w, v, 1);                                      /* S:288 */
+        if (qtb)
+            for (int64_t i = 0; i < m; ++i) qtb[i + (int64_t)r * m] = (double)v[i];
+        if (x) {
+            ext_backsolve(m, n, w, al, v);                             /* S:291 */
+            for (int64_t i = 0; i < n; ++i) x[i + (int64_t)r * n] = (double)v[i];
+        }
+    }
+    free(w); free(al); free(v);
+    return 0;
+}
+
+/* ComplexF64 twin (S:9, S:51-59, S:162-196), real and imaginary parts kept as separate long doubles.  Interleaved complex128
+ * in and out; same arguments as dhqr_oracle_qr_ext without qb (the library's apply_q_ is Float64 only). */
+int dhqr_oracle_qr_ext_c(int64_t m, int64_t n, double *a, int64_t lda, double *alpha, int nrhs, const double *b, int64_t ldb,
+                         double *qtb, double *x, int nthreads) {
+    if (m < 0) return -1;
+    if (n < 0 || n > m) return -2;
+    if (lda < (m > 1 ? m : 1)) return -4;
+    if (nrhs > 0 && (!b || ldb < m)) return -5;
+    if (nthreads < 1) nthreads = dhqr_oracle_max_threads();
+    const size_t mn = (size_t)(m > 0 ? m : 1) * (size_t)(n > 0 ? n : 1);
+    ldbl *wr = (ldbl *)malloc(sizeof(ldbl) * mn), *wi = (ldbl *)malloc(sizeof(ldbl) * mn);
+    ldbl *ar = (ldbl *)malloc(sizeof(ldbl) * (size_t)(n > 0 ? n : 1)), *ai = (ldbl *)malloc(sizeof(ldbl) * (size_t)(n > 0 ? n : 1));
+    ldbl *vr = (ldbl *)malloc(sizeof(ldbl) * (size_t)(m > 0 ? m : 1)), *vi = (ldbl *)malloc(sizeof(ldbl) * (size_t)(m > 0 ? m : 1));
+    if (!wr || !wi || !ar || !ai || !vr || !vi) { free(wr); free(wi); free(ar); free(ai); free(vr); free(vi); return -100; }
+    for (int64_t j = 0; j < n; ++j)
+        for (int64_t i = 0; i < m; ++i) {
+            wr[i + j * m] = a[2 * (i + j * lda)];
+            wi[i + j * m] = a[2 * (i + j * lda) + 1];
+        }
+    for (int64_t j = 0; j < n; ++j) {
+        ldbl *cr = wr + j * m, *ci = wi + j * m;
+        ldbl s = 0.0L;
+        for (int64_t i = j; i < m; ++i) s += cr[i] * cr[i] + ci[i] * ci[i];
+        s = sqrtl(s);                                                  /* S:129 */
+        const ldbl xr = cr[j], xi = ci[j], ax = hypotl(xr, xi);
+        /* S:130, S:9: alpha = -exp(im*angle(x)) * s; angle(0) = 0 */
+        ar[j] = ax > 0.0L ? -s * (xr / ax) : -s;
+        ai[j] = ax > 0.0L ? -s * (xi / ax) : 0.0L;
+        const ldbl f = 1.0L / sqrtl(s * (s + ax));                    /* S:131 */
+        cr[j] -= ar[j];                                                /* S:132 */
+        ci[j] -= ai[j];
+        for (int64_t i = j; i < m; ++i) { cr[i] *= f; ci[i] *= f; }    /* S:133-135 */
+#pragma omp parallel for schedule(static) num_threads(nthreads)
+        for (int64_t jj = j + 1; jj < n; ++jj) {
+            ldbl *dr = wr + jj * m, *di = wi + jj * m;
+            ldbl tr = 0.0L, ti = 0.0L;                                 /* S:51-59: sum conj(v) d */
+            for (int64_t i = j; i < m; ++i) {
+                tr += cr[i] * dr[i] + ci[i] * di[i];
+                ti += cr[i] * di[i] - ci[i] * dr[i];
+            }
+            for (int64_t i = j; i < m; ++i) {                          /* S:162-196: d -= v t */
+                dr[i] -= cr[i] * tr - ci[i] * ti;
+                di[i] -= cr[i] * ti + ci[i] * tr;
+            }
+        }
+    }
+    for (int64_t j = 0; j < n; ++j) {
+        alpha[2 * j] = (double)ar[j];
+        alpha[2 * j + 1] = (double)ai[j];
+        for (int64_t i = 0; i < m; ++i) {
+            a[2 * (i + j * lda)] = (double)wr[i + j * m];
+            a[2 * (i + j * lda) + 1] = (double)wi[i + j * m];
+        }
+    }
+    for (int r = 0; r < nrhs; ++r) {
+        const double *br = b + 2 * (int64_t)r * ldb;
+        for (int64_t i = 0; i < m; ++i) { vr[i] = br[2 * i]; vi[i] = br[2 * i + 1]; }
+        for (int64_t j = 0; j < n; ++j) {                              /* S:232-242 with the complex partialdot */
+            const ldbl *cr = wr + j * m, *ci = wi + j * m;
+            ldbl tr = 0.0L, ti = 0.0L;
+            for (int64_t i = j; i < m; ++i) {
+                tr += cr[i] * vr[i] + ci[i] * vi[i];
+                ti += cr[i] * vi[i] - ci[i] * vr[i];
+            }
+            for (int64_t i = j; i < m; ++i) {
+                vr[i] -= cr[i] * tr - ci[i] * ti;
+                vi[i] -= cr[i] * ti + ci[i] * tr;
+            }
+        }
+        if (qtb)
+            for (int64_t i = 0; i < m; ++i) { qtb[2 * (i + (int64_t)r * m)] = (double)vr[i]; qtb[2 * (i + (int64_t)r * m) + 1] = (double)vi[i]; }
+        if (x) {
+            for (int64_t i = n - 1; i >= 0; --i) {                     /* S:256-282, no conjugation */
+                ldbl sr = 0.0L, si = 0.0L;
+                for (int64_t k = i + 1; k < n; ++k) {
+                    const ldbl hr = wr[i + k * m], hi = wi[i + k * m];
+                    sr += hr * vr[k] - hi * vi[k];
+                    si += hr * vi[k] + hi * vr[k];
+                }
+                const ldbl nr = vr[i] - sr, ni = vi[i] - si, d = ar[i] * ar[i] + ai[i] * ai[i];
+                vr[i] = (nr * ar[i] + ni * ai[i]) / d;
+                vi[i] = (ni * ar[i] - nr * ai[i]) / d;
+            }
+            for (int64_t i = 0; i < n; ++i) { x[2 * (i + (int64_t)r * n)] = (double)vr[i]; x[2 * (i + (int64_t)r * n) + 1] = (double)vi[i]; }
+        }
+    }
+    free(wr); free(wi); free(ar); free(ai); free(vr); free(vi);
+    return 0;
 }
 
 /* Synthetic inputs: A[i,j] ~ U[0,1) mirroring rand(T,m,n) at test/runtests.jl:45-46.  Julia's

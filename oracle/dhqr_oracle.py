@@ -7,7 +7,8 @@ Four things live here, each citing the reference lines it follows
 (S:n = line n of the reference's src/DistributedHouseholderQR.jl, T:n = test/runtests.jl:n):
 
 * ``COracle``  — ctypes binding of oracle/dhqr_oracle.c (the C restatement, OpenMP threads over
-  trailing-column chunks like S:203-211).
+  trailing-column chunks like S:203-211), including ``qr_ext`` / ``qr_ext_c``: the same recurrences in long double, the
+  yardstick for the accuracy of both the fp64 oracle and the library.
 * ``np_*``     — a pure-numpy twin of the same recurrences (small cases; independent code path).
 * ``np_*_c``   — the same recurrences for ComplexF64 (S:9, S:51-59, S:162-196; the reference tests both element types,
   T:43): oracle only so far, there is no complex CUDA path to check against it yet.
@@ -78,10 +79,65 @@ class COracle:
         L.dhqr_oracle_fill_uniform.restype = None
         L.dhqr_oracle_fill_uniform.argtypes = [C.c_uint64, i64, i64, i64, i64, vp, i64]
         L.dhqr_oracle_max_threads.restype = ci
+        L.dhqr_oracle_ext_mant_dig.restype = ci
+        L.dhqr_oracle_qr_ext.argtypes = [i64, i64, vp, i64, vp, ci, vp, i64, vp, vp, vp, ci]
+        L.dhqr_oracle_qr_ext_c.argtypes = [i64, i64, vp, i64, vp, ci, vp, i64, vp, vp, ci]
 
     # -- scalars / primitives -------------------------------------------------
     def max_threads(self) -> int:
         return int(self.lib.dhqr_oracle_max_threads())
+
+    def ext_mant_dig(self) -> int:
+        """Significand bits of the extended-precision reference (LDBL_MANT_DIG: 64 on x86-64, 113 on aarch64)."""
+        return int(self.lib.dhqr_oracle_ext_mant_dig())
+
+    # -- extended-precision reference (same recurrences in long double) ---------------------------------------------
+    def _ext(self, a, b, nthreads, want_qb, cplx):
+        dt = np.complex128 if cplx else np.float64
+        h = np.array(a, dtype=dt, order="F", copy=True)
+        m, n = h.shape
+        alpha = np.zeros(n, dtype=dt)
+        bb = None if b is None else np.asfortranarray(np.asarray(b, dtype=dt).reshape(m, -1))
+        k = 0 if bb is None else bb.shape[1]
+        qtb = np.zeros((m, k), dtype=dt, order="F")
+        qb = np.zeros((m, k), dtype=dt, order="F") if want_qb else None
+        x = np.zeros((n, k), dtype=dt, order="F")
+        if nthreads <= 0:
+            nthreads = self.max_threads()
+        p = lambda t: None if t is None or t.size == 0 else C.c_void_p(t.ctypes.data)
+        lda, ldb = max(m, 1), max(m, 1)
+        if cplx:
+            rc = self.lib.dhqr_oracle_qr_ext_c(m, n, p(h), lda, p(alpha), k, p(bb), ldb, p(qtb), p(x), nthreads)
+        else:
+            rc = self.lib.dhqr_oracle_qr_ext(m, n, p(h), lda, p(alpha), k, p(bb), ldb, p(qtb), p(qb), p(x), nthreads)
+        if rc:
+            raise RuntimeError(f"dhqr_oracle_qr_ext rc={rc}")
+        return h, alpha, qtb, qb, x
+
+    def qr_ext(self, a: np.ndarray, b=None, nthreads: int = 0, want_qb: bool = False):
+        """qr!(A) in long double, rounded to double: returns (H, alpha) without touching ``a``.  With ``b`` (length m, or
+        m x k) the right-hand sides go through the long double factorisation as well and the result is
+        (H, alpha, Q'b, Qb or None, H \\ b), each of shape (m, k) / (n, k)."""
+        h, alpha, qtb, qb, x = self._ext(a, b, nthreads, want_qb, False)
+        return (h, alpha) if b is None else (h, alpha, qtb, qb, x)
+
+    def apply_qt_ext(self, a: np.ndarray, b: np.ndarray, nthreads: int = 0) -> np.ndarray:
+        """Q'b (S:232-242) with Q from the long double factorisation of ``a`` (the input matrix, not H)."""
+        return self._ext(a, b, nthreads, False, False)[2].reshape(np.shape(b))
+
+    def ldiv_ext(self, a: np.ndarray, b: np.ndarray, nthreads: int = 0) -> np.ndarray:
+        """qr!(A) \\ b (S:317-321) entirely in long double; ``a`` is the input matrix."""
+        x = self._ext(a, b, nthreads, False, False)[4]
+        return x[:, 0] if np.ndim(b) == 1 else x
+
+    def qr_ext_c(self, a: np.ndarray, b=None, nthreads: int = 0):
+        """ComplexF64 twin of qr_ext (np_qr_c / np_apply_qt_c in long double): (H, alpha) or (H, alpha, Q'b, H \\ b)."""
+        h, alpha, qtb, _, x = self._ext(a, b, nthreads, False, True)
+        return (h, alpha) if b is None else (h, alpha, qtb, x)
+
+    def ldiv_ext_c(self, a: np.ndarray, b: np.ndarray, nthreads: int = 0) -> np.ndarray:
+        x = self._ext(a, b, nthreads, False, True)[4]
+        return x[:, 0] if np.ndim(b) == 1 else x
 
     def alphafactor(self, x: float) -> float:
         return float(self.lib.dhqr_oracle_alphafactor(float(x)))

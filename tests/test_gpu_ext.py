@@ -1,0 +1,463 @@
+"""Every code path of the factorisation against the extended-precision reference, on inputs where kernels go wrong (run with
+-m gpu on an H100).
+
+The reference is oracle/dhqr_oracle.c's loop in long double (COracle.qr_ext): the reference's recurrences with a forward error
+of about kappa * 1e-19.  The fp64 oracle runs the same loop in double, so its error against the extended reference on the
+same input is what the reference algorithm in the reference's precision achieves.  The library is held to that:
+
+    err_gpu <= C_REL * max(err_fp64_oracle, FLOOR)        for each metric below, on every family and path
+
+Metrics (all against the extended reference; tests/matrix_families.py has the inputs):
+    V     max |dH| over the lower trapezoid (the reflectors, entries O(1) since |v|^2 = 2)
+    R     max |dR_ij| / ||A[:, j]|| over the strict upper triangle and alpha (column-relative: R spans 10^+-120 in colscale)
+    qtb   ||d(Q'b)|| / ||b||          qb  ||d(Qb)|| / ||b||          x   ||dx|| / ||x||
+FLOOR = 16 eps for V and R, 16 eps sqrt(m) for the solve metrics.  Two absolute bounds on every family inside the reference's
+range:
+    bwd   max_j ||(QR - A)[:, j]|| / ||A[:, j]|| < 1e-13
+    orth  max_j | ||v_j||^2 - 2 | < 1e-13
+Where a variant runs the same floating-point operations in the same order as another path, the two must agree bit for bit.
+
+A table of err_gpu / max(err_fp64_oracle, FLOOR) per path x family is written to build/test_gpu_ext_ratios.md.
+"""
+import contextlib
+import hashlib
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import matrix_families as F
+
+pytestmark = pytest.mark.gpu
+
+EPS = np.finfo(np.float64).eps
+C_REL = 8            # headroom over the fp64 oracle: the blocked paths sum in other orders (split-K, CholeskyQR2 + reconstruction)
+# Where the floor decides, the margin is thinnest: on triangular input the oracle's reflectors are +-sqrt(2) e_j to an ulp, while
+# the blocked update still rounds every R entry once per 128-column panel to its left and in its split-K sums.  Measured on an
+# H100 SXM (132 SMs): R error 98 eps (ratio 6.1) at 4099 x 640, 1.5 at 2048 x 1024; every non-triangular cell <= 1.5.  Split
+# counts follow the SM count, so a part with other SMs moves this cell first; a ratio near 8 there is summation order, not a bug.
+FLOOR_EPS = 16       # FLOOR = 16 eps x size factor: for inputs where the fp64 oracle happens to be (nearly) exact, e.g. triangular
+SIZE = {"V": lambda m: 1.0, "R": lambda m: 1.0,            # one rounded result of a stable recurrence per entry: the oracle lands at 1-4 eps
+        "qtb": np.sqrt, "qb": np.sqrt, "x": np.sqrt}        # a sweep over m rows: rounding errors add up like a random walk
+TOL_BWD = 1e-13      # column-wise backward error: Householder QR is column-wise backward stable whatever kappa is
+TOL_ORTH = 1e-13     # |v_j|^2 = 2 exactly in exact arithmetic (S:131-135)
+COUNTERS = ("wide_panels", "wide_redone", "panels_fast", "panels_fallback")
+
+# path -> (m, n, nb, extra rows of lda, options, path whose output it must equal bit for bit)
+PATHS = {
+    # blocked, default: 128-column wide chain + look-ahead
+    "default": (2048, 1024, 0, 0, {}, None),
+    # narrow (32-column) chain
+    "wide_panel0": (2048, 1024, 0, 0, {"wide_panel": 0}, None),
+    "nb32": (2048, 1024, 32, 0, {}, None),
+    "nb64": (2048, 1024, 64, 0, {}, None),
+    "nb96": (2048, 1024, 96, 0, {}, None),
+    "panel_fast0": (2048, 1024, 0, 0, {"wide_panel": 0, "panel_fast": 0}, None),
+    # serial schedules.  profile and sync both take the serial driver with the wide chain's side kernels on the main stream:
+    # the same kernels, splits and order as lookahead = 0 (whose side stream only changes when they run)
+    "lookahead0": (2048, 1024, 0, 0, {"lookahead": 0}, None),
+    "profile1": (2048, 1024, 0, 0, {"profile": 1}, "lookahead0"),
+    "sync1": (2048, 1024, 0, 0, {"sync": 1}, "lookahead0"),
+    # kernel variants.  gram_sym = 0 (k_gemm_vta + k_wreduce: other split-K partials), wide_trecon = 0 (T' by k_tinv from V'V
+    # instead of from the reconstruction) and cvy_defer = 0 (K_G2W: the accumulators start at C instead of adding C after a
+    # k-stage; it only takes the 128-wide update when cvy_persist = 0) change the arithmetic: relative rule only
+    "gram_sym0": (2048, 1024, 0, 0, {"gram_sym": 0}, None),
+    "wide_trecon0": (2048, 1024, 0, 0, {"wide_trecon": 0}, None),
+    "cvy_defer0": (2048, 1024, 0, 0, {"cvy_persist": 0, "cvy_defer": 0}, None),
+    # wide_aux = 0 / hp2 = 0 move the same launches (same workspace sizes, hence the same splits) onto another stream;
+    # cvy_persist = 0 runs K_G2D (k_gemm_cvy<4,..,DEFER>) one tile per CTA, the tile code of k_gemm_cvy_p
+    "wide_aux0": (2048, 1024, 0, 0, {"wide_aux": 0}, "default"),
+    "hp2_0": (2048, 1024, 0, 0, {"hp2": 0}, "default"),
+    "cvy_persist0": (2048, 1024, 0, 0, {"cvy_persist": 0}, "default"),
+    # cvy_warps = 4 (K_G2: 64x32 warp tiles) and K_G2W (32x32) both start from C and walk k in the same order per element
+    "cvy_warps4": (2048, 1024, 0, 0, {"cvy_warps": 4}, "cvy_defer0"),
+    # odd lda, a row count that is not a multiple of anything
+    "lda+3": (4099, 640, 0, 3, {}, None),
+    # nb = 1: persistent k_unblocked_wave (m <= 8192); fused k_house1 + k_apply1_tma chain (m <= 8531: its tile is sized by
+    # (m + 2) & ~1 rows; odd lda at 8193 and 8531); above that one launch pair per column, k_apply1_tma while the tile of
+    # (len + lead + 1) & ~1 rows fits 200 KiB: the whole of m = 8532, and k_apply1_direct for the first steps from m = 8533 on
+    # (steps 0 and 1 at 8533, steps 0..469 at 9000; all of 32768 x 256 below)
+    "nb1_m8192": (8192, 128, 1, 0, {}, None),
+    "nb1_m8193": (8193, 128, 1, 0, {}, None),
+    "nb1_m8531": (8531, 128, 1, 0, {}, None),
+    "nb1_m8532": (8532, 128, 1, 0, {}, None),
+    "nb1_m8533": (8533, 128, 1, 0, {}, None),
+    "nb1_9000x600": (9000, 600, 1, 0, {}, None),
+    "nb1_wave0": (4096, 512, 1, 0, {"unblocked_wave": 0}, None),
+    "nb1_fuse0": (4096, 512, 1, 0, {"fuse_house": 0}, None),
+    "nb1_lda+3": (4096, 512, 1, 3, {}, None),
+}
+BITWISE_TARGETS = {v[5] for v in PATHS.values() if v[5]}
+RHS = 4              # column 0: the single right-hand side; 1..3: the nrhs = 3 block
+
+
+@pytest.fixture(scope="module")
+def D():
+    import dhqr_b200
+    assert torch.cuda.is_available()
+    return dhqr_b200
+
+
+@contextlib.contextmanager
+def options(h, **kw):
+    """Set options on a handle for the duration of a block and put back what was there.  A profiled block drains the per-launch
+    CUDA-event brackets it left on the handle."""
+    prev = {k: h.get_option(k) for k in kw}
+    try:
+        for k, v in kw.items():
+            h.set_option(k, v)
+        yield h
+    finally:
+        for k, v in prev.items():
+            h.set_option(k, v)
+        if kw.get("profile"):
+            h.profile_reset()
+
+
+def counters(h):
+    return {k: h.get_option(k) for k in COUNTERS}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# references: one extended + one fp64 computation per (family, shape), shared by every path
+# ---------------------------------------------------------------------------------------------------------------------
+def nrm(v):
+    s = float(np.nanmax(np.abs(v))) if np.size(v) else 0.0
+    return s * float(np.linalg.norm(v / s)) if s > 0 and np.isfinite(s) else s
+
+
+def qb_sweep(h, b):
+    w = np.array(b, dtype=h.dtype, copy=True)
+    for j in range(h.shape[1] - 1, -1, -1):
+        w[j:] -= h[j:, j] * (h[j:, j] @ w[j:])
+    return w
+
+
+class Ref:
+    """Extended and fp64 results for one input.  ``k`` leading columns are compared (the leading-column identity: H[:, :k] and
+    alpha[:k] depend on A[:, :k] only); for the zero-column families k is the zero column, and the NaN pattern of the whole
+    fp64 oracle is kept for comparison."""
+
+    def __init__(self, coracle, oracle, family, m, n, k=None, cplx=False, solve=True):
+        self.family, self.m, self.n = family, m, n
+        A = F.make_complex(family, m, n) if cplx else F.make(family, m, n)
+        self.A = A
+        self.nan_cols = self.nan_alpha = None
+        if family in F.NAN_FAMILIES:
+            with np.errstate(all="ignore"):
+                H64, a64 = coracle.qr(A.copy(order="F"))
+            self.nan_cols, self.nan_alpha = np.isnan(H64).any(0), np.isnan(a64)
+            k, solve = F.zero_column(family, n), False
+        k = n if k is None else k
+        self.k, self.solve = k, solve
+        Ak = np.asfortranarray(A[:, :k])
+        self.cn = np.linalg.norm(Ak, axis=0)
+        if cplx:
+            self.b = F.rhs(m, 1, cplx=True)
+            self.He, self.ae, qtb, x = coracle.qr_ext_c(Ak, self.b)
+            self.qtb_e, self.x_e = qtb[:, 0], x[:, 0]
+            self.H64, self.a64 = oracle.np_qr_c(Ak)
+            self.qtb64 = oracle.np_apply_qt_c(self.H64, self.b)
+            self.x64 = oracle.np_ldiv_c(self.H64, self.a64, self.b)
+        elif solve:
+            self.b = F.rhs(m, RHS)
+            self.He, self.ae, self.qtb_e, self.qb_e, self.x_e = coracle.qr_ext(Ak, self.b, want_qb=True)
+            self.H64, self.a64 = coracle.qr(Ak.copy(order="F"))
+            self.qtb64 = np.stack([coracle.apply_qt(self.H64, self.b[:, r].copy()) for r in range(RHS)], 1)
+            self.qb64 = np.stack([qb_sweep(self.H64, self.b[:, r]) for r in range(RHS)], 1)
+            self.x64 = np.stack([coracle.ldiv(self.H64, self.a64, self.b[:, r].copy()) for r in range(RHS)], 1)
+        else:
+            self.He, self.ae = coracle.qr_ext(Ak)
+            self.H64, self.a64 = coracle.qr(Ak.copy(order="F"))
+        self.e64 = factor_errors(self.H64, self.a64, self)
+        del self.H64                                     # only its errors (and solves, above) are needed from here on
+
+
+@pytest.fixture(scope="session")
+def refs(oracle, coracle):
+    # the paths of one shape run back to back; 2048 x 1024 is shared by the solve and host-entry tests further down, every
+    # other shape is dropped once the next one is asked for (a shape's set is up to ~0.4 GB of host memory)
+    cache = {}
+    keep = (2048, 1024)
+
+    def get(family, m, n, k=None, cplx=False, solve=True):
+        key = (family, m, n, k, cplx, solve)
+        if key not in cache:
+            for old in [c for c in cache if c[1:3] != (m, n) and c[1:3] != keep]:
+                del cache[old]
+            cache[key] = Ref(coracle, oracle, family, m, n, k, cplx, solve)
+        return cache[key]
+    return get
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# metrics and the acceptance rule
+# ---------------------------------------------------------------------------------------------------------------------
+def factor_errors(H, alpha, ref):
+    k = ref.k
+    dH = H[:, :k] - ref.He
+    with np.errstate(all="ignore"):
+        return {"V": float(np.abs(np.tril(dH)).max()),
+                "R": float(max((np.abs(np.triu(dH[:k], 1)) / ref.cn).max(), (np.abs(alpha[:k] - ref.ae) / ref.cn).max()))}
+
+
+def orth_error(H, k):
+    v = np.tril(H[:, :k])
+    return float(np.abs((np.abs(v) ** 2).sum(0) - 2.0).max())
+
+
+def backward_error(A0, H, alpha, dev="cuda:0"):
+    """max_j ||(QR - A)[:, j]|| / ||A[:, j]||, formed on the GPU in fp64.  Columns are first scaled by a power of two near their
+    norm (exact), so 1e-150 or 1e+-120 columns neither underflow nor overflow in the residual."""
+    m, k = A0.shape
+    cn = np.linalg.norm(A0, axis=0)
+    p = np.ldexp(1.0, np.round(np.log2(np.where(cn > 0, cn, 1.0))).astype(int))
+    A = torch.from_numpy(np.ascontiguousarray(A0 / p)).to(dev)
+    Hd = torch.from_numpy(np.ascontiguousarray(H[:, :k])).to(dev)
+    al = torch.from_numpy(np.ascontiguousarray(alpha[:k]))
+    R = torch.zeros(m, k, dtype=A.dtype, device=dev)
+    R[:k] = torch.triu(Hd[:k], 1) + torch.diag(al.to(dev))
+    R /= torch.from_numpy(p).to(dev)
+    for c in range(((k - 1) // 128) * 128, -1, -128):
+        kb = min(128, k - c)
+        V = torch.tril(Hd[c:, c:c + kb])
+        Tinv = torch.eye(kb, dtype=A.dtype, device=dev) + torch.triu(V.mH @ V, 1)
+        R[c:] -= V @ torch.linalg.solve_triangular(Tinv, V.mH @ R[c:], upper=True)
+    return float(((R - A).norm(dim=0) / A.norm(dim=0)).max())
+
+
+RATIOS = {}
+
+
+@pytest.fixture(scope="module", autouse=True)
+def ratio_table():
+    yield
+    if not RATIOS:
+        return
+    paths = list(dict.fromkeys(p for p, _ in RATIOS))
+    fams = list(dict.fromkeys(f for _, f in RATIOS))
+    lines = ["# err_gpu / max(err_fp64_oracle, FLOOR), worst metric per cell (rule: <= %d)" % C_REL, "",
+             "| path | " + " | ".join(fams) + " |", "|---|" + "---|" * len(fams)]
+    tail = ["", "wide chain per factorisation: (panels it factored, restarts after a refusal)", ""] + \
+        [f"- {p} {f}: {c}" for (p, f), c in COUNTS.items()]
+    for p in paths:
+        cells = []
+        for f in fams:
+            r = RATIOS.get((p, f))
+            cells.append("" if r is None else f"{r[0]:.2g} {r[1]}")
+        lines.append(f"| {p} | " + " | ".join(cells) + " |")
+    try:
+        out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build")
+        os.makedirs(out, exist_ok=True)
+        with open(os.path.join(out, "test_gpu_ext_ratios.md"), "w") as fh:
+            fh.write("\n".join(lines + tail) + "\n")
+    except OSError:
+        pass
+
+
+def check(path, ref, gpu, e64, absolute=None, note=""):
+    """The relative rule on every metric in ``gpu`` (err_gpu <= C_REL max(err_fp64, FLOOR)) and the absolute bounds."""
+    floor = {key: FLOOR_EPS * EPS * SIZE[key](ref.m) for key in gpu}
+    worst = max(((gpu[key] / max(e64[key], floor[key]), key) for key in gpu), key=lambda t: (np.nan_to_num(t[0], nan=np.inf), t[1]))
+    RATIOS[(path, ref.family)] = worst
+    where = f"path {path}, family {ref.family}, {ref.m}x{ref.n}; {note}"
+    for key in gpu:
+        assert gpu[key] <= C_REL * max(e64[key], floor[key]), \
+            f"{key}: err_gpu {gpu[key]:.3e} > {C_REL} x max(err_fp64 {e64[key]:.3e}, floor {floor[key]:.1e}); {where}"
+    for key, (val, tol) in (absolute or {}).items():
+        assert val < tol, f"{key} = {val:.3e} >= {tol:.0e}; {where}"
+
+
+def run_qr(D, A0, nb=0, lda_extra=0, **opts):
+    h = D.default_handle(0)
+    m, n = A0.shape
+    with options(h, **opts):
+        c0 = counters(h)
+        dA = D.colmajor_empty(m, n, "cuda:0", lda=m + lda_extra, dtype=torch.from_numpy(A0[:1, :1]).dtype)
+        dA.copy_(torch.from_numpy(A0))
+        st = D.qr_(dA, nb=nb)
+        torch.cuda.synchronize()
+        c1 = counters(h)
+    note = "counters " + ", ".join(f"{k} {c0[k]}->{c1[k]}" for k in COUNTERS)
+    return dA, st, note, {k: c1[k] - c0[k] for k in COUNTERS}
+
+
+COUNTS = {}
+ACCEPTED = ("uniform", "centered", "normal", "graded2")
+
+
+def check_regime(path, ref, delta, note):
+    """The wide chain's decisions: well-conditioned panels are all taken by it, a kappa = 1e12 spectrum at 4099 x 640 gets both
+    verdicts, a zero column is refused and the factorisation restarts from that panel (the panels before it stay accepted)."""
+    if path not in ("default", "lda+3"):
+        return
+    COUNTS[(path, ref.family)] = (delta["wide_panels"], delta["wide_redone"])
+    where = f"path {path}, family {ref.family}, {ref.m}x{ref.n}; {note}"
+    if ref.family in ACCEPTED:
+        assert delta["wide_panels"] == ref.n // 128 and delta["wide_redone"] == 0, f"every panel should be accepted; {where}"
+    if (path, ref.family) == ("lda+3", "graded12"):     # kappa = 1e12 at 4099 x 640 straddles the guard: both verdicts occur
+        assert 1 <= delta["wide_redone"] < delta["wide_panels"], f"some panels accepted, some refused and redone; {where}"
+    if ref.family == "zerocol_wide":
+        assert delta["wide_redone"] >= 1 and delta["wide_panels"] >= F.zero_column(ref.family, ref.n) // 128, \
+            f"the panel with the zero column should be refused and redone; {where}"
+
+
+def check_nan_pattern(path, ref, H, alpha, note):
+    where = f"path {path}, family {ref.family}, {ref.m}x{ref.n}; {note}"
+    assert np.array_equal(np.isnan(H).any(0), ref.nan_cols), f"NaN columns differ from the fp64 oracle's; {where}"
+    assert np.array_equal(np.isnan(alpha), ref.nan_alpha), f"NaN entries of alpha differ from the fp64 oracle's; {where}"
+    assert np.isfinite(H[:, :ref.k]).all() and np.isfinite(alpha[:ref.k]).all(), where
+
+
+def factor_checks(path, ref, H, alpha, note):
+    if ref.nan_cols is not None:
+        check_nan_pattern(path, ref, H, alpha, note)
+    k = ref.k
+    gpu = factor_errors(H, alpha, ref)
+    absolute = {"bwd": (backward_error(np.asfortranarray(ref.A[:, :k]), H, alpha), TOL_BWD), "orth": (orth_error(H, k), TOL_ORTH)}
+    return gpu, absolute
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the path matrix
+# ---------------------------------------------------------------------------------------------------------------------
+_bitwise = {}
+
+
+def digest(H, alpha):
+    return hashlib.sha256(np.ascontiguousarray(H).tobytes() + np.ascontiguousarray(alpha).tobytes()).hexdigest()
+
+
+@pytest.mark.parametrize("family", F.FAMILIES)
+@pytest.mark.parametrize("path", list(PATHS))
+def test_path(D, refs, path, family):
+    m, n, nb, extra, opts, same_as = PATHS[path]
+    ref = refs(family, m, n)
+    dA, st, note, delta = run_qr(D, ref.A, nb, extra, **opts)
+    check_regime(path, ref, delta, note)
+    H, alpha = dA.cpu().numpy(), st.α.cpu().numpy()
+    gpu, absolute = factor_checks(path, ref, H, alpha, note)
+    e64 = dict(ref.e64)
+    if ref.solve:
+        b = torch.from_numpy(ref.b[:, 0].copy()).cuda()
+        qtb = D.apply_qt_(b.clone(), dA).cpu().numpy()
+        x = D.ldiv(st, b).cpu().numpy()
+        gpu["qtb"] = nrm(qtb - ref.qtb_e[:, 0]) / nrm(ref.b[:, 0])
+        gpu["x"] = nrm(x - ref.x_e[:, 0]) / nrm(ref.x_e[:, 0])
+        e64["qtb"] = nrm(ref.qtb64[:, 0] - ref.qtb_e[:, 0]) / nrm(ref.b[:, 0])
+        e64["x"] = nrm(ref.x64[:, 0] - ref.x_e[:, 0]) / nrm(ref.x_e[:, 0])
+    check(path, ref, gpu, e64, absolute, note)
+    if path in BITWISE_TARGETS:
+        _bitwise[(path, family)] = digest(H, alpha)
+    if same_as:
+        if (same_as, family) not in _bitwise:
+            _, _, nb2, extra2, opts2, _ = PATHS[same_as]
+            dB, st2, _, _ = run_qr(D, ref.A, nb2, extra2, **opts2)
+            _bitwise[(same_as, family)] = digest(dB.cpu().numpy(), st2.α.cpu().numpy())
+        assert digest(H, alpha) == _bitwise[(same_as, family)], \
+            f"path {path} is not bitwise equal to path {same_as} on family {family}; {note}"
+
+
+@pytest.mark.parametrize("family", [f for f in F.FAMILIES if f not in F.NAN_FAMILIES])
+def test_solve_paths(D, refs, family):
+    # Q'b with the GEMV-shaped sweep (qt_vec = 1) and the block update (0); Qb; back-substitution as one wavefront
+    # (bs_wave = 1) and as k_backsolve_step blocks (0); three right-hand sides with ldb > m
+    m, n = 2048, 1024
+    ref = refs(family, m, n)
+    dA, st, note, _ = run_qr(D, ref.A)
+    h = D.default_handle(0)
+    b = torch.from_numpy(ref.b[:, 0].copy()).cuda()
+    nb_ = nrm(ref.b[:, 0])
+    e_qtb64 = nrm(ref.qtb64[:, 0] - ref.qtb_e[:, 0]) / nb_
+    e_x64 = nrm(ref.x64[:, 0] - ref.x_e[:, 0]) / nrm(ref.x_e[:, 0])
+    for qv in (1, 0):
+        with options(h, qt_vec=qv):
+            qtb = D.apply_qt_(b.clone(), dA).cpu().numpy()
+        check(f"apply_qt qt_vec={qv}", ref, {"qtb": nrm(qtb - ref.qtb_e[:, 0]) / nb_}, {"qtb": e_qtb64}, note=note)
+    qb = D.apply_q_(b.clone(), dA).cpu().numpy()
+    check("apply_q", ref, {"qb": nrm(qb - ref.qb_e[:, 0]) / nb_}, {"qb": nrm(ref.qb64[:, 0] - ref.qb_e[:, 0]) / nb_}, note=note)
+    for bw in (1, 0):
+        with options(h, bs_wave=bw):
+            x = D.ldiv(st, b).cpu().numpy()
+        check(f"ldiv bs_wave={bw}", ref, {"x": nrm(x - ref.x_e[:, 0]) / nrm(ref.x_e[:, 0])}, {"x": e_x64}, note=note)
+    B = D.colmajor_empty(m, 3, "cuda:0", lda=m + 5)
+    B.copy_(torch.from_numpy(ref.b[:, 1:]))
+    Q = D.colmajor_empty(m, 3, "cuda:0", lda=m + 5)
+    Q.copy_(B)
+    D.apply_qt_(Q, dA)
+    X = D.solve_householder_(B, dA, st.α).cpu().numpy()
+    Q = Q.cpu().numpy()
+    for r in range(1, RHS):
+        nbr = nrm(ref.b[:, r])
+        gpu = {"qtb": nrm(Q[:, r - 1] - ref.qtb_e[:, r]) / nbr, "x": nrm(X[:, r - 1] - ref.x_e[:, r]) / nrm(ref.x_e[:, r])}
+        e64 = {"qtb": nrm(ref.qtb64[:, r] - ref.qtb_e[:, r]) / nbr, "x": nrm(ref.x64[:, r] - ref.x_e[:, r]) / nrm(ref.x_e[:, r])}
+        check(f"nrhs=3 ldb=m+5 (rhs {r})", ref, gpu, e64, note=note)
+
+
+@pytest.mark.parametrize("family", [f"graded{k}" for k in F.GRADED] + ["colscale"])
+def test_host_entry(D, refs, family):
+    # dhqr_qr_host_f64: upload in 128-column chunks that join the look-ahead schedule late, then dhqr_ldiv_host_f64
+    m, n = 2048, 1024
+    ref = refs(family, m, n)
+    h = D.default_handle(0)
+    A = ref.A.copy(order="F")
+    with options(h, host_chunk=128):
+        c0 = counters(h)
+        st = D.qr_(A)
+        c1 = counters(h)
+    note = "counters " + ", ".join(f"{k} {c0[k]}->{c1[k]}" for k in COUNTERS)
+    gpu, absolute = factor_checks("host host_chunk=128", ref, A, st.α, note)
+    x = D.ldiv(st, ref.b[:, 0].copy())
+    gpu["x"] = nrm(x - ref.x_e[:, 0]) / nrm(ref.x_e[:, 0])
+    e64 = dict(ref.e64, x=nrm(ref.x64[:, 0] - ref.x_e[:, 0]) / nrm(ref.x_e[:, 0]))
+    check("host host_chunk=128", ref, gpu, e64, absolute, note)
+
+
+@pytest.mark.parametrize("family", F.COMPLEX_FAMILIES)
+def test_complex(D, refs, family):
+    m, n = 1024, 384
+    ref = refs(family, m, n, cplx=True)
+    dA, st, note, _ = run_qr(D, ref.A)
+    H, alpha = dA.cpu().numpy(), st.α.cpu().numpy()
+    gpu, absolute = factor_checks("complex", ref, H, alpha, note)
+    b = torch.from_numpy(ref.b.copy()).cuda()
+    x = D.ldiv(st, b).cpu().numpy()
+    gpu["qtb"] = nrm(D.apply_qt_(b.clone(), dA).cpu().numpy() - ref.qtb_e) / nrm(ref.b)
+    gpu["x"] = nrm(x - ref.x_e) / nrm(ref.x_e)
+    e64 = dict(ref.e64, qtb=nrm(ref.qtb64 - ref.qtb_e) / nrm(ref.b), x=nrm(ref.x64 - ref.x_e) / nrm(ref.x_e))
+    check("complex", ref, gpu, e64, absolute, note)
+
+
+LARGE_FAMILIES = ("uniform", "centered", "colscale", "rowscale")
+
+
+@pytest.mark.parametrize("family", LARGE_FAMILIES)
+@pytest.mark.parametrize("shape", [(32768, 4096, 0), (32768, 256, 1)], ids=["32768x4096", "32768x256-nb1"])
+def test_large_shapes_leading_columns(D, oracle, coracle, shape, family):
+    # BASELINE config 3 on the default path (its first 256 columns) and the nb = 1 direct-kernel path (all of H); not cached
+    m, n, nb = shape
+    ref = Ref(coracle, oracle, family, m, n, k=256, solve=False)
+    dA, st, note, _ = run_qr(D, ref.A, nb)
+    H, alpha = dA[:, :256].cpu().numpy(), st.α[:256].cpu().numpy()
+    gpu, absolute = factor_checks(f"{m}x{n} nb={nb}", ref, H, alpha, note)
+    check(f"{m}x{n} nb={nb}", ref, gpu, ref.e64, absolute, note)
+
+
+def test_row_limit(D, oracle, coracle):
+    # the resident 32-column panel kernel holds 728 rows per CTA on at most 160 CTAs: m = 728 min(SMs, 160) is the tallest
+    # matrix the blocked paths take (96 096 on a 132-SM H100 SXM); one row more is refused with -2 before anything runs
+    h = D.default_handle(0)
+    lim = 728 * min(h.get_option("sms"), 160)
+    ref = Ref(coracle, oracle, "normal", lim, 256, k=128, solve=False)
+    dA, st, note, _ = run_qr(D, ref.A)
+    H, alpha = dA[:, :128].cpu().numpy(), st.α[:128].cpu().numpy()
+    gpu, absolute = factor_checks("row limit", ref, H, alpha, note)
+    check(f"row limit m={lim}", ref, gpu, ref.e64, absolute, note)
+    A1 = F.make("normal", lim + 1, 256)
+    dB = D.to_colmajor(A1, "cuda:0")
+    with pytest.raises(D._lib.DhqrError) as e:
+        D.qr_(dB)
+    assert e.value.code == -2
+    torch.cuda.synchronize()
+    assert np.array_equal(dB.cpu().numpy(), A1)

@@ -174,3 +174,83 @@ def test_complex_alphafactor_and_partialdot(oracle):
     b = _complex_matrix(oracle, 2, 50, 1)[:, 0]
     for i0 in (0, 7, 49):                                                        # every suffix, test/partialdot.jl:11-22
         assert abs(oracle.np_partialdot_c(a, b, i0, 50) - np.sum(np.conj(a[i0:]) * b[i0:])) < 1e-13
+
+
+# ---- extended-precision reference (the same recurrences in long double) -----------------------------------------------
+def test_ext_has_extended_significand(coracle):
+    # 64 bits on x86-64 (x87 extended), 113 on aarch64 (software quad): either is far enough beyond double's 53
+    assert coracle.ext_mant_dig() >= 64
+
+
+@pytest.mark.parametrize("mn", [(110, 100), (1024, 128), (513, 200)])
+def test_ext_storage_format_equals_lapack(mn, oracle, coracle):
+    m, n = mn
+    A = coracle.fill_uniform(2, m, n)
+    He, ae = coracle.qr_ext(A)
+    Hl, al = oracle.lapack_qr_refformat(A)
+    assert np.abs(He - Hl).max() < 1e-12 and np.abs(ae - al).max() < 1e-12
+    b = oracle.np_uniform(3, m, 1)[:, 0].copy()
+    _, _, qtb, qb, x = coracle.qr_ext(A, b, want_qb=True)
+    assert np.abs(x[:, 0] - oracle.lapack_lstsq(A, b)).max() < 1e-9 * np.abs(x).max()
+    assert np.abs(qtb[:, 0] - coracle.apply_qt(coracle.qr(A.copy(order="F"))[0], b)).max() < 1e-13 * np.sqrt(m)
+    # Qb applies the same reflectors in reverse order: Q(Q'b) = b
+    w = qtb[:, 0].copy()
+    for j in range(n - 1, -1, -1):
+        w[j:] -= He[j:, j] * (He[j:, j] @ w[j:])
+    assert np.abs(w - b).max() < 1e-13 * np.sqrt(m)
+    assert np.abs(np.linalg.norm(qb[:, 0]) - np.linalg.norm(b)) < 1e-13 * np.linalg.norm(b)
+
+
+def test_ext_is_independent_of_thread_count(coracle):
+    A = coracle.fill_uniform(6, 300, 97)
+    b = np.asfortranarray(coracle.fill_uniform(7, 300, 2))
+    r1 = coracle.qr_ext(A, b, nthreads=1, want_qb=True)
+    r5 = coracle.qr_ext(A, b, nthreads=5, want_qb=True)
+    for u, v in zip(r1, r5):
+        assert np.array_equal(u, v)
+    c1 = coracle.qr_ext_c(A + 1j * A[::-1], b[:, 0] + 0j, nthreads=1)
+    c3 = coracle.qr_ext_c(A + 1j * A[::-1], b[:, 0] + 0j, nthreads=3)
+    for u, v in zip(c1, c3):
+        assert np.array_equal(u, v)
+
+
+def test_ext_mirrors_zero_column_and_zero_pivot(oracle, coracle):
+    # the same recurrences, so the same divergences: a zero column gives NaN from that column on (S:131), an exactly zero
+    # pivot gives alpha = 0 (S:8)
+    Z = coracle.fill_uniform(8, 40, 6)
+    Z[:, 2] = 0.0
+    with np.errstate(all="ignore"):
+        H, a = coracle.qr(Z.copy(order="F"))
+        He, ae = coracle.qr_ext(Z)
+    assert np.array_equal(np.isnan(He), np.isnan(H)) and np.array_equal(np.isnan(ae), np.isnan(a))
+    assert np.isnan(He[2:, 2]).all() and np.isfinite(He[:, :2]).all()
+    P = coracle.fill_uniform(9, 40, 6)
+    P[0, 0] = 0.0
+    assert coracle.qr_ext(P)[1][0] == 0.0
+
+
+@pytest.mark.parametrize("family,h_err,a_err", [("uniform", 2.5e-14, 1.6e-16), ("normal", 1.3e-14, 3.5e-16),
+                                                ("graded6", 5.4e-12, 2.6e-12), ("graded12", 3.5e-6, 1.2e-6)])
+def test_fp64_oracle_forward_error_against_ext(family, h_err, a_err, oracle, coracle):
+    # pins the yardstick: at 2048 x 512 the fp64 oracle sits where kappa * eps puts it, and the extended reference is far
+    # enough beyond it to measure that (a lower bound too: an "extended" reference that rounded like double would give 0)
+    import matrix_families as F
+    A = F.make(family, 2048, 512, 0)
+    He, ae = coracle.qr_ext(A)
+    H, a = coracle.qr(A.copy(order="F"))
+    eh = np.abs(H - He).max()
+    ea = (np.abs(a - ae) / np.abs(ae)).max()
+    assert h_err / 8 < eh < h_err * 8, eh
+    assert a_err / 8 < ea < a_err * 8, ea
+
+
+def test_ext_complex_matches_numpy_twin_and_lstsq(oracle, coracle):
+    A = _complex_matrix(oracle, 13, 300, 37)
+    b = _complex_matrix(oracle, 14, 300, 1)[:, 0]
+    He, ae, qtb, x = coracle.qr_ext_c(A, b)
+    Hn, an = oracle.np_qr_c(A)
+    assert np.abs(He - Hn).max() < 1e-13 and np.abs(ae - an).max() < 1e-13 * np.abs(an).max()
+    assert np.abs(qtb[:, 0] - oracle.np_apply_qt_c(Hn, b)).max() < 1e-13 * np.sqrt(300)
+    xl = np.linalg.lstsq(A, b, rcond=None)[0]
+    assert np.abs(x[:, 0] - xl).max() < 1e-12 * np.abs(xl).max()
+    assert np.array_equal(coracle.ldiv_ext_c(A, b), x[:, 0])
