@@ -60,6 +60,14 @@ def zero_rows(m: int, n: int) -> int:
     return max(1, (m - n) // 2) | 1
 
 
+def singular(family: str, m: int, n: int) -> bool:
+    """True where the family is rank deficient by construction at this shape (no solution to compare): zerorows once its
+    zero block leaves fewer than n non-zero rows (m = n, for one), and the zero-column families."""
+    if family == "zerorows":
+        return m - zero_rows(m, n) < n
+    return family in NAN_FAMILIES
+
+
 def make(family: str, m: int, n: int, seed: int = 0) -> np.ndarray:
     assert m >= n >= 1
     rng = _rng(family, m, n, seed)

@@ -17,32 +17,17 @@ range:
     orth  max_j | ||v_j||^2 - 2 | < 1e-13
 Where a variant runs the same floating-point operations in the same order as another path, the two must agree bit for bit.
 
-A table of err_gpu / max(err_fp64_oracle, FLOOR) per path x family is written to build/test_gpu_ext_ratios.md.
+A table of err_gpu / max(err_fp64_oracle, FLOOR) per path x family is written to build/test_gpu_ext_ratios.md.  The rule, its
+constants and the references live in tests/ext_rule.py, shared with test_gpu_shapes.py.
 """
-import contextlib
-import hashlib
-import os
-
 import numpy as np
 import pytest
 import torch
 
 import matrix_families as F
+from ext_rule import COUNTERS, RHS, Ref, Table, counters, digest, factor_checks, nrm, options, run_qr
 
 pytestmark = pytest.mark.gpu
-
-EPS = np.finfo(np.float64).eps
-C_REL = 8            # headroom over the fp64 oracle: the blocked paths sum in other orders (split-K, CholeskyQR2 + reconstruction)
-# Where the floor decides, the margin is thinnest: on triangular input the oracle's reflectors are +-sqrt(2) e_j to an ulp, while
-# the blocked update still rounds every R entry once per 128-column panel to its left and in its split-K sums.  Measured on an
-# H100 SXM (132 SMs): R error 98 eps (ratio 6.1) at 4099 x 640, 1.5 at 2048 x 1024; every non-triangular cell <= 1.5.  Split
-# counts follow the SM count, so a part with other SMs moves this cell first; a ratio near 8 there is summation order, not a bug.
-FLOOR_EPS = 16       # FLOOR = 16 eps x size factor: for inputs where the fp64 oracle happens to be (nearly) exact, e.g. triangular
-SIZE = {"V": lambda m: 1.0, "R": lambda m: 1.0,            # one rounded result of a stable recurrence per entry: the oracle lands at 1-4 eps
-        "qtb": np.sqrt, "qb": np.sqrt, "x": np.sqrt}        # a sweep over m rows: rounding errors add up like a random walk
-TOL_BWD = 1e-13      # column-wise backward error: Householder QR is column-wise backward stable whatever kappa is
-TOL_ORTH = 1e-13     # |v_j|^2 = 2 exactly in exact arithmetic (S:131-135)
-COUNTERS = ("wide_panels", "wide_redone", "panels_fast", "panels_fallback")
 
 # path -> (m, n, nb, extra rows of lda, options, path whose output it must equal bit for bit)
 PATHS = {
@@ -89,7 +74,6 @@ PATHS = {
     "nb1_lda+3": (4096, 512, 1, 3, {}, None),
 }
 BITWISE_TARGETS = {v[5] for v in PATHS.values() if v[5]}
-RHS = 4              # column 0: the single right-hand side; 1..3: the nrhs = 3 block
 
 
 @pytest.fixture(scope="module")
@@ -97,81 +81,6 @@ def D():
     import dhqr_b200
     assert torch.cuda.is_available()
     return dhqr_b200
-
-
-@contextlib.contextmanager
-def options(h, **kw):
-    """Set options on a handle for the duration of a block and put back what was there.  A profiled block drains the per-launch
-    CUDA-event brackets it left on the handle."""
-    prev = {k: h.get_option(k) for k in kw}
-    try:
-        for k, v in kw.items():
-            h.set_option(k, v)
-        yield h
-    finally:
-        for k, v in prev.items():
-            h.set_option(k, v)
-        if kw.get("profile"):
-            h.profile_reset()
-
-
-def counters(h):
-    return {k: h.get_option(k) for k in COUNTERS}
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# references: one extended + one fp64 computation per (family, shape), shared by every path
-# ---------------------------------------------------------------------------------------------------------------------
-def nrm(v):
-    s = float(np.nanmax(np.abs(v))) if np.size(v) else 0.0
-    return s * float(np.linalg.norm(v / s)) if s > 0 and np.isfinite(s) else s
-
-
-def qb_sweep(h, b):
-    w = np.array(b, dtype=h.dtype, copy=True)
-    for j in range(h.shape[1] - 1, -1, -1):
-        w[j:] -= h[j:, j] * (h[j:, j] @ w[j:])
-    return w
-
-
-class Ref:
-    """Extended and fp64 results for one input.  ``k`` leading columns are compared (the leading-column identity: H[:, :k] and
-    alpha[:k] depend on A[:, :k] only); for the zero-column families k is the zero column, and the NaN pattern of the whole
-    fp64 oracle is kept for comparison."""
-
-    def __init__(self, coracle, oracle, family, m, n, k=None, cplx=False, solve=True):
-        self.family, self.m, self.n = family, m, n
-        A = F.make_complex(family, m, n) if cplx else F.make(family, m, n)
-        self.A = A
-        self.nan_cols = self.nan_alpha = None
-        if family in F.NAN_FAMILIES:
-            with np.errstate(all="ignore"):
-                H64, a64 = coracle.qr(A.copy(order="F"))
-            self.nan_cols, self.nan_alpha = np.isnan(H64).any(0), np.isnan(a64)
-            k, solve = F.zero_column(family, n), False
-        k = n if k is None else k
-        self.k, self.solve = k, solve
-        Ak = np.asfortranarray(A[:, :k])
-        self.cn = np.linalg.norm(Ak, axis=0)
-        if cplx:
-            self.b = F.rhs(m, 1, cplx=True)
-            self.He, self.ae, qtb, x = coracle.qr_ext_c(Ak, self.b)
-            self.qtb_e, self.x_e = qtb[:, 0], x[:, 0]
-            self.H64, self.a64 = oracle.np_qr_c(Ak)
-            self.qtb64 = oracle.np_apply_qt_c(self.H64, self.b)
-            self.x64 = oracle.np_ldiv_c(self.H64, self.a64, self.b)
-        elif solve:
-            self.b = F.rhs(m, RHS)
-            self.He, self.ae, self.qtb_e, self.qb_e, self.x_e = coracle.qr_ext(Ak, self.b, want_qb=True)
-            self.H64, self.a64 = coracle.qr(Ak.copy(order="F"))
-            self.qtb64 = np.stack([coracle.apply_qt(self.H64, self.b[:, r].copy()) for r in range(RHS)], 1)
-            self.qb64 = np.stack([qb_sweep(self.H64, self.b[:, r]) for r in range(RHS)], 1)
-            self.x64 = np.stack([coracle.ldiv(self.H64, self.a64, self.b[:, r].copy()) for r in range(RHS)], 1)
-        else:
-            self.He, self.ae = coracle.qr_ext(Ak)
-            self.H64, self.a64 = coracle.qr(Ak.copy(order="F"))
-        self.e64 = factor_errors(self.H64, self.a64, self)
-        del self.H64                                     # only its errors (and solves, above) are needed from here on
 
 
 @pytest.fixture(scope="session")
@@ -191,99 +100,17 @@ def refs(oracle, coracle):
     return get
 
 
-# ---------------------------------------------------------------------------------------------------------------------
-# metrics and the acceptance rule
-# ---------------------------------------------------------------------------------------------------------------------
-def factor_errors(H, alpha, ref):
-    k = ref.k
-    dH = H[:, :k] - ref.He
-    with np.errstate(all="ignore"):
-        return {"V": float(np.abs(np.tril(dH)).max()),
-                "R": float(max((np.abs(np.triu(dH[:k], 1)) / ref.cn).max(), (np.abs(alpha[:k] - ref.ae) / ref.cn).max()))}
-
-
-def orth_error(H, k):
-    v = np.tril(H[:, :k])
-    return float(np.abs((np.abs(v) ** 2).sum(0) - 2.0).max())
-
-
-def backward_error(A0, H, alpha, dev="cuda:0"):
-    """max_j ||(QR - A)[:, j]|| / ||A[:, j]||, formed on the GPU in fp64.  Columns are first scaled by a power of two near their
-    norm (exact), so 1e-150 or 1e+-120 columns neither underflow nor overflow in the residual."""
-    m, k = A0.shape
-    cn = np.linalg.norm(A0, axis=0)
-    p = np.ldexp(1.0, np.round(np.log2(np.where(cn > 0, cn, 1.0))).astype(int))
-    A = torch.from_numpy(np.ascontiguousarray(A0 / p)).to(dev)
-    Hd = torch.from_numpy(np.ascontiguousarray(H[:, :k])).to(dev)
-    al = torch.from_numpy(np.ascontiguousarray(alpha[:k]))
-    R = torch.zeros(m, k, dtype=A.dtype, device=dev)
-    R[:k] = torch.triu(Hd[:k], 1) + torch.diag(al.to(dev))
-    R /= torch.from_numpy(p).to(dev)
-    for c in range(((k - 1) // 128) * 128, -1, -128):
-        kb = min(128, k - c)
-        V = torch.tril(Hd[c:, c:c + kb])
-        Tinv = torch.eye(kb, dtype=A.dtype, device=dev) + torch.triu(V.mH @ V, 1)
-        R[c:] -= V @ torch.linalg.solve_triangular(Tinv, V.mH @ R[c:], upper=True)
-    return float(((R - A).norm(dim=0) / A.norm(dim=0)).max())
-
-
-RATIOS = {}
+TABLE = Table("test_gpu_ext_ratios.md")
+check = TABLE.check
+COUNTS = TABLE.counts
 
 
 @pytest.fixture(scope="module", autouse=True)
 def ratio_table():
     yield
-    if not RATIOS:
-        return
-    paths = list(dict.fromkeys(p for p, _ in RATIOS))
-    fams = list(dict.fromkeys(f for _, f in RATIOS))
-    lines = ["# err_gpu / max(err_fp64_oracle, FLOOR), worst metric per cell (rule: <= %d)" % C_REL, "",
-             "| path | " + " | ".join(fams) + " |", "|---|" + "---|" * len(fams)]
-    tail = ["", "wide chain per factorisation: (panels it factored, restarts after a refusal)", ""] + \
-        [f"- {p} {f}: {c}" for (p, f), c in COUNTS.items()]
-    for p in paths:
-        cells = []
-        for f in fams:
-            r = RATIOS.get((p, f))
-            cells.append("" if r is None else f"{r[0]:.2g} {r[1]}")
-        lines.append(f"| {p} | " + " | ".join(cells) + " |")
-    try:
-        out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build")
-        os.makedirs(out, exist_ok=True)
-        with open(os.path.join(out, "test_gpu_ext_ratios.md"), "w") as fh:
-            fh.write("\n".join(lines + tail) + "\n")
-    except OSError:
-        pass
+    TABLE.write()
 
 
-def check(path, ref, gpu, e64, absolute=None, note=""):
-    """The relative rule on every metric in ``gpu`` (err_gpu <= C_REL max(err_fp64, FLOOR)) and the absolute bounds."""
-    floor = {key: FLOOR_EPS * EPS * SIZE[key](ref.m) for key in gpu}
-    worst = max(((gpu[key] / max(e64[key], floor[key]), key) for key in gpu), key=lambda t: (np.nan_to_num(t[0], nan=np.inf), t[1]))
-    RATIOS[(path, ref.family)] = worst
-    where = f"path {path}, family {ref.family}, {ref.m}x{ref.n}; {note}"
-    for key in gpu:
-        assert gpu[key] <= C_REL * max(e64[key], floor[key]), \
-            f"{key}: err_gpu {gpu[key]:.3e} > {C_REL} x max(err_fp64 {e64[key]:.3e}, floor {floor[key]:.1e}); {where}"
-    for key, (val, tol) in (absolute or {}).items():
-        assert val < tol, f"{key} = {val:.3e} >= {tol:.0e}; {where}"
-
-
-def run_qr(D, A0, nb=0, lda_extra=0, **opts):
-    h = D.default_handle(0)
-    m, n = A0.shape
-    with options(h, **opts):
-        c0 = counters(h)
-        dA = D.colmajor_empty(m, n, "cuda:0", lda=m + lda_extra, dtype=torch.from_numpy(A0[:1, :1]).dtype)
-        dA.copy_(torch.from_numpy(A0))
-        st = D.qr_(dA, nb=nb)
-        torch.cuda.synchronize()
-        c1 = counters(h)
-    note = "counters " + ", ".join(f"{k} {c0[k]}->{c1[k]}" for k in COUNTERS)
-    return dA, st, note, {k: c1[k] - c0[k] for k in COUNTERS}
-
-
-COUNTS = {}
 ACCEPTED = ("uniform", "centered", "normal", "graded2")
 
 
@@ -303,30 +130,10 @@ def check_regime(path, ref, delta, note):
             f"the panel with the zero column should be refused and redone; {where}"
 
 
-def check_nan_pattern(path, ref, H, alpha, note):
-    where = f"path {path}, family {ref.family}, {ref.m}x{ref.n}; {note}"
-    assert np.array_equal(np.isnan(H).any(0), ref.nan_cols), f"NaN columns differ from the fp64 oracle's; {where}"
-    assert np.array_equal(np.isnan(alpha), ref.nan_alpha), f"NaN entries of alpha differ from the fp64 oracle's; {where}"
-    assert np.isfinite(H[:, :ref.k]).all() and np.isfinite(alpha[:ref.k]).all(), where
-
-
-def factor_checks(path, ref, H, alpha, note):
-    if ref.nan_cols is not None:
-        check_nan_pattern(path, ref, H, alpha, note)
-    k = ref.k
-    gpu = factor_errors(H, alpha, ref)
-    absolute = {"bwd": (backward_error(np.asfortranarray(ref.A[:, :k]), H, alpha), TOL_BWD), "orth": (orth_error(H, k), TOL_ORTH)}
-    return gpu, absolute
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # the path matrix
 # ---------------------------------------------------------------------------------------------------------------------
 _bitwise = {}
-
-
-def digest(H, alpha):
-    return hashlib.sha256(np.ascontiguousarray(H).tobytes() + np.ascontiguousarray(alpha).tobytes()).hexdigest()
 
 
 @pytest.mark.parametrize("family", F.FAMILIES)
