@@ -145,8 +145,8 @@ struct dhqr_context {
     int unblocked_wave = 1;                                             // nb = 1, m <= 8192: the column loop as one persistent launch
     unsigned int* uw_flags = nullptr; size_t uw_flags_n = 0; unsigned int uw_epoch = 0;
     int fuse_house = 1;                                                 // nb = 1: next reflector formed inside the apply kernel (one launch per column)
-    int cvy_persist = 4;                                                // 128-wide gemm_cvy: consecutive tiles per CTA (0: one-tile kernel); 4 is fastest on an H100 at one CTA per SM
-    int cvy_defer = 1;                                                  // 128-wide gemm_cvy: C tile read in batches behind the k-stages
+    int cvy_persist = 4;                                                // 128-wide gemm_cvy: consecutive tiles per CTA (0: one tile per CTA); 4 is fastest on an H100 at one CTA per SM
+    int cvy_defer = 1;                                                  // read only when cvy_persist = 0; 0 runs the 128-wide update by k_gemm_cvy (accumulators start at C)
     int cvy_warps = 8;                                                  // MMA warps per gemm_cvy CTA (4: 64x32 warp tiles, 8: 32x32)
     int tail_cols = 0;                                                  // trailing width below which the chain is considered critical
     int wide_panel_ctas = 64;                                           // panel CTAs while the bulk update is wide
@@ -216,9 +216,8 @@ static size_t smem_ymake(int nbp) { return ((size_t)nbp * nbp + YCOLS * nbp) * 8
 
 #define K_G1_128 k_gemm_vta<128, G1_BN, 4, 2, G1_NPW>
 #define K_G1_32 k_gemm_vta<32, G1S_BN, 1, 4, G1S_NPW>
-#define K_G2 k_gemm_cvy<2, 2, false>
-#define K_G2W k_gemm_cvy<4, 2, false>
-#define K_G2D k_gemm_cvy<4, 2, true>
+#define K_G2 k_gemm_cvy<2, 2>
+#define K_G2W k_gemm_cvy<4, 2>
 
 static int set_attrs(dhqr_context* c) {
     if (c->attrs_set) return 0;
@@ -228,8 +227,6 @@ static int set_attrs(dhqr_context* c) {
     CU(cudaFuncSetAttribute(K_G2, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(K_G2W, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2()));
     CU(cudaFuncSetAttribute(K_G2W, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    CU(cudaFuncSetAttribute(K_G2D, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2()));
-    CU(cudaFuncSetAttribute(K_G2D, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2()));
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(k_gram_sym, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_GRAM_SYM));
@@ -432,10 +429,9 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     g2.ctl = c->wctl; g2.gate = gate;
     dim3 grid2((unsigned)((rows + G2_BM - 1) / G2_BM), (unsigned)((ncols + G2_BN - 1) / G2_BN));
     g2.tiles_m = (int)grid2.x; g2.tiles_n = (int)grid2.y;
-    g2.tiles_per_cta = c->cvy_persist;
-    if (c->cvy_warps == 8 && g2.nkq == 4 && c->cvy_persist > 0)
-        k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + c->cvy_persist - 1) / c->cvy_persist, 9 * 32, smem_g2(), st>>>(g2);
-    else if (c->cvy_warps == 8 && g2.nkq == 4 && c->cvy_defer) K_G2D<<<grid2, 9 * 32, smem_g2(), st>>>(g2);
+    g2.tiles_per_cta = std::max(c->cvy_persist, 1);   // cvy_persist = 0: one tile per CTA
+    if (c->cvy_warps == 8 && g2.nkq == 4 && (c->cvy_persist > 0 || c->cvy_defer))
+        k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, 9 * 32, smem_g2(), st>>>(g2);
     else if (c->cvy_warps == 8) K_G2W<<<grid2, 9 * 32, smem_g2(), st>>>(g2);
     else K_G2<<<grid2, 5 * 32, smem_g2(), st>>>(g2);
     TRY(post(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols));
