@@ -246,14 +246,16 @@ static int set_attrs(dhqr_context* c) {
     return 0;
 }
 
+// Grows a workspace buffer.  The zero fill goes on `st`, the stream of the call that needs the buffer: a synchronous
+// cudaMemset would run on the legacy default stream, which a non-blocking caller stream is not ordered after.
 template <typename T>
-static int ensure(T** p, size_t* have, size_t need) {
+static int ensure(T** p, size_t* have, size_t need, cudaStream_t st) {
     if (*have >= need && *p) return 0;
     if (*p) CU(cudaFree(*p));
     *p = nullptr;
     *have = 0;
     CU(cudaMalloc((void**)p, need * sizeof(T)));
-    CU(cudaMemset(*p, 0, need * sizeof(T)));
+    CU(cudaMemsetAsync(*p, 0, need * sizeof(T), st));
     *have = need;
     return 0;
 }
@@ -262,46 +264,48 @@ static constexpr int64_t WPART_TILES = 2304;   // capacity of the partial buffer
 
 // npanels: outer panels of the factorisation about to run (T' slots of the look-ahead schedule); catchup: also size the fourth
 // V buffer / workspace set (dhqr_qr_host_f64 only)
-static int ensure_workspace(dhqr_context* c, int64_t m, int64_t n_local_max, int64_t npanels = 0, bool catchup = false) {
+static int ensure_workspace(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n_local_max, int64_t npanels = 0, bool catchup = false) {
     TRY(set_attrs(c));
     const int64_t vrows = rup(m, 128) + 128;
     if (c->vrows_cap < vrows || !c->vpk2[0]) {
-        for (int b = 0; b < 3; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK));
+        for (int b = 0; b < 3; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
         c->vrows_cap = vrows;
     }
-    if (catchup) for (int b = 3; b < 3 + c->host_cu_streams; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK));
-    TRY(ensure(&c->linv_all, &c->linv_all_elems, (size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX));
+    if (catchup) for (int b = 3; b < 3 + c->host_cu_streams; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
+    TRY(ensure(&c->linv_all, &c->linv_all_elems, (size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
     const int64_t tiles_max = (n_local_max + NBMAX + G1_BN - 1) / G1_BN + 1;
     for (int b = 0; b < (catchup ? 3 + c->host_cu_streams : 3); ++b) {
         auto& w = c->ws[b];
         // set 2 only ever updates the <= 128 columns of one panel: a quarter of the split-K partial buffer is plenty
-        TRY(ensure(&w.wpart, &w.wpart_elems, (size_t)(b != 2 ? std::max(WPART_TILES, tiles_max) : WPART_TILES / 4) * NBMAX * G1_BN));
-        TRY(ensure(&w.wsum, &w.wsum_elems, (size_t)NBMAX * (rup(n_local_max + NBMAX, 128) + 128)));
-        TRY(ensure(&w.ypk, &w.ypk_elems, (size_t)(NBMAX / KC) * YT * LDK * ((n_local_max + YT - 1) / YT + 2)));
-        TRY(ensure(&w.linv, &w.linv_elems, (size_t)NBMAX * NBMAX));
+        TRY(ensure(&w.wpart, &w.wpart_elems, (size_t)(b != 2 ? std::max(WPART_TILES, tiles_max) : WPART_TILES / 4) * NBMAX * G1_BN, st));
+        TRY(ensure(&w.wsum, &w.wsum_elems, (size_t)NBMAX * (rup(n_local_max + NBMAX, 128) + 128), st));
+        TRY(ensure(&w.ypk, &w.ypk_elems, (size_t)(NBMAX / KC) * YT * LDK * ((n_local_max + YT - 1) / YT + 2), st));
+        TRY(ensure(&w.linv, &w.linv_elems, (size_t)NBMAX * NBMAX, st));
     }
     size_t one = 0;
-    if (!c->sm_ticket) { CU(cudaMalloc((void**)&c->sm_ticket, sizeof(unsigned int) * 1024)); CU(cudaMemset(c->sm_ticket, 0, sizeof(unsigned int) * 1024)); }
+    if (!c->sm_ticket) { CU(cudaMalloc((void**)&c->sm_ticket, sizeof(unsigned int) * 1024)); CU(cudaMemsetAsync(c->sm_ticket, 0, sizeof(unsigned int) * 1024, st)); }
     if (!c->cells2) {
         const size_t words = (2 * (size_t)(PANEL_MAXG + 1) * (IB * (IB + 1) / 2) + IB * IB + 2 * IB) * 2;
         CU(cudaMalloc((void**)&c->cells2, words * sizeof(unsigned long long)));
-        CU(cudaMemset(c->cells2, 0, words * sizeof(unsigned long long)));
+        CU(cudaMemsetAsync(c->cells2, 0, words * sizeof(unsigned long long), st));
         CU(cudaMalloc((void**)&c->fast_stats, 2 * sizeof(int)));
-        CU(cudaMemset(c->fast_stats, 0, 2 * sizeof(int)));
+        CU(cudaMemsetAsync(c->fast_stats, 0, 2 * sizeof(int), st));
         c->ll_epoch = 0;
     }
-    if (!c->cells) { one = 0; TRY(ensure(&c->cells, &one, (size_t)IB * (PANEL_MAXG + 2) * IB * 2)); c->ll_epoch = 0; }
+    if (!c->cells) { one = 0; TRY(ensure(&c->cells, &one, (size_t)IB * (PANEL_MAXG + 2) * IB * 2, st)); c->ll_epoch = 0; }
     if (!c->wctl) {
         CU(cudaMalloc((void**)&c->wctl, sizeof(WideCtl)));
-        const WideCtl init = {W_NOFAIL, 0, {0, 0}};
-        CU(cudaMemcpy(c->wctl, &init, sizeof(init), cudaMemcpyHostToDevice));
+        CU(cudaMemsetAsync(c->wctl, 0, sizeof(WideCtl), st));
+        k_wide_reset<<<1, 32, 0, st>>>(c->wctl);              // initial state {W_NOFAIL, 0}, in the caller's stream order
+        c->launches++;
+        CU(cudaGetLastError());
         size_t o3 = 0;
-        TRY(ensure(&c->wbuf, &o3, (size_t)5 * WP * WP + 3 * XL_ELEMS));
+        TRY(ensure(&c->wbuf, &o3, (size_t)5 * WP * WP + 3 * XL_ELEMS, st));
         CU(cudaMalloc((void**)&c->wstamps, 32 * sizeof(long long)));
-        CU(cudaMemset(c->wstamps, 0, 32 * sizeof(long long)));
+        CU(cudaMemsetAsync(c->wstamps, 0, 32 * sizeof(long long), st));
     }
-    TRY(ensure(&c->v1, &c->v1_elems, (size_t)2 * rup(m + 4, 2)));
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)1));
+    TRY(ensure(&c->v1, &c->v1_elems, (size_t)2 * rup(m + 4, 2), st));
+    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)1, st));
     return 0;
 }
 
@@ -991,7 +995,7 @@ static int qr_blocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, in
     for (auto v : nls) nlmax = std::max(nlmax, v);
     std::vector<Panel> panels;
     build_panels(col0s, nls, nb, panels);
-    TRY(ensure_workspace(c, m, nlmax, (int64_t)panels.size(), !c->up_chunks.empty()));
+    TRY(ensure_workspace(c, st, m, nlmax, (int64_t)panels.size(), !c->up_chunks.empty()));
     if (panels.empty()) return 0;
     // rank-uniform precondition, checked on every rank BEFORE the first collective: a panel that neither chain can take
     // would otherwise fail on its owner only and leave the other ranks inside ncclBroadcast
@@ -1035,7 +1039,7 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
     std::vector<int64_t> col0s, nls;
     TRY(gather_partition(c, st, col0, nl, col0s, nls));
     TRY(check_partition(col0s, nls, n));
-    TRY(ensure_workspace(c, m, nl));
+    TRY(ensure_workspace(c, st, m, nl));
     const int64_t lend = col0 + nl;
     if (c->nranks == 1 && n > 0 && m <= (int64_t)UW_MAXI * UW_THREADS && c->unblocked_wave && !c->profile && !c->sync) {
         // single GPU, short columns: the whole column loop as one persistent cooperative launch (k_unblocked_wave)
@@ -1043,7 +1047,7 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
             if (c->uw_flags) CU(cudaFree(c->uw_flags));
             c->uw_flags = nullptr;
             CU(cudaMalloc((void**)&c->uw_flags, sizeof(unsigned int) * (size_t)(n + 64)));
-            CU(cudaMemset(c->uw_flags, 0, sizeof(unsigned int) * (size_t)(n + 64)));
+            CU(cudaMemsetAsync(c->uw_flags, 0, sizeof(unsigned int) * (size_t)(n + 64), st));
             c->uw_flags_n = (size_t)n + 64;
             c->uw_epoch = 0;
         }
@@ -1151,11 +1155,11 @@ static constexpr int QT_MAXG = 1024;
 static int qt_prepare(dhqr_context* c, cudaStream_t st, int64_t m, int64_t col0, int64_t nl, const double* A, int64_t lda) {
     const int npl = (int)((nl + NBMAX - 1) / NBMAX);
     if (npl <= 0) return 0;
-    TRY(ensure(&c->qt_T, &c->qt_T_elems, (size_t)npl * NBMAX * NBMAX));
+    TRY(ensure(&c->qt_T, &c->qt_T_elems, (size_t)npl * NBMAX * NBMAX, st));
     if (!c->qt_part) {
         CU(cudaMalloc((void**)&c->qt_part, sizeof(double) * (size_t)(QT_MAXG + 1) * WP));     // last row: y
         CU(cudaMalloc((void**)&c->qt_ticket, sizeof(unsigned int)));
-        CU(cudaMemset(c->qt_ticket, 0, sizeof(unsigned int)));
+        CU(cudaMemsetAsync(c->qt_ticket, 0, sizeof(unsigned int), st));
     }
     auto& w = c->ws[0];
     if ((size_t)npl * NBMAX * NBMAX > w.wsum_elems) return set_err(4006, "internal: Gram workspace too small");
@@ -1424,7 +1428,9 @@ int dhqr_set_option(dhqr_handle c, const char* key, int64_t value) {
     } else if (!strcmp(key, "panel_trace")) {
         if (value && !c->panel_trace) {
             CU(cudaMalloc((void**)&c->panel_trace, sizeof(long long) * (size_t)PANEL_MAXG * IB * 8));
-            CU(cudaMemset(c->panel_trace, 0, sizeof(long long) * (size_t)PANEL_MAXG * IB * 8));
+            // no stream here: the fill is complete before the call returns, so every later call sees it
+            CU(cudaMemsetAsync(c->panel_trace, 0, sizeof(long long) * (size_t)PANEL_MAXG * IB * 8, cudaStreamLegacy));
+            CU(cudaStreamSynchronize(cudaStreamLegacy));
         } else if (!value && c->panel_trace) {
             CU(cudaFree(c->panel_trace));
             c->panel_trace = nullptr;
@@ -1538,7 +1544,7 @@ int dhqr_apply_qt_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
     std::vector<int64_t> col0s, nls;
     TRY(gather_partition(c, st, col0, n_local, col0s, nls));
     TRY(check_partition(col0s, nls, n_global));
-    TRY(ensure_workspace(c, m, std::max<int64_t>(n_local, nrhs)));
+    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n_local, nrhs)));
     // C3 (S:227-229): owners act on b one after the other; b travels rank -> rank
     const size_t cnt = (size_t)ldb * (nrhs - 1) + m;
     const bool vec = qt_vec_ok(c, m, nrhs);
@@ -1565,7 +1571,7 @@ int dhqr_apply_q_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, i
     std::vector<int64_t> col0s, nls;
     TRY(gather_partition(c, st, col0, n_local, col0s, nls));
     TRY(check_partition(col0s, nls, n_global));
-    TRY(ensure_workspace(c, m, std::max<int64_t>(n_local, nrhs)));
+    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n_local, nrhs)));
     // b <- H_1 ... H_n b: the owners act in reverse rank order, b travels rank -> rank - 1
     const size_t cnt = (size_t)ldb * (nrhs - 1) + m;
     const bool vec = qt_vec_ok(c, m, nrhs);
@@ -1593,13 +1599,13 @@ int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     std::vector<int64_t> col0s, nls;
     TRY(gather_partition(c, st, col0, n_local, col0s, nls));
     TRY(check_partition(col0s, nls, n_global));
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n_global * nrhs));
+    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n_global * nrhs, st));
     if (c->bs_cells_blocks < (size_t)(n_local + 31) / 32 + 1) {
         if (c->bs_cells) CU(cudaFree(c->bs_cells));
         c->bs_cells = nullptr;
         c->bs_cells_blocks = (size_t)(n_local + 31) / 32 + 64;
         CU(cudaMalloc((void**)&c->bs_cells, c->bs_cells_blocks * 32 * 16));
-        CU(cudaMemset(c->bs_cells, 0, c->bs_cells_blocks * 32 * 16));
+        CU(cudaMemsetAsync(c->bs_cells, 0, c->bs_cells_blocks * 32 * 16, st));
         c->bs_epoch = 0;
     }
     if (!c->bs_wave_max_ctas) {
@@ -1656,7 +1662,7 @@ int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t n = n_global;
-    TRY(ensure_workspace(c, 2 * m, n));
+    TRY(ensure_workspace(c, st, 2 * m, n));
     double2* A = (double2*)dA;
     double2* alpha = (double2*)d_alpha;
     for (int64_t c0 = 0; c0 < n; c0 += CPW) {
@@ -1691,7 +1697,7 @@ int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, 2 * m, std::max<int64_t>(n_global, nrhs)));
+    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n_global, nrhs)));
     const double2* A = (const double2*)dA;
     double2* b = (double2*)d_b;
     for (int64_t c0 = 0; c0 < n_global; c0 += CPW) {         // S:232-242, panel by panel
@@ -1714,7 +1720,7 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t n = n_global;
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)2 * n * nrhs));
+    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)2 * n * nrhs, st));
     const double2* A = (const double2*)dA;
     double2* x = (double2*)c->xbuf;
     for (int64_t o = ((n - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {     // S:260: i = n:-1:1, by blocks
@@ -1822,12 +1828,12 @@ int dhqr_qr_host_f64(dhqr_handle c, int64_t m, int64_t n, double* hA, int64_t ld
     if (blocked) plan_upload(&um, m, n, nbe, B, join);
     else { B = {0, n}; join = {0}; }
     const int nch = (int)B.size() - 1;
-    TRY(ensure(&c->hostA, &c->hostA_elems, (size_t)ldd * n + (size_t)n));
+    cudaStream_t st = c->copy_stream;
+    TRY(ensure(&c->hostA, &c->hostA_elems, (size_t)ldd * n + (size_t)n, st));
     // everything sized once, before the pipeline starts: growing a buffer later would synchronise the device
-    TRY(ensure_workspace(c, m, n, blocked ? (n + nbe - 1) / nbe + 1 : 0, nch > 1));
+    TRY(ensure_workspace(c, st, m, n, blocked ? (n + nbe - 1) / nbe + 1 : 0, nch > 1));
     double* dA = c->hostA;
     double* dal = c->hostA + (size_t)ldd * n;
-    cudaStream_t st = c->copy_stream;
     int rc = 0;
     std::vector<cudaEvent_t> evUp;
     struct timespec ts0;
@@ -1906,11 +1912,11 @@ int dhqr_ldiv_host_f64(dhqr_handle c, int64_t m, int64_t n, const double* hA, in
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     const int64_t ldd = rup(m, 32);
-    TRY(ensure(&c->hostA, &c->hostA_elems, (size_t)ldd * n + (size_t)n));
-    TRY(ensure(&c->hostB, &c->hostB_elems, (size_t)ldd));
+    cudaStream_t st = c->copy_stream;
+    TRY(ensure(&c->hostA, &c->hostA_elems, (size_t)ldd * n + (size_t)n, st));
+    TRY(ensure(&c->hostB, &c->hostB_elems, (size_t)ldd, st));
     double* dA = c->hostA;
     double* dal = c->hostA + (size_t)ldd * n;
-    cudaStream_t st = c->copy_stream;
     CU(cudaMemcpy2DAsync(dA, (size_t)ldd * 8, hA, (size_t)lda * 8, (size_t)m * 8, (size_t)n, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(dal, h_alpha, (size_t)n * 8, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(c->hostB, h_b, (size_t)m * 8, cudaMemcpyHostToDevice, st));   // S:318: b itself is never touched
@@ -1961,7 +1967,7 @@ int dhqr_k_block_reflector_f64(dhqr_handle c, int64_t rows, int nbp, const doubl
     if (!dC) return set_err(-8, "null C");
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, rows, ncols));
+    TRY(ensure_workspace(c, st, rows, ncols));
     const int nbk = nbp <= IB ? IB : NBMAX;
     const int64_t vrows = rup(rows, 128);
     dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), nbk);
@@ -2007,7 +2013,7 @@ int dhqr_k_panel_f64(dhqr_handle c, int64_t rows, int ncols, double* dP, int64_t
     if (!d_alpha) return set_err(-6, "null alpha");
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, rows, ncols));
+    TRY(ensure_workspace(c, st, rows, ncols));
     return launch_panel(c, st, c->vpk2[0], dP, ldp, rows, ncols, d_alpha, 0, 0, rup(rows, 128));
 }
 
@@ -2020,7 +2026,7 @@ int dhqr_k_wide_panel_f64(dhqr_handle c, int64_t rows, double* dP, int64_t ldp, 
     if (!refused) return set_err(-6, "null result");
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, rows, WP));
+    TRY(ensure_workspace(c, st, rows, WP));
     k_wide_reset<<<1, 32, 0, st>>>(c->wctl);
     TRY(post(c, st, "k_wide_reset"));
     const Panel p = {0, 0, WP};

@@ -21,7 +21,9 @@
  *     refused panel is redone by the 32-column chain); (iii) with nranks > 1 every qr / apply_qt /
  *     backsolve call exchanges the column partition first (one small all-gather + stream sync);
  *     (iv) workspace growth (first call, or a larger problem than any before) allocates device memory.
- *     Everything else returns without synchronising.
+ *     Everything else returns without synchronising.  Any caller stream works, non-blocking and prioritised ones
+ *     included: the library depends on no stream but the caller's (workspace zero fills included; its internal streams
+ *     fork from and join back to the caller's stream with events).  tests/test_gpu_streams.py holds every entry point to this.
  *   - no pointer to caller memory is retained after return; workspace lives in the handle.
  *   - a handle is not thread-safe and its calls share one workspace: one handle per host thread, and
  *     consecutive calls on one handle must be on the same stream or ordered by the caller (events);
@@ -84,7 +86,8 @@ int dhqr_destroy(dhqr_handle h);
  *   "profile"     1: CUDA-event bracket per launch (implies serial), read with dhqr_profile_get
  *   also readable: "cvy_persist", "cvy_defer", "wide_trecon", "wide_aux", "hp2", "bs_wave", "unblocked_wave", "fuse_house"
  *                 (kernel and schedule variants, see dhqr_api.cu), so that a caller can put back what it changed
- *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path),
+ *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
+ *                 counters of work the device has finished: read them after synchronising the stream of the calls),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
  *                 "panel_variant" (compile-time DHQR_PANEL_VARIANT of the panel kernel's fast path)
  *   experiment knobs kept for tools/: "panel_levels", "panel_backoff", "panel_trace", "la_trace", "vta_max_chunks",
