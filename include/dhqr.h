@@ -73,9 +73,7 @@ int dhqr_destroy(dhqr_handle h);
  *   "panel_fast"  1 (default): inner panels by CholeskyQR2 + Householder reconstruction with on-device fallback
  *                 to the column-by-column kernel; 0: always column by column
  *   "panel_ctas"  CTAs of the cooperative panel kernel (0 = default: 64 under look-ahead, one per SM otherwise)
- *   "cvy_warps"   MMA warps per gemm_cvy CTA: 8 (default, 32x32 warp tiles) or 4 (64x32)
- *   "gram_sym"    1 (default): Gram matrices of a packed 128-column panel by k_gram_sym (chunk staged once, upper blocks only);
- *                 0: k_gemm_vta with the panel as both operands.  Environment DHQR_GRAM_SYM overrides the default at handle creation
+ *   "cvy_persist" consecutive tiles per CTA of the 128-wide trailing update (default 4; 0: one tile per CTA, same result)
  *   "qt_vec"      1 (default): Q'b / Qb with ONE right-hand side as a GEMV sweep (T' of every panel computed first, then two
  *                 HBM-bound launches per panel that read the reflectors in place); 0: the GEMM-shaped block update, as for nrhs > 1
  *   "host_chunk"  columns per upload chunk of dhqr_qr_host_f64 (default 512, a multiple of 128; 0: one upload, no overlap);
@@ -84,14 +82,17 @@ int dhqr_destroy(dhqr_handle h);
  *                 "host_trace" 1: stage timeline on stderr.  A wrong assumption costs idle time, never correctness
  *   "sync"        1: cudaStreamSynchronize + error check after every kernel launch (debugging; implies serial)
  *   "profile"     1: CUDA-event bracket per launch (implies serial), read with dhqr_profile_get
- *   also readable: "cvy_persist", "cvy_defer", "wide_trecon", "wide_aux", "hp2", "bs_wave", "unblocked_wave", "fuse_house"
- *                 (kernel and schedule variants, see dhqr_api.cu), so that a caller can put back what it changed
+ *   "bs_wave", "unblocked_wave", "fuse_house"  1 (default): back-substitution as one wavefront launch, nb = 1 as one persistent
+ *                 launch (m <= 8192), nb = 1 with the next reflector formed inside the apply kernel, where the shape allows;
+ *                 0: the per-block / per-column launches those paths otherwise take
+ *   "wide_kappa"  guard of the 128-column chain on ||D R1^{-1}||_F of its first Cholesky factor (default 1000)
+ *   traces:       "panel_trace", "la_trace", "wide_trace" (timestamps read with dhqr_debug_copy_f64)
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
- *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
- *                 "panel_variant" (compile-time DHQR_PANEL_VARIANT of the panel kernel's fast path)
- *   experiment knobs kept for tools/: "panel_levels", "panel_backoff", "panel_trace", "la_trace", "vta_max_chunks",
- *                 "hp_max_ctas", "hp_priority", "cvy_stagger" */
+ *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal)
+ *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
+ *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys.
+ *   Any other key returns -2 (unknown option). */
 int dhqr_set_option(dhqr_handle h, const char *key, int64_t value);
 int dhqr_get_option(dhqr_handle h, const char *key, int64_t *value);
 /* Number of kernel launches enqueued by this handle since creation (bench.py: gpu_launches). */

@@ -44,19 +44,8 @@ PATHS = {
     "lookahead0": (2048, 1024, 0, 0, {"lookahead": 0}, None),
     "profile1": (2048, 1024, 0, 0, {"profile": 1}, "lookahead0"),
     "sync1": (2048, 1024, 0, 0, {"sync": 1}, "lookahead0"),
-    # kernel variants.  gram_sym = 0 (k_gemm_vta + k_wreduce: other split-K partials), wide_trecon = 0 (T' by k_tinv from V'V
-    # instead of from the reconstruction) and cvy_defer = 0 (K_G2W: the accumulators start at C instead of adding C after a
-    # k-stage; it only takes the 128-wide update when cvy_persist = 0) change the arithmetic: relative rule only
-    "gram_sym0": (2048, 1024, 0, 0, {"gram_sym": 0}, None),
-    "wide_trecon0": (2048, 1024, 0, 0, {"wide_trecon": 0}, None),
-    "cvy_defer0": (2048, 1024, 0, 0, {"cvy_persist": 0, "cvy_defer": 0}, None),
-    # wide_aux = 0 / hp2 = 0 move the same launches (same workspace sizes, hence the same splits) onto another stream;
-    # cvy_persist = 0 runs K_G2D (k_gemm_cvy<4,..,DEFER>) one tile per CTA, the tile code of k_gemm_cvy_p
-    "wide_aux0": (2048, 1024, 0, 0, {"wide_aux": 0}, "default"),
-    "hp2_0": (2048, 1024, 0, 0, {"hp2": 0}, "default"),
+    # cvy_persist = 0 launches k_gemm_cvy_p with one tile per CTA: the same tile code as the default walk
     "cvy_persist0": (2048, 1024, 0, 0, {"cvy_persist": 0}, "default"),
-    # cvy_warps = 4 (K_G2: 64x32 warp tiles) and K_G2W (32x32) both start from C and walk k in the same order per element
-    "cvy_warps4": (2048, 1024, 0, 0, {"cvy_warps": 4}, "cvy_defer0"),
     # odd lda, a row count that is not a multiple of anything
     "lda+3": (4099, 640, 0, 3, {}, None),
     # nb = 1: persistent k_unblocked_wave (m <= 8192); fused k_house1 + k_apply1_tma chain (m <= 8531: its tile is sized by

@@ -66,6 +66,42 @@ def test_native_library_is_what_runs(D):
     assert h.launch_count() > l0
 
 
+# keys that no longer select anything, with the value they used to default to: a caller that still sets one gets an error
+RETIRED_OPTIONS = {"cvy_warps": 8, "cvy_defer": 1, "cvy_stagger": 0, "gram_sym": 1, "wide_trecon": 1, "wide_aux": 1, "hp2": 1,
+                   "hp_priority": 1, "vta_max_chunks": 0, "hp_max_ctas": 0, "tail_cols": 0, "wide_panel_ctas": 64,
+                   "panel_levels": 2, "panel_backoff": 0, "panel_variant": 4}
+# settable and readable keys -> a valid value other than the default
+READABLE_OPTIONS = {"nb": 64, "panel_ctas": 48, "sync": 1, "profile": 1, "lookahead": 0, "panel_fast": 0, "wide_panel": 0,
+                    "cvy_persist": 2, "qt_vec": 0, "bs_wave": 0, "unblocked_wave": 0, "fuse_house": 0, "host_chunk": 256}
+# settable only -> (a valid value, the default)
+SET_ONLY_OPTIONS = {"wide_kappa": (100, 1000), "host_first": (512, 0), "host_h2d_gbs": (25, 50), "host_tflops": (40, 27),
+                    "host_chain_us": (200, 300), "host_cu_streams": (2, 3), "host_trace": (1, 0), "panel_trace": (1, 0),
+                    "la_trace": (1, 0), "wide_trace": (1, 0)}
+
+
+def test_option_keys(D):
+    lib = D._lib.load()
+    h = D.Handle(0)
+    try:
+        v = C.c_int64(-7)
+        for key, old in RETIRED_OPTIONS.items():
+            assert lib.dhqr_set_option(h.raw, key.encode(), old) == -2, key
+            assert lib.dhqr_get_option(h.raw, key.encode(), C.byref(v)) == -2, key
+            assert v.value == -7
+        for key, val in READABLE_OPTIONS.items():
+            default = h.get_option(key)
+            assert default != val, key
+            h.set_option(key, val)
+            assert h.get_option(key) == val, key
+            h.set_option(key, default)
+            assert h.get_option(key) == default, key
+        for key, (val, default) in SET_ONLY_OPTIONS.items():
+            assert lib.dhqr_set_option(h.raw, key.encode(), val) == 0, key
+            assert lib.dhqr_set_option(h.raw, key.encode(), default) == 0, key
+    finally:
+        h.close()
+
+
 def test_fill_uniform_bit_exact(D, dev, oracle):
     A = D.colmajor_empty(257, 33, dev)
     D.fill_uniform_(A, 7, 3, 5)

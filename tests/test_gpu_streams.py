@@ -320,9 +320,6 @@ def qr_c64_case(D, h):
 # id -> (builder(D, h, fac), options).  The id names the path.
 QR_CASES = {
     "qr-default": (lambda D, h, fac: qr_case(D, h, M2, N2), {}),              # look-ahead, wide chain (synchronises)
-    "qr-wide_aux0": (lambda D, h, fac: qr_case(D, h, M2, N2), {"wide_aux": 0}),
-    "qr-hp2_0": (lambda D, h, fac: qr_case(D, h, M2, N2), {"hp2": 0}),
-    "qr-wide_trecon0": (lambda D, h, fac: qr_case(D, h, M2, N2), {"wide_trecon": 0}),
     "qr-narrow": (lambda D, h, fac: qr_case(D, h, M2, N2), {"wide_panel": 0}),   # look-ahead, 32-column chain, no sync
     "qr-lookahead0": (lambda D, h, fac: qr_case(D, h, M2, N2), {"lookahead": 0}),
     "qr-nb32-lda+1": (lambda D, h, fac: qr_case(D, h, 1000, 300, nb=32, lda_extra=1), {}),

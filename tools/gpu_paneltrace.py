@@ -8,8 +8,8 @@ dev = torch.device("cuda:0"); h = D.default_handle(0)
 rows = int(sys.argv[1]) if len(sys.argv) > 1 else 32768
 vp = lambda t: C.c_void_p(t.data_ptr()); sp = lambda: C.c_void_p(torch.cuda.current_stream().cuda_stream)
 P = D.colmajor_empty(rows, 32, dev); al = torch.zeros(32, dtype=torch.float64, device=dev)
-for pc, bo in ((0, 0), (0, 20), (0, 100), (64, 0), (32, 0)):
-    h.set_option("panel_ctas", pc); h.set_option("panel_trace", 1); h.set_option("panel_backoff", bo)
+for pc in (0, 64, 32):
+    h.set_option("panel_ctas", pc); h.set_option("panel_trace", 1)
     for rep in range(3):
         D.fill_uniform_(P, 1)
         torch.cuda.synchronize()
@@ -21,7 +21,7 @@ for pc, bo in ((0, 0), (0, 20), (0, 100), (64, 0), (32, 0)):
     D._lib.call("dhqr_debug_copy_f64", h.raw, b"panel_trace", vp(tr), 160 * 32 * 8, sp())
     torch.cuda.synchronize()
     t = tr.cpu().numpy().view(np.int64).reshape(160, 32, 8)
-    print(f"panel_ctas={pc} backoff={bo}: kernel {e0.elapsed_time(e1) * 1e3:.1f} us", flush=True)
+    print(f"panel_ctas={pc}: kernel {e0.elapsed_time(e1) * 1e3:.1f} us", flush=True)
     for cta in (0, 40):
         x = t[cta].astype(np.float64)
         names = ["enter", "w0 totals", "block sync", "scalars", "step1+sync", "produce"]

@@ -32,8 +32,8 @@ t = buf.cpu().numpy().reshape(32, 3); h.set_option("la_trace", 0)
 dp = np.diff(np.concatenate([[0], t[:, 0]])); db = np.diff(np.concatenate([[0], t[:, 2]]))
 print("timeline: total %.2f ms; panel steps (ms):" % t[-1].max(), np.round(dp, 2).tolist(), flush=True)
 print("          bulk steps (ms):", np.round(db, 2).tolist(), flush=True)
-for opts in ({"panel_ctas": 132}, {"panel_ctas": 96}, {"cvy_warps": 8}, {"cvy_warps": 8, "panel_ctas": 132}, {"panel_fast": 0}):
+for opts in ({"panel_ctas": 132}, {"panel_ctas": 96}, {"panel_fast": 0}):
     for k, v in opts.items(): h.set_option(k, v)
     show(str(opts))
-    h.set_option("panel_ctas", 0); h.set_option("cvy_warps", 4); h.set_option("panel_fast", 1)
-h.set_option("lookahead", 0); show("serial"); h.set_option("cvy_warps", 8); show("serial cvy_warps=8"); h.set_option("cvy_warps", 4); h.set_option("lookahead", 1)
+    h.set_option("panel_ctas", 0); h.set_option("panel_fast", 1)
+h.set_option("lookahead", 0); show("serial"); h.set_option("lookahead", 1)

@@ -1,4 +1,4 @@
-"""Option sweep on the bench workload (look-ahead)."""
+"""panel_ctas sweep on the bench workload (look-ahead)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -15,9 +15,7 @@ def timeit(reps=3):
         e0.record(); D.householder_(A, al, 0); e1.record(); torch.cuda.synchronize()
         best = min(best, e0.elapsed_time(e1))
     return best
-base = {"hp_max_ctas": 0, "panel_ctas": 0, "vta_max_chunks": 0}
-sweep = ({}, {"panel_ctas": 32}, {"panel_ctas": 48}, {"panel_ctas": 64}, {"panel_ctas": 96}, {"panel_ctas": 128}, {"panel_ctas": 132})
-for opts in sweep:
-    for k, v in {**base, **opts}.items(): h.set_option(k, v)
-    t = timeit(); print(f"{opts}: {t:.2f} ms  {fl / t / 1e9:.2f} TFLOP/s", flush=True)
-for k, v in base.items(): h.set_option(k, v)
+for pc in (0, 32, 48, 64, 96, 128, 132):
+    h.set_option("panel_ctas", pc)
+    t = timeit(); print(f"panel_ctas={pc}: {t:.2f} ms  {fl / t / 1e9:.2f} TFLOP/s", flush=True)
+h.set_option("panel_ctas", 0)

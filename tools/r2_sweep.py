@@ -15,14 +15,12 @@ def timeit(reps=5):
         e0.record(); D.householder_(A, al, 0); e1.record(); torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1))
     return min(ts[1:]), float(np.median(ts[1:]))
-base = {"cvy_persist": 2, "cvy_defer": 1, "lookahead": 1, "wide_panel": 1}
+base = {"cvy_persist": 4, "lookahead": 1, "wide_panel": 1}
 def run(tag, **opts):
     for k, v in {**base, **opts}.items(): h.set_option(k, v)
     t, md = timeit()
     print(f"{tag:40s} min {t:.2f} ms  median {md:.2f} ms  {fl / t / 1e9:.2f} TFLOP/s", flush=True)
     for k, v in base.items(): h.set_option(k, v)
-run("one-tile cvy, loads up front", cvy_persist=0, cvy_defer=0)
-run("one-tile cvy, deferred C", cvy_persist=0)
 for tpc in (1, 2, 3, 4, 6, 8, 16, 1000000):
     run(f"cvy_persist={tpc}", cvy_persist=tpc)
 for tpc in (0, 2, 4, 1000000):

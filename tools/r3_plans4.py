@@ -1,4 +1,4 @@
-"""dhqr_qr_host_f64 at BASELINE config 3: Gram kernel of the panel chain (gram_sym) x catch-up streams x first upload; timeline of the default."""
+"""dhqr_qr_host_f64 at BASELINE config 3: catch-up streams x first upload, against the resident factorisation; timeline of the default."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C
@@ -20,24 +20,22 @@ def run(reps=4):
     return ts
 run(2)
 for rnd in range(2):
-    for gs in (1, 0):
-        for cus in (3, 2):
-            for first in (0, 768):
-                h.set_option("gram_sym", gs); h.set_option("host_cu_streams", cus); h.set_option("host_first", first)
-                run(1)
-                ts = run()
-                print(f"gram_sym {gs} cu_streams {cus} first {first:4d}: " + " ".join(f"{t:.2f}" for t in ts) + " ms", flush=True)
-# device-resident factorisation with both Gram kernels (same process, interleaved)
+    for cus in (3, 2):
+        for first in (0, 768):
+            h.set_option("host_cu_streams", cus); h.set_option("host_first", first)
+            run(1)
+            ts = run()
+            print(f"cu_streams {cus} first {first:4d}: " + " ".join(f"{t:.2f}" for t in ts) + " ms", flush=True)
+# device-resident factorisation (same process)
 A = D.colmajor_empty(m, n, dev); alpha = torch.zeros(n, dtype=torch.float64, device=dev)
-for gs in (1, 0, 1, 0):
-    h.set_option("gram_sym", gs)
+for rnd in range(2):
     ts = []
     for _ in range(6):
         D.fill_uniform_(A, 0); torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); D.householder_(A, alpha, 0); e1.record(); torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1))
-    print(f"resident qr!, gram_sym {gs}: " + " ".join(f"{t:.2f}" for t in ts[1:]) + " ms", flush=True)
-h.set_option("gram_sym", 1); h.set_option("host_cu_streams", 3); h.set_option("host_first", 0)
+    print("resident qr!: " + " ".join(f"{t:.2f}" for t in ts[1:]) + " ms", flush=True)
+h.set_option("host_cu_streams", 3); h.set_option("host_first", 0)
 h.set_option("host_trace", 1)
 run(1)
