@@ -35,6 +35,8 @@ SIGNATURES = {
     "dhqr_backsolve_c64": [_vp, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
     "dhqr_solve_c64": [_vp, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
     "dhqr_partialdot_c64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],
+    "dhqr_form_q_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp],
+    "dhqr_form_q_c64": [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

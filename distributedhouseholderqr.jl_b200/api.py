@@ -388,6 +388,40 @@ def apply_q_(b: torch.Tensor, A, handle: Optional[Handle] = None) -> torch.Tenso
     return _apply("dhqr_apply_q_", b, A, handle)
 
 
+def form_q(A, out: Optional[torch.Tensor] = None, handle: Optional[Handle] = None) -> torch.Tensor:
+    """The thin Q of a factorisation: the first n columns of H_1 ... H_n (numpy.linalg.qr / torch.linalg.qr mode "reduced",
+    LAPACK orgqr / ungqr).  ``A`` is the factored matrix (as for apply_q_ / backsolve_), Float64 or ComplexF64.  Returns Q as an
+    (m, n) column-major tensor of A's dtype: freshly allocated for ``out=None``; ``out is A`` overwrites the factorisation with Q
+    (R is lost: take form_r first); any other ``out`` must be an (m, n) column-major tensor that does not overlap A.
+    Single GPU: a ColumnBlockMatrix on a multi-rank handle raises the library's -1."""
+    if isinstance(A, np.ndarray):
+        raise TypeError("form_q works on a device-resident factorisation (a CUDA tensor), not a numpy array")
+    loc, n, _, h = _dev_args(A)
+    h = handle or h
+    m = loc.shape[0]
+    if out is A:
+        out = loc
+    if out is None:
+        out = colmajor_empty(m, n, loc.device, dtype=loc.dtype)
+    elif out is not loc:
+        if out.dtype != loc.dtype or out.device != loc.device:
+            raise TypeError(f"out must be a {loc.dtype} tensor on {loc.device}")
+        if tuple(out.shape) != (m, n):
+            raise ValueError(f"out must have shape ({m}, {n})")
+    with torch.cuda.device(loc.device):
+        _lib.call("dhqr_form_q_" + _sfx(loc), h.raw, m, n, C.c_void_p(loc.data_ptr()), _lda(loc), C.c_void_p(out.data_ptr()),
+                  _lda(out), _stream_ptr(loc.device))
+    return out
+
+
+def form_r(A, alpha: torch.Tensor) -> torch.Tensor:
+    """R = triu(A[:n], 1) + diag(alpha) as an (n, n) tensor, from the factored matrix and alpha (torch, no kernel of its own).
+    Take it before an in-place form_q, which overwrites R's rows."""
+    loc = A.local if isinstance(A, ColumnBlockMatrix) else A
+    n = loc.shape[1]
+    return torch.triu(loc[:n], 1) + torch.diag(alpha.to(loc.dtype))
+
+
 def backsolve_(b: torch.Tensor, A, alpha: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
     """_solve_householder2! (S:256-282): b[0:n] <- R^{-1} b[0:n] with R = triu(A,1) + diag(alpha); returns b[0:n]."""
     loc, n, col0, h = _dev_args(A)

@@ -1662,6 +1662,80 @@ int dhqr_partialdot_c64(dhqr_handle c, const void* d_a, const void* d_b, int64_t
     return post(c, st, "k_partialdot_c");
 }
 
+// ---- explicit thin Q (LAPACK orgqr / ungqr) ---------------------------------------------------------------------------------
+// Q <- H_1 ... H_n [I_n; 0], accumulated backwards over panels p = last .. 0 with columns [cs, cs + kb): pack V_p from A, make the
+// panel's columns of Q those of the identity (all m rows, which also clears R's rows when Q is A), then apply I - V_p T_p V_p'
+// (T, not T') to rows >= cs, columns [cs, n) of Q.  Columns left of cs are still unit vectors with zeros in rows >= cs, so the
+// panel leaves them alone: 2mn^2 - 2n^3/3 flops instead of the 4mn^2 - 2n^3 of Q applied to [I; 0].  V_p is packed before its
+// columns are overwritten, so in place and out of place are the same sweep.
+static int check_form_q(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* Q, int64_t ldq, size_t esz) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "form_q is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (n > 0 && !A) return set_err(-4, "null matrix pointer");
+    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
+    if (n > 0 && !Q) return set_err(-6, "null Q");
+    if (ldq < std::max<int64_t>(1, m)) return set_err(-7, "ldq < max(1,m)");
+    if (n > 0) {
+        const uintptr_t a0 = (uintptr_t)A, a1 = a0 + ((size_t)(n - 1) * lda + m) * esz;
+        const uintptr_t q0 = (uintptr_t)Q, q1 = q0 + ((size_t)(n - 1) * ldq + m) * esz;
+        if (q0 < a1 && a0 < q1 && !(Q == A && ldq == lda))
+            return set_err(-6, "Q overlaps A without being A itself (Q == A needs ldq == lda)");
+    }
+    return 0;
+}
+
+static int eye_cols(dhqr_context* c, cudaStream_t st, void* Q, bool cplx, int64_t ldq, int64_t m, int64_t c0, int kb) {
+    const dim3 grid((unsigned)std::min<int64_t>((m + 255) / 256, 64), kb);
+    pre(c, st);
+    if (cplx) k_eye_cols<double2><<<grid, 256, 0, st>>>((double2*)Q, ldq, m, c0);
+    else k_eye_cols<double><<<grid, 256, 0, st>>>((double*)Q, ldq, m, c0);
+    return post(c, st, cplx ? "k_eye_cols_c" : "k_eye_cols");
+}
+
+int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, double* dQ, int64_t ldq, void* stream) {
+    TRY(check_form_q(c, m, n, dA, lda, dQ, ldq, sizeof(double)));
+    if (n == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(ensure_workspace(c, st, m, n));
+    TRY(qt_prepare(c, st, m, 0, n, dA, lda));                    // T' of every panel, from A before the sweep writes anything
+    for (int64_t p = (n - 1) / NBMAX; p >= 0; --p) {
+        const int64_t cs = p * NBMAX, rows = m - cs, vrows = rup(rows, 128);   // cs is 128-aligned: the window starts at row cs
+        const int kb = (int)std::min<int64_t>(NBMAX, n - cs);
+        dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), NBMAX);
+        pre(c, st);
+        k_pack<<<grid, 256, 0, st>>>(dA + cs * lda + cs, lda, rows, kb, 1, c->vpk2[0], 0, 0, vrows);
+        TRY(post(c, st, "k_pack"));
+        TRY(eye_cols(c, st, dQ, false, ldq, m, cs, kb));
+        TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, dQ + cs * ldq + cs, ldq, (int)(n - cs), true,
+                                  c->qt_T + (size_t)p * NBMAX * NBMAX, 0, 1));
+    }
+    return 0;
+}
+
+// ComplexF64: the same sweep over 64-column complex panels on the real view of Q (2m x n, leading dimension 2 ldq), each panel the
+// real block reflector of its 128 vectors [v_r, v_i] (dhqr_complex.cuh); T from the Gram block of the update itself.
+int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, void* dQ, int64_t ldq, void* stream) {
+    TRY(check_form_q(c, m, n, dA, lda, dQ, ldq, sizeof(double2)));
+    if (n == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(ensure_workspace(c, st, 2 * m, n));
+    const double2* A = (const double2*)dA;
+    double2* Q = (double2*)dQ;
+    for (int64_t c0 = ((n - 1) / CPW) * CPW; c0 >= 0; c0 -= CPW) {
+        const int kb = (int)std::min<int64_t>(CPW, n - c0);
+        const int64_t mpc = m - c0, rows = 2 * mpc, vrows = rup(rows, 128);
+        TRY(pack_complex_panel(c, st, A + c0 * lda + c0, lda, mpc, kb, vrows));
+        TRY(eye_cols(c, st, Q, true, ldq, m, c0, kb));
+        TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, (double*)(Q + c0 * ldq + c0), 2 * ldq, (int)(n - c0),
+                                  false, nullptr, 0, 1));
+    }
+    return 0;
+}
+
 // ---- host-buffer entry points --------------------------------------------------------------------
 // Plan of the chunked upload of dhqr_qr_host_f64: chunk boundaries B (multiples of nb; B[0] = 0, B.back() = n) and, for every
 // chunk after the first, the step of the look-ahead schedule at which it joins the trailing matrix.  A chunk joins as soon as

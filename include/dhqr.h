@@ -153,6 +153,21 @@ int dhqr_solve_c64(dhqr_handle h, int64_t m, int64_t n_global, int64_t col0, int
 int dhqr_partialdot_c64(dhqr_handle h, const void *d_a, const void *d_b, int64_t i0, int64_t i1, void *d_out,
                         void *stream);
 
+/* ---- explicit thin Q (not in the reference, which never forms Q; SURVEY 8f-3, the second half of Q as an operator) ----------
+ * Q <- the first n columns of Q = H_1 H_2 ... H_n, i.e. Q [I_n; 0] (LAPACK orgqr / ungqr), from a factorisation (dA, lda) in
+ * the library's storage format (any path: blocked, nb = 1, ComplexF64).  dQ: m x n, ldq >= m; written, never read on entry.
+ * dQ == dA with ldq == lda overwrites the factorisation with Q (R is lost: read it first); any other overlap of the two is
+ * rejected.  Whatever reflectors are stored are used as they are: after an exact zero pivot of nb = 1 (INTEGRATION.md) that is
+ * H_1 ... H_n [I; 0] of those reflectors.  Single GPU (a handle with nranks > 1 returns -1).  Stream-ordered, no synchronisation
+ * apart from workspace growth (point (iv)).  Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 / -6 null
+ * matrix with n > 0, -5 / -7 leading dimension < max(1, m), -6 dQ overlaps dA without being it, or dQ == dA with ldq != lda.
+ * n = 0 is a no-op. */
+int dhqr_form_q_f64(dhqr_handle h, int64_t m, int64_t n, const double *dA, int64_t lda, double *dQ, int64_t ldq,
+                    void *stream);
+/* ComplexF64: interleaved (re, im); lda, ldq in complex elements.  Q = H_1 ... H_n with H_j = I - v_j v_j^H. */
+int dhqr_form_q_c64(dhqr_handle h, int64_t m, int64_t n, const void *dA, int64_t lda, void *dQ, int64_t ldq,
+                    void *stream);
+
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
  * the result is in host memory.  With pinned host memory the call is a pipeline: the matrix goes up in
