@@ -197,6 +197,7 @@ static constexpr int G2_BM = 128, G2_BN = YT;               // gemm_cvy: 128 x 6
 
 static size_t smem_g1(int nbp, int bn) { return (size_t)2 * (nbp + bn) * LD1 * 8 + 4 * 8; }
 static size_t smem_g2() { return (size_t)2 * (2 * KC * LD1 + G2_BN * LDK) * 8 + 4 * 8; }
+static size_t smem_g2p() { return (size_t)(2 * (2 * KC * LD1 + G2_BN * LDK) + G2_BN * LDCT) * 8 + 6 * 8; }   // + the C tile: 169 KB
 static size_t smem_tinv(int nbp) { return ((size_t)nbp * (nbp + 1) + 4 * 32 * 33 + (nbp == 128 ? 64 * 65 : 0)) * 8; }
 static size_t smem_ymake(int nbp) { return ((size_t)nbp * nbp + YCOLS * nbp) * 8; }
 
@@ -209,7 +210,7 @@ static int set_attrs(dhqr_context* c) {
     CU(cudaFuncSetAttribute(K_G1_32, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g1(32, G1S_BN)));
     CU(cudaFuncSetAttribute(k_gemm_cvy, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2()));
     CU(cudaFuncSetAttribute(k_gemm_cvy, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2()));
+    CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2p()));
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(k_gram_sym, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_GRAM_SYM));
     CU(cudaFuncSetAttribute(k_tinv<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(128)));
@@ -408,7 +409,9 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     dim3 grid2((unsigned)((rows + G2_BM - 1) / G2_BM), (unsigned)((ncols + G2_BN - 1) / G2_BN));
     g2.tiles_m = (int)grid2.x; g2.tiles_n = (int)grid2.y;
     g2.tiles_per_cta = std::max(c->cvy_persist, 1);   // cvy_persist = 0: one tile per CTA
-    if (g2.nkq == 4) k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, 9 * 32, smem_g2(), st>>>(g2);
+    g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
+    if (g2.nkq == 4)
+        k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, CVYP_THREADS, smem_g2p(), st>>>(g2);
     else k_gemm_cvy<<<grid2, 9 * 32, smem_g2(), st>>>(g2);
     TRY(post(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols));
     return 0;

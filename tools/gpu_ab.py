@@ -1,6 +1,6 @@
 """A/B timing of two builds of libdhqr.so on the bench workload, interleaved in subprocesses on the same box.
 usage: python tools/gpu_ab.py build/libdhqr_prev.so distributedhouseholderqr.jl_b200/libdhqr.so ... [rounds]
-(a library argument may carry options: path:key=value,key=value)"""
+(a library argument may carry options: path:key=value,key=value; the pseudo-option lda=L stores A with leading dimension L)"""
 import os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if os.environ.get("DHQR_AB_LIB"):
@@ -9,10 +9,14 @@ if os.environ.get("DHQR_AB_LIB"):
     import dhqr_b200 as D
     D._lib.LIB_PATH = os.path.abspath(os.environ["DHQR_AB_LIB"])
     dev = torch.device("cuda:0"); h = D.default_handle(0)
-    for kv in os.environ.get("DHQR_AB_OPTS", "").split(","):
-        if kv: k, v = kv.split("="); h.set_option(k, int(v))
     m, n = 32768, 4096
-    A = D.colmajor_empty(m, n, dev); al = torch.zeros(n, dtype=torch.float64, device=dev)
+    lda = m
+    for kv in os.environ.get("DHQR_AB_OPTS", "").split(","):
+        if not kv: continue
+        k, v = kv.split("=")
+        if k == "lda": lda = int(v)
+        else: h.set_option(k, int(v))
+    A = D.colmajor_empty(m, n, dev, lda=lda); al = torch.zeros(n, dtype=torch.float64, device=dev)
     ts = []
     for _ in range(7):
         D.fill_uniform_(A, 0); torch.cuda.synchronize()
