@@ -1561,6 +1561,28 @@ static int check_complex(dhqr_context* c, int64_t m, int64_t n_global, int64_t c
     return 0;
 }
 
+// The complex kernels load and store whole double2 elements, so a ComplexF64 pointer must be 16 B aligned.  The C-ABI takes void*
+// and an 8 B aligned one is legal C (double _Complex, Julia's ComplexF64, a reinterpreted view of a Float64 vector); it is turned
+// down here, before anything is enqueued, instead of faulting on the device.
+static int check_c64_ptr(const void* p, int arg, const char* name) {
+    if ((uintptr_t)p % alignof(double2)) return set_err(arg, "%s is not 16-byte aligned (ComplexF64 data needs the alignment of double2)", name);
+    return 0;
+}
+
+// arguments of dhqr_backsolve_c64 and dhqr_solve_c64 (same signature)
+static int check_c64_args(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
+                          const void* d_alpha, const void* d_b, int64_t ldb, int nrhs) {
+    TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
+    TRY(check_c64_ptr(dA, -6, "A"));
+    if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
+    TRY(check_c64_ptr(d_alpha, -8, "alpha"));
+    if (nrhs < 0) return set_err(-11, "nrhs < 0");
+    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
+    TRY(check_c64_ptr(d_b, -9, "b"));
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
+    return 0;
+}
+
 static int pack_complex_panel(dhqr_context* c, cudaStream_t st, const double2* P, int64_t lda, int64_t mpc, int kb, int64_t vrows) {
     dim3 grid((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), NBMAX);
     k_pack_c<<<grid, 256, 0, st>>>(P, lda, mpc, kb, c->vpk2[0], 0, vrows);
@@ -1570,7 +1592,9 @@ static int pack_complex_panel(dhqr_context* c, cudaStream_t st, const double2* P
 int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, void* dA, int64_t lda, void* d_alpha,
                 void* stream) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
+    TRY(check_c64_ptr(dA, -6, "A"));
     if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
+    TRY(check_c64_ptr(d_alpha, -8, "alpha"));
     if (n_global == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -1604,8 +1628,10 @@ int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
 int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                       void* d_b, int64_t ldb, int nrhs, void* stream) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
+    TRY(check_c64_ptr(dA, -6, "A"));
     if (nrhs < 0) return set_err(-10, "nrhs < 0");
     if (nrhs > 0 && !d_b) return set_err(-8, "null b");
+    TRY(check_c64_ptr(d_b, -8, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-9, "ldb < max(1,m)");
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
@@ -1624,11 +1650,7 @@ int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
 
 int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                        const void* d_alpha, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
-    if (nrhs < 0) return set_err(-11, "nrhs < 0");
-    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
+    TRY(check_c64_args(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs));
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -1648,6 +1670,7 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
 
 int dhqr_solve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                    const void* d_alpha, void* d_b, int64_t ldb, int nrhs, void* stream) {
+    TRY(check_c64_args(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs));   // every argument, before Q'b runs
     TRY(dhqr_apply_qt_c64(c, m, n_global, col0, n_local, dA, lda, d_b, ldb, nrhs, stream));                   // S:288
     return dhqr_backsolve_c64(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs, stream);       // S:291
 }
@@ -1659,6 +1682,9 @@ int dhqr_partialdot_c64(dhqr_handle c, const void* d_a, const void* d_b, int64_t
     if (i0 < 0) return set_err(-4, "i0 < 0");
     if (i1 < i0) return set_err(-5, "i1 < i0");
     if (!d_out) return set_err(-6, "null out");
+    TRY(check_c64_ptr(d_a, -2, "a"));
+    TRY(check_c64_ptr(d_b, -3, "b"));
+    TRY(check_c64_ptr(d_out, -6, "out"));
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     k_partialdot_c<<<1, 1024, 0, st>>>((const double2*)d_a, (const double2*)d_b, i0, i1, (double2*)d_out);
@@ -1722,6 +1748,8 @@ int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64
 // real block reflector of its 128 vectors [v_r, v_i] (dhqr_complex.cuh); T from the Gram block of the update itself.
 int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, void* dQ, int64_t ldq, void* stream) {
     TRY(check_form_q(c, m, n, dA, lda, dQ, ldq, sizeof(double2)));
+    TRY(check_c64_ptr(dA, -4, "A"));
+    TRY(check_c64_ptr(dQ, -6, "Q"));
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;

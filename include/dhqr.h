@@ -13,6 +13,10 @@
  *     LAPACK-info style; > 0 = CUDA/NCCL failure (text via dhqr_last_error()).
  *   - matrices are column-major double with leading dimension lda >= m (Julia Matrix /
  *     localpart(DArray)).  Device pointers unless the name says _host_.
+ *   - storage: any leading dimension >= max(1, m) and any base address with the element type's natural alignment: 8 B for
+ *     Float64, 16 B for ComplexF64 (the _c64 entry points return -(index) for a ComplexF64 pointer that is only 8 B aligned,
+ *     before anything is enqueued).  Results are bitwise independent of both.  Nothing outside the m x n operand (vector,
+ *     alpha) is written, and padding rows or neighbouring data never enter a result, even when they are Inf or NaN.
  *   - stream-ordered: work is enqueued on the caller's cudaStream_t (passed as void*; NULL =
  *     legacy default stream).  Synchronisation points, all of them: (i) the _host_ entry points block
  *     until their result is in host memory; (ii) dhqr_qr_f64 with the default blocked path synchronises
@@ -138,7 +142,10 @@ int dhqr_solve_f64(dhqr_handle h, int64_t m, int64_t n_global, int64_t col0, int
  * partialdot S:51-59, the complex hotloop! S:162-196).  Matrices and vectors are interleaved (re, im) doubles = Julia
  * ComplexF64 / C double _Complex; lda, ldb count COMPLEX elements; alpha is complex (length n).  Same storage format:
  * v scaled to |v|^2 = 2 in the lower trapezoid including the diagonal, H_j = I - v_j v_j^H, diag(R) in alpha.
- * Single GPU: col0 must be 0 and n_local == n_global.  Stream-ordered, no synchronisation. */
+ * Single GPU: col0 must be 0 and n_local == n_global.  Stream-ordered, no synchronisation.  Every ComplexF64 pointer (dA_local,
+ * d_alpha, d_b, dQ, d_a, d_out) must be 16 B aligned: the kernels move whole (re, im) pairs; an 8 B aligned one returns minus its
+ * argument index (dhqr_qr_c64: -6 / -8; apply_qt: -6 / -8; backsolve and solve: -6 / -8 / -9 for A / alpha / b; form_q_c64: -4 / -6;
+ * partialdot_c64: -2 / -3 / -6) and nothing is enqueued. */
 int dhqr_qr_c64(dhqr_handle h, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, void *dA_local,
                 int64_t lda, void *d_alpha, void *stream);
 int dhqr_apply_qt_c64(dhqr_handle h, int64_t m, int64_t n_global, int64_t col0, int64_t n_local,
