@@ -118,6 +118,10 @@ struct dhqr_context {
     } ws[6];                                                            // [2]: the chain's second apply (columns of panel k+2) on its own stream; [3..5]: catch-up (host entry)
     double* linv_all = nullptr; size_t linv_all_elems = 0;              // T' of every outer panel of the factorisation in flight (look-ahead): slot k = panel k
     double* tslot(int k) const { return linv_all + (size_t)k * 128 * 128; }
+    double* gram_all = nullptr; size_t gram_all_elems = 0;              // G = V_b' V_a of each panel pair (slot = first panel of the pair)
+    double* gslot(int k) const { return gram_all + (size_t)k * 128 * 128; }
+    double* vpkb[3] = {nullptr, nullptr, nullptr}; size_t vpkb_elems[3] = {0, 0, 0};   // V of the second panel of a pair, ring as vpk2[0..2]
+    int64_t pair_units = 0;                                             // statistics: panel pairs applied as one 256-wide block
     cudaStream_t hp_stream = nullptr;                                   // stream of the panel chain (high priority)
     cudaStream_t comm_stream = nullptr;                                 // collectives of the look-ahead schedule (high priority)
     cudaStream_t aux_stream = nullptr;                                  // small side kernels of the wide chain (Rt = R2 R1, k_trecon), high priority
@@ -217,6 +221,7 @@ static int set_attrs(dhqr_context* c) {
     CU(cudaFuncSetAttribute(k_tinv<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(32)));
     CU(cudaFuncSetAttribute(k_ymake<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(128)));
     CU(cudaFuncSetAttribute(k_ymake<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(32)));
+    CU(cudaFuncSetAttribute(k_ymake2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_YMAKE2));
     CU(cudaFuncSetAttribute(k_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
     CU(cudaFuncSetAttribute(k_chol128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_WIDE1));
     CU(cudaFuncSetAttribute(k_hr128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_WIDE1));
@@ -252,17 +257,21 @@ static int ensure_workspace(dhqr_context* c, cudaStream_t st, int64_t m, int64_t
     const int64_t vrows = rup(m, 128) + 128;
     if (c->vrows_cap < vrows || !c->vpk2[0]) {
         for (int b = 0; b < 3; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
+        for (int b = 0; b < 3; ++b) TRY(ensure(&c->vpkb[b], &c->vpkb_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
         c->vrows_cap = vrows;
     }
     if (catchup) for (int b = 3; b < 3 + c->host_cu_streams; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
     TRY(ensure(&c->linv_all, &c->linv_all_elems, (size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
+    TRY(ensure(&c->gram_all, &c->gram_all_elems, (size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
     const int64_t tiles_max = (n_local_max + NBMAX + G1_BN - 1) / G1_BN + 1;
     for (int b = 0; b < (catchup ? 3 + c->host_cu_streams : 3); ++b) {
         auto& w = c->ws[b];
         // set 2 only ever updates the <= 128 columns of one panel: a quarter of the split-K partial buffer is plenty
         TRY(ensure(&w.wpart, &w.wpart_elems, (size_t)(b != 2 ? std::max(WPART_TILES, tiles_max) : WPART_TILES / 4) * NBMAX * G1_BN, st));
-        TRY(ensure(&w.wsum, &w.wsum_elems, (size_t)NBMAX * (rup(n_local_max + NBMAX, 128) + 128), st));
-        TRY(ensure(&w.ypk, &w.ypk_elems, (size_t)(NBMAX / KC) * YT * LDK * ((n_local_max + YT - 1) / YT + 2), st));
+        // sets 0-2 also hold W and Y of a panel pair: W_a and W_b side by side, 8 k-chunks of Y per column tile
+        const size_t pairx = b < 3 ? 2 : 1;
+        TRY(ensure(&w.wsum, &w.wsum_elems, pairx * NBMAX * (rup(n_local_max + NBMAX, 128) + 128), st));
+        TRY(ensure(&w.ypk, &w.ypk_elems, pairx * (NBMAX / KC) * YT * LDK * ((n_local_max + YT - 1) / YT + 2), st));
         TRY(ensure(&w.linv, &w.linv_elems, (size_t)NBMAX * NBMAX, st));
     }
     size_t one = 0;
@@ -410,11 +419,82 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     g2.tiles_m = (int)grid2.x; g2.tiles_n = (int)grid2.y;
     g2.tiles_per_cta = std::max(c->cvy_persist, 1);   // cvy_persist = 0: one tile per CTA
     g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
+    g2.nks = 4; g2.vpk2 = nullptr;
     if (g2.nkq == 4)
         k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, CVYP_THREADS, smem_g2p(), st>>>(g2);
     else k_gemm_cvy<<<grid2, 9 * 32, smem_g2(), st>>>(g2);
     TRY(post(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols));
     return 0;
+}
+
+// Partials of W = V' B (V: the 128 packed columns of vpk, B: ncols columns of user storage, `rows` rows) -> w.wpart.
+static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_context::WSet& w, const double* B, int64_t ldb,
+                               int64_t rows, int ncols, const char* what, int* nsplit_out, int64_t* pstride_out) {
+    const int tiles = (ncols + G1_BN - 1) / G1_BN;
+    const int nchunks = (int)((rows + KC1 - 1) / KC1);
+    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart_elems / ((size_t)G1_BN * NBMAX)));
+    const int64_t pstride = (int64_t)tiles * G1_BN * NBMAX;
+    if ((size_t)(pstride * nsplit) > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
+    GemmVtaArgs g1;
+    g1.vpk = vpk; g1.voff = 0; g1.nv = 0;
+    g1.A = B; g1.lda = ldb; g1.rows = rows; g1.na = ncols; g1.nchunks = nchunks;
+    g1.a_aligned = (((uintptr_t)B & 15) == 0 && (ldb & 1) == 0) ? 1 : 0;
+    g1.Wp = w.wpart; g1.pstride = pstride;
+    pre(c, st);
+    K_G1_128<<<dim3(tiles, nsplit), (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
+    *nsplit_out = nsplit;
+    *pstride_out = pstride;
+    return post(c, st, what, 2.0 * (double)rows * NBMAX * ncols);
+}
+
+// W = V' C for one 128-column block -> Ws (128 x ncols, col-major), T' reused
+static int block_w(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_context::WSet& w, const double* C, int64_t ldc, int64_t rows,
+                   int ncols, double* Ws) {
+    int nsplit = 0;
+    int64_t pstride = 0;
+    TRY(launch_vta_partials(c, st, vpk, w, C, ldc, rows, ncols, "k_gemm_vta128", &nsplit, &pstride));
+    pre(c, st);
+    const int64_t nelem = (int64_t)ncols * NBMAX;
+    k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, Ws);
+    return post(c, st, "k_wreduce");
+}
+
+// G = V_b' V_a of a panel pair (a = panel at column ca, b = the next 128 columns) into gout.  Below row ca + 128 the columns of
+// panel a in A hold V_a (the panel is final once factored), so the product runs against A with the existing W kernel.
+static int form_pair_gram(dhqr_context* c, cudaStream_t st, const double* vpk_b, dhqr_context::WSet& w, const double* A, int64_t lda,
+                          int64_t col0, int64_t ca, int64_t m, double* gout) {
+    int nsplit = 0;
+    int64_t pstride = 0;
+    TRY(launch_vta_partials(c, st, vpk_b, w, A + (ca - col0) * lda + ca + WP, lda, m - ca - WP, WP, "k_gram_pair", &nsplit, &pstride));
+    pre(c, st);
+    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, gout);
+    return post(c, st, "k_wreduce");
+}
+
+// Two 128-column blocks a then b in one pass over C:  C <- (I - V_b T_b' V_b')(I - V_a T_a' V_a') C,  i.e.  C += [V_a V_b] [Y_a; Y_b]
+// with K = 256 (k_ymake2).  C = `rows` rows of a's window (starting at a's pivot row); V_b's window starts 128 rows lower.
+// T_a', T_b' and G = V_b' V_a come from their slots.  Skipped on the device when a panel below `gate` was refused.
+static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const double* vpb, dhqr_context::WSet& w, int64_t rows,
+                      double* C, int64_t ldc, int ncols, const double* Ta, const double* Tb, const double* G, int gate) {
+    if (ncols <= 0) return 0;
+    if ((size_t)2 * ncols * NBMAX > w.wsum_elems) return set_err(4003, "internal: W workspace too small");
+    double* Wa = w.wsum, *Wb = w.wsum + (size_t)ncols * NBMAX;
+    TRY(block_w(c, st, vpa, w, C, ldc, rows, ncols, Wa));
+    TRY(block_w(c, st, vpb, w, C + WP, ldc, rows - WP, ncols, Wb));
+    pre(c, st);
+    k_ymake2<<<(ncols + YCOLS - 1) / YCOLS, 256, SMEM_YMAKE2, st>>>(Wa, Wb, ncols, Ta, Tb, G, w.ypk);
+    TRY(post(c, st, "k_ymake2"));
+    pre(c, st);
+    GemmCvyArgs g2;
+    g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.row_lo = 0; g2.ncols = ncols;
+    g2.vpk = vpa; g2.voff = 0; g2.vpk2 = vpb; g2.ypk = w.ypk;
+    g2.nkq = 8; g2.nkq_alloc = 8; g2.nks = 8;
+    g2.ctl = c->wctl; g2.gate = gate;
+    g2.tiles_m = (int)((rows + G2_BM - 1) / G2_BM); g2.tiles_n = (ncols + G2_BN - 1) / G2_BN;
+    g2.tiles_per_cta = std::max(c->cvy_persist, 1);
+    g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
+    k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, CVYP_THREADS, smem_g2p(), st>>>(g2);
+    return post(c, st, "k_gemm_cvy256", 2.0 * ((double)rows * WP + (double)(rows - WP) * WP) * (double)ncols);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -654,21 +734,67 @@ static bool plan_wide(const dhqr_context* c, const Plan& pl, const std::vector<P
     return k >= pl.wide_from && wide_eligible(c, panels[k], m, pl.nb);
 }
 
-// single stream, one panel after the other (options lookahead = 0, sync, profile; any number of ranks)
+// Unit of work of the drivers: one panel, or a pair of panels (a, a + 1) whose trailing update is one 256-wide block (apply_pair),
+// so the bulk update reads and writes C once per 256 reflectors.  A pair needs one rank, both panels through the 128-column
+// chain (nb = 128), and not the windowed first pass of the host entry, whose catch-ups apply one panel at a time.
+struct Unit { int a; int np; };
+static void build_units(const dhqr_context* c, const Plan& pl, const std::vector<Panel>& panels, int64_t m, bool windowed,
+                        std::vector<Unit>& units) {
+    units.clear();
+    const bool pairs = c->nranks == 1 && !windowed;
+    for (int k = pl.kstart; k < (int)panels.size();) {
+        const bool two = pairs && k + 1 < (int)panels.size() && plan_wide(c, pl, panels, k, m) && plan_wide(c, pl, panels, k + 1, m);
+        units.push_back({k, two ? 2 : 1});
+        k += two ? 2 : 1;
+    }
+}
+
+// Factor the panels of unit u into va (and vb): a pair factors a, applies V_a to the columns of b (K = 128, T'_a from its slot),
+// factors b and forms G = V_b' V_a.  T' of a single panel goes to linv_single, of a pair's panels to their slots.  Returns in
+// *ownT whether T' of the unit is known on this rank.
+static int factor_unit(dhqr_context* c, cudaStream_t st, const Unit& u, double* va, double* vb, dhqr_context::WSet& w,
+                       const std::vector<Panel>& panels, const Plan& pl, int64_t m, int64_t col0, double* A, int64_t lda, double* alpha,
+                       double* linv_single, bool* ownT) {
+    const int a = u.a;
+    const Panel& pa = panels[a];
+    if (u.np == 1) {
+        const bool wide = plan_wide(c, pl, panels, a, m);
+        TRY(factor_outer_panel(c, st, va, w, pa, m, col0, A, lda, alpha, a, wide, linv_single));
+        TRY(mirror_panel_to_host(c, st, pa, m, col0, A, lda));
+        *ownT = wide;
+        return 0;
+    }
+    const Panel& pb = panels[a + 1];
+    const PanelGeom ga = panel_geom(pa, m);
+    TRY(factor_outer_panel(c, st, va, w, pa, m, col0, A, lda, alpha, a, true, c->tslot(a)));
+    TRY(mirror_panel_to_host(c, st, pa, m, col0, A, lda));
+    TRY(apply_block_reflector(c, st, va, w, 0, WP, ga.rows, 0, A + (pb.c - col0) * lda + ga.r0, lda, WP, true, c->tslot(a), a + 1));
+    TRY(factor_outer_panel(c, st, vb, w, pb, m, col0, A, lda, alpha, a + 1, true, c->tslot(a + 1)));
+    TRY(mirror_panel_to_host(c, st, pb, m, col0, A, lda));
+    TRY(form_pair_gram(c, st, vb, w, A, lda, col0, pa.c, m, c->gslot(a)));
+    c->pair_units++;
+    *ownT = true;
+    return 0;
+}
+
+// single stream, one unit after the other (options lookahead = 0, sync, profile; any number of ranks)
 static int qr_blocked_serial(dhqr_context* c, cudaStream_t st, int64_t m, int64_t col0, int64_t nl, double* A, int64_t lda,
-                             double* alpha, const std::vector<Panel>& panels, const Plan& pl) {
+                             double* alpha, const std::vector<Panel>& panels, const Plan& pl, const std::vector<Unit>& units) {
     const int64_t lend = col0 + nl;
     double* vpk = c->vpk2[0];
     auto& w = c->ws[0];
-    for (int k = pl.kstart; k < (int)panels.size(); ++k) {
+    for (const Unit& u : units) {
+        const int k = u.a;
         const Panel& p = panels[k];
         const PanelGeom g = panel_geom(p, m);
         bool haveT = false;
-        if (c->rank == p.owner) {
-            const bool wide = plan_wide(c, pl, panels, k, m);
-            TRY(factor_outer_panel(c, st, vpk, w, p, m, col0, A, lda, alpha, k, wide, w.linv));
-            TRY(mirror_panel_to_host(c, st, p, m, col0, A, lda));
-            haveT = wide;
+        if (c->rank == p.owner) TRY(factor_unit(c, st, u, vpk, c->vpkb[0], w, panels, pl, m, col0, A, lda, alpha, w.linv, &haveT));
+        if (u.np == 2) {
+            const int64_t t0 = panels[k + 1].c + WP;
+            if (t0 < lend)
+                TRY(apply_pair(c, st, vpk, c->vpkb[0], w, g.rows, A + (t0 - col0) * lda + g.r0, lda, (int)(lend - t0), c->tslot(k),
+                               c->tslot(k + 1), c->gslot(k), k + 2));
+            continue;
         }
         if (c->nranks > 1) {
             // C2 (S:141-143): the owner's reflectors go to every rank, once per panel instead of once per column
@@ -696,10 +822,14 @@ static int qr_blocked_serial(dhqr_context* c, cudaStream_t st, int64_t m, int64_
 // Every column block receives every V exactly once and in order; the panel chain only depends on the small
 // (a) parts, i.e. it has two bulk updates of slack.  Three V buffers: V_{k+2} replaces V_{k-1}, whose last
 // reader (b)_{k-1} precedes (a)_k on st (hence the wait on next[k-1] on every rank before the broadcast).
+// k counts units (build_units): "panel k" above is unit k, a single panel or a pair whose updates run with K = 256; a pair's
+// second V buffer (vpkb) and G slot follow the same ring rule.  la_times stays per panel (both panels of a pair get the pair's).
 static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int64_t col0, int64_t nl, double* A, int64_t lda,
-                                double* alpha, const std::vector<Panel>& panels, const Plan& pl) {
+                                double* alpha, const std::vector<Panel>& panels, const Plan& pl, const std::vector<Unit>& units) {
     const int64_t lend = col0 + nl;
-    const int K = (int)panels.size(), K0 = pl.kstart;
+    const int K = (int)units.size(), K0 = 0;
+    auto P = [&](int k) -> const Panel& { return panels[units[k].a]; };                              // first panel of unit k
+    auto uend = [&](int k) { const Panel& q = panels[units[k].a + units[k].np - 1]; return q.c + q.kb; };
     cudaStream_t hp = c->hp_stream;
     std::vector<cudaEvent_t> evPanel(K), evNext(K), evBulk(K), evA2(K);
     std::vector<char> haveA2(K, 0);
@@ -720,14 +850,14 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     std::vector<cudaEvent_t> evHp(K, nullptr);
     auto publish = [&](int k) -> int {
         if (c->nranks > 1) {
-            const PanelGeom g = panel_geom(panels[k], m);
+            const PanelGeom g = panel_geom(P(k), m);
             double* v = c->vpk2[k % 3];
             CU(cudaEventCreateWithFlags(&evHp[k], cudaEventDisableTiming));
             CU(cudaEventRecord(evHp[k], hp));
             CU(cudaStreamWaitEvent(cs, evHp[k], 0));
-            NC(g_nccl.Broadcast(v, v, (size_t)(g.vrows / KC1) * VPK_CHUNK, ncclFloat64, panels[k].owner, c->comm, cs));
-            NC(g_nccl.Broadcast(alpha + panels[k].c, alpha + panels[k].c, (size_t)panels[k].kb, ncclFloat64, panels[k].owner, c->comm, cs));
-            k_wide_note<<<1, 32, 0, cs>>>(c->wctl, v + KC1, k);   // the owner's verdict on the panel arrived with the buffer
+            NC(g_nccl.Broadcast(v, v, (size_t)(g.vrows / KC1) * VPK_CHUNK, ncclFloat64, P(k).owner, c->comm, cs));
+            NC(g_nccl.Broadcast(alpha + P(k).c, alpha + P(k).c, (size_t)P(k).kb, ncclFloat64, P(k).owner, c->comm, cs));
+            k_wide_note<<<1, 32, 0, cs>>>(c->wctl, v + KC1, units[k].a);   // the owner's verdict on the panel arrived with the buffer
             TRY(post(c, cs, "k_wide_note"));
             CU(cudaEventRecord(evPanel[k], cs));
         } else {
@@ -737,7 +867,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     };
     // V_k is usable on stream s: the owner has it once its own chain got there (hp order / evHp), the others once it arrived
     auto wait_panel = [&](cudaStream_t s, int k) {
-        if (c->nranks > 1 && c->rank == panels[k].owner) {
+        if (c->nranks > 1 && c->rank == P(k).owner) {
             if (s != hp) cudaStreamWaitEvent(s, evHp[k], 0);
         } else {
             cudaStreamWaitEvent(s, evPanel[k], 0);
@@ -748,7 +878,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     // while it still lies right of panel k+2 - after a CATCH-UP on its own stream: the reflectors of panels < k, re-packed from
     // the factored columns, applied to the chunk with the T' kept in the per-panel slots.  Same reflectors in the same order on
     // every column, only the time at which a column receives them changes.
-    const bool windowed = !c->up_chunks.empty() && c->nranks == 1 && K0 == 0;
+    const bool windowed = !c->up_chunks.empty() && c->nranks == 1 && pl.kstart == 0;   // then every unit is one panel
     int64_t wend = windowed ? std::min(lend, c->up_chunks.front().c0) : lend;
     size_t upnext = 0;
     std::vector<char> haveTslot(K, 0);
@@ -758,7 +888,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
         auto& ws_cu = c->ws[3 + lane];
         cudaStreamWaitEvent(cu, u.ev, 0);
         for (int q = K0; q < k; ++q) {
-            const Panel& pq = panels[q];
+            const Panel& pq = P(q);
             const PanelGeom gq = panel_geom(pq, m);
             cudaStreamWaitEvent(cu, evPanel[q], 0);                   // V_q is final in A ...
             cudaStreamWaitEvent(cu, evNext[q], 0);                    // ... and T'_q sits in its slot
@@ -766,7 +896,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             k_pack<<<grid, 256, 0, cu>>>(A + (pq.c - col0) * lda + pq.c, lda, m - pq.c, pq.kb, 1, vpk_cu, 0, pq.c - gq.r0, gq.vrows);
             TRY(post(c, cu, "k_pack"));
             TRY(apply_block_reflector(c, cu, vpk_cu, ws_cu, 0, gq.nbp, gq.rows, pq.c - gq.r0, A + (u.c0 - col0) * lda + gq.r0, lda,
-                                      (int)(u.c1 - u.c0), haveTslot[q] != 0, c->tslot(q), q + 1));
+                                      (int)(u.c1 - u.c0), haveTslot[q] != 0, c->tslot(units[q].a), units[q].a + 1));
         }
         cudaEventRecord(done, cu);
         return 0;
@@ -780,26 +910,35 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
         cudaEventRecord(fork, st);
         cudaStreamWaitEvent(hp, fork, 0);                          // hp starts after everything already queued on st
         std::vector<char> ownT(K, 0);       // T'_k already sits in the ring slot on this rank (wide panel factored here, k_trecon)
-        if (c->rank == panels[K0].owner) {
-            const bool wide = plan_wide(c, pl, panels, K0, m);
-            if ((rc = factor_outer_panel(c, hp, c->vpk2[K0 % 3], c->ws[1], panels[K0], m, col0, A, lda, alpha, K0, wide, c->tslot(K0)))) break;
-            if ((rc = mirror_panel_to_host(c, hp, panels[K0], m, col0, A, lda))) break;
+        if (c->rank == P(K0).owner) {
+            bool wide = false;
+            if ((rc = factor_unit(c, hp, units[K0], c->vpk2[K0 % 3], c->vpkb[K0 % 3], c->ws[1], panels, pl, m, col0, A, lda, alpha,
+                                  c->tslot(units[K0].a), &wide))) break;
             if (wide) { ownT[K0] = 1; cudaEventRecord(evNext[K0], hp); }
         }
         if ((rc = publish(K0))) break;
         for (int k = K0; k < K && !rc; ++k) {
-            const Panel& p = panels[k];
+            const Panel& p = P(k);
             const PanelGeom g = panel_geom(p, m);
             const double* vk = c->vpk2[k % 3];
-            const int64_t t0 = p.c + p.kb;                                               // first trailing column
-            const int64_t t1 = k + 1 < K ? panels[k + 1].c + panels[k + 1].kb : t0;      // end of panel k+1
-            const int64_t t2 = k + 2 < K ? panels[k + 2].c + panels[k + 2].kb : t1;      // end of panel k+2
+            const int pk = units[k].a;                                                   // first panel of the unit
+            const int64_t t0 = uend(k);                                                  // first trailing column
+            const int64_t t1 = k + 1 < K ? uend(k + 1) : t0;                             // end of unit k+1
+            const int64_t t2 = k + 2 < K ? uend(k + 2) : t1;                             // end of unit k+2
+            // V_k (one panel, or both panels of a pair: K = 256, T' and G from their slots) -> local columns [lo, hi) on stream s
+            auto apply_k = [&](cudaStream_t s, dhqr_context::WSet& w, int64_t lo, int64_t hi, bool haveT, double* linv_io) -> int {
+                double* C = A + (lo - col0) * lda + g.r0;
+                if (units[k].np == 2)
+                    return apply_pair(c, s, vk, c->vpkb[k % 3], w, g.rows, C, lda, (int)(hi - lo), c->tslot(pk), c->tslot(pk + 1),
+                                      c->gslot(pk), pk + 2);
+                return apply_block_reflector(c, s, vk, w, 0, g.nbp, g.rows, p.c - g.r0, C, lda, (int)(hi - lo), haveT, linv_io, pk + 1);
+            };
             int64_t lo, hi;
             // chunks that join the window at this step: planned, or forced because step k+1 would reach into them
             const int64_t wold = wend;
             const size_t up0 = upnext;
             if (windowed) {
-                const int64_t t3 = k + 3 < K ? panels[k + 3].c + panels[k + 3].kb : lend;   // end of panel k+3
+                const int64_t t3 = k + 3 < K ? uend(k + 3) : lend;                         // end of unit k+3
                 while (upnext < c->up_chunks.size() && (c->up_chunks[upnext].join <= k || c->up_chunks[upnext].c0 < t3)) {
                     const auto& u = c->up_chunks[upnext];
                     if (u.c0 < t2 || u.c0 != wend) { rc = set_err(4005, "internal: upload chunk %d joins too late (step %d)", (int)upnext, k); break; }
@@ -814,7 +953,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
                 if (rc) break;
                 if (wend < t2) { rc = set_err(4005, "internal: window ends at %lld before panel %d", (long long)wend, k + 2); break; }
             }
-            double* lk = c->tslot(k);
+            double* lk = c->tslot(pk);
             bool haveT = ownT[k];                                        // T'_k in lk (this rank)
             if (k + 1 < K) {
                 // vpk[(k+1)%3] was last read by the bulk update k-2 (and, on the owner of panel k-2, by its broadcast)
@@ -823,21 +962,19 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
                     if (haveA2[k - 2]) cudaStreamWaitEvent(hp, evA2[k - 2], 0);
                     if (c->nranks > 1) cudaStreamWaitEvent(hp, evPanel[k - 2], 0);
                 }
-                if (c->rank == panels[k + 1].owner) {
+                if (c->rank == P(k + 1).owner) {
                     wait_panel(hp, k);
                     if (k - 1 >= K0 && haveA2[k - 1]) cudaStreamWaitEvent(hp, evA2[k - 1], 0);   // V_{k-1} reached these columns
                     if (clip(t0, t1, lo, hi)) {
                         const bool hadT = haveT;
-                        if ((rc = apply_block_reflector(c, hp, vk, c->ws[1], 0, g.nbp, g.rows, p.c - g.r0, A + (lo - col0) * lda + g.r0,
-                                                        lda, (int)(hi - lo), haveT, lk, k + 1))) break;
+                        if ((rc = apply_k(hp, c->ws[1], lo, hi, haveT, lk))) break;
                         haveT = true;
                         if (!hadT) cudaEventRecord(evNext[k], hp);       // T'_k is in the ring: the bulk update may start
                     }
-                    const bool widen = plan_wide(c, pl, panels, k + 1, m);
-                    if ((rc = factor_outer_panel(c, hp, c->vpk2[(k + 1) % 3], c->ws[1], panels[k + 1], m, col0, A, lda, alpha, k + 1, widen,
-                                                 c->tslot(k + 1)))) break;
+                    bool widen = false;
+                    if ((rc = factor_unit(c, hp, units[k + 1], c->vpk2[(k + 1) % 3], c->vpkb[(k + 1) % 3], c->ws[1], panels, pl, m, col0, A,
+                                          lda, alpha, c->tslot(units[k + 1].a), &widen))) break;
                     if (widen) { ownT[k + 1] = 1; cudaEventRecord(evNext[k + 1], hp); }
-                    if ((rc = mirror_panel_to_host(c, hp, panels[k + 1], m, col0, A, lda))) break;
                 }
                 if ((rc = publish(k + 1))) break;
             }
@@ -851,8 +988,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
                 if (k - 1 >= K0) cudaStreamWaitEvent(s2, evBulk[k - 1], 0);
                 wait_panel(s2, k);
                 const bool hadT = haveT;
-                if ((rc = apply_block_reflector(c, s2, vk, c->ws[2], 0, g.nbp, g.rows, p.c - g.r0,
-                                                A + (lo - col0) * lda + g.r0, lda, (int)(hi - lo), haveT, lk, k + 1))) break;
+                if ((rc = apply_k(s2, c->ws[2], lo, hi, haveT, lk))) break;
                 haveT = true;
                 if (!hadT) cudaEventRecord(evNext[k], s2);               // T'_k came from this apply
                 cudaEventRecord(evA2[k], s2);
@@ -862,15 +998,13 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             wait_panel(st, k);
             if (clip(t2, std::min(lend, wold), lo, hi)) {
                 if (haveT) cudaStreamWaitEvent(st, evNext[k], 0);
-                if ((rc = apply_block_reflector(c, st, vk, c->ws[0], 0, g.nbp, g.rows, p.c - g.r0, A + (lo - col0) * lda + g.r0, lda,
-                                                (int)(hi - lo), haveT, haveT ? lk : nullptr, k + 1))) break;
+                if ((rc = apply_k(st, c->ws[0], lo, hi, haveT, haveT ? lk : nullptr))) break;
             }
             for (size_t j = up0; j < upnext && !rc; ++j) {             // the chunks that joined at this step, each behind its catch-up
                 const auto& u = c->up_chunks[j];
                 cudaStreamWaitEvent(st, evCatch[j], 0);
                 if (haveT) cudaStreamWaitEvent(st, evNext[k], 0);
-                rc = apply_block_reflector(c, st, vk, c->ws[0], 0, g.nbp, g.rows, p.c - g.r0, A + (u.c0 - col0) * lda + g.r0, lda,
-                                           (int)(u.c1 - u.c0), haveT, haveT ? lk : nullptr, k + 1);
+                rc = apply_k(st, c->ws[0], u.c0, u.c1, haveT, haveT ? lk : nullptr);
             }
             if (rc) break;
             haveTslot[k] = haveT;
@@ -885,12 +1019,13 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
         if (c->la_trace) {
             cudaStreamSynchronize(st);
             cudaStreamSynchronize(hp);
-            c->la_times.assign((size_t)K * 3, 0.f);
-            for (int k = K0; k < K; ++k) {
-                cudaEventElapsedTime(&c->la_times[3 * k + 0], fork, evPanel[k]);
-                cudaEventElapsedTime(&c->la_times[3 * k + 1], fork, evNext[k]);
-                cudaEventElapsedTime(&c->la_times[3 * k + 2], fork, evBulk[k]);
-            }
+            c->la_times.assign(panels.size() * 3, 0.f);
+            for (int k = K0; k < K; ++k)
+                for (int q = units[k].a; q < units[k].a + units[k].np; ++q) {
+                    cudaEventElapsedTime(&c->la_times[3 * q + 0], fork, evPanel[k]);
+                    cudaEventElapsedTime(&c->la_times[3 * q + 1], fork, evNext[k]);
+                    cudaEventElapsedTime(&c->la_times[3 * q + 2], fork, evBulk[k]);
+                }
             if (c->host_trace) {   // stage timeline of the pipelined host entry (ms since the first chunk was on the device)
                 for (size_t j = 0; j < evCatch.size(); ++j) {
                     float tu = -1.f, tc = -1.f;
@@ -900,7 +1035,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
                     fprintf(stderr, "[dhqr host] chunk at column %5lld: uploaded %7.2f ms, joins at step %2d (planned %2d), caught up %7.2f ms\n",
                             (long long)c->up_chunks[j].c0, tu, joinedAt[j], c->up_chunks[j].join, tc);
                 }
-                for (int k = K0; k < K; ++k)
+                for (int k = pl.kstart; k < (int)panels.size(); ++k)
                     fprintf(stderr, "[dhqr host] step %2d: panel %7.2f  T' %7.2f  bulk %7.2f ms\n", k, c->la_times[3 * k], c->la_times[3 * k + 1],
                             c->la_times[3 * k + 2]);
             }
@@ -969,8 +1104,10 @@ static int qr_blocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, in
             for (const auto& u : c->up_chunks) CU(cudaStreamWaitEvent(st, u.ev, 0));
             c->up_chunks.clear();
         }
-        const int rc = use_la ? qr_blocked_lookahead(c, st, m, col0, nl, A, lda, alpha, panels, pl)
-                              : qr_blocked_serial(c, st, m, col0, nl, A, lda, alpha, panels, pl);
+        std::vector<Unit> units;
+        build_units(c, pl, panels, m, use_la && !c->up_chunks.empty() && pl.kstart == 0, units);
+        const int rc = use_la ? qr_blocked_lookahead(c, st, m, col0, nl, A, lda, alpha, panels, pl, units)
+                              : qr_blocked_serial(c, st, m, col0, nl, A, lda, alpha, panels, pl, units);
         c->up_chunks.clear();                     // every chunk has joined (or the pass failed): a restart sees the whole matrix
         if (rc || !any_wide) return rc;
         // The wide chain is speculative: its guards are evaluated on the device.  One synchronisation per factorisation to
@@ -982,6 +1119,20 @@ static int qr_blocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, in
         if (fail == W_NOFAIL) return 0;
         if (fail < pl.kstart || fail >= (int)panels.size()) return set_err(4004, "internal: bad restart index %d", fail);
         c->wide_redone++;
+        for (const Unit& u : units)
+            if (u.np == 2 && u.a + 1 == fail) {
+                // the refused panel is the second of a pair: V_a reached b's columns (inner apply), but not the columns right of b,
+                // whose merged update was skipped.  Apply V_a alone there (re-packed from A, T'_a from its slot) before redoing b.
+                const Panel& pa = panels[u.a];
+                const PanelGeom ga = panel_geom(pa, m);
+                const int64_t t0 = panels[fail].c + panels[fail].kb;
+                if (t0 >= col0 + nl) break;
+                dim3 grid((unsigned)std::min<int64_t>((ga.vrows / 4 + 255) / 256, 4 * c->sms), NBMAX);
+                k_pack<<<grid, 256, 0, st>>>(A + (pa.c - col0) * lda + pa.c, lda, m - pa.c, pa.kb, 1, c->vpk2[0], 0, 0, ga.vrows);
+                TRY(post(c, st, "k_pack"));
+                TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, WP, ga.rows, 0, A + (t0 - col0) * lda + ga.r0, lda,
+                                          (int)(col0 + nl - t0), true, c->tslot(u.a), 0));
+            }
         pl.kstart = fail;
         pl.wide_from = fail + 1;
     }
@@ -1380,6 +1531,7 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
     else if (!strcmp(key, "host_chunk")) *value = c->host_chunk;
     else if (!strcmp(key, "wide_panels")) *value = c->wide_panels;
     else if (!strcmp(key, "wide_redone")) *value = c->wide_redone;
+    else if (!strcmp(key, "pair_units")) *value = c->pair_units;
     else if (!strcmp(key, "panels_fast") || !strcmp(key, "panels_fallback")) {
         int st2[2] = {0, 0};
         if (c->fast_stats) CU(cudaMemcpy(st2, c->fast_stats, sizeof(st2), cudaMemcpyDeviceToHost));
