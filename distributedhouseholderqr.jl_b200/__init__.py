@@ -5,10 +5,11 @@ Import as ``import dhqr_b200`` (repo-root shim) — the directory keeps the name
 """
 from . import _lib
 from .api import (ColumnBlockMatrix, DistributedHouseholderQRStruct, Handle, LocalColumnBlock, alphafactor,
-                  apply_q_, apply_qt_, backsolve_, balanced_splits, colmajor_empty, default_handle, fill_uniform_, form_q, form_r, householder_,
-                  init_distributed, ldiv, partialdot, plan_host_upload, qr_, qr_bang, shutdown_distributed, solve_householder_, splits, to_colmajor)
+                  apply_q_, apply_qt_, backsolve_, balanced_splits, colmajor_empty, default_handle, fill_uniform_, form_q, form_r,
+                  forwardsolve_, householder_, init_distributed, ldiv, ldiv_adjoint, partialdot, plan_host_upload, qr_, qr_bang,
+                  shutdown_distributed, solve_adjoint_, solve_householder_, splits, to_colmajor)
 
 __all__ = ["ColumnBlockMatrix", "DistributedHouseholderQRStruct", "Handle", "LocalColumnBlock", "alphafactor",
-           "apply_q_", "apply_qt_", "backsolve_", "balanced_splits", "colmajor_empty", "default_handle", "fill_uniform_", "form_q", "form_r", "householder_", "init_distributed",
-           "ldiv", "partialdot", "plan_host_upload", "qr_", "qr_bang", "shutdown_distributed", "solve_householder_", "splits",
-           "to_colmajor", "_lib"]
+           "apply_q_", "apply_qt_", "backsolve_", "balanced_splits", "colmajor_empty", "default_handle", "fill_uniform_", "form_q", "form_r",
+           "forwardsolve_", "householder_", "init_distributed", "ldiv", "ldiv_adjoint", "partialdot", "plan_host_upload", "qr_", "qr_bang",
+           "shutdown_distributed", "solve_adjoint_", "solve_householder_", "splits", "to_colmajor", "_lib"]

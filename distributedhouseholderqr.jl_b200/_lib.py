@@ -37,6 +37,10 @@ SIGNATURES = {
     "dhqr_partialdot_c64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],
     "dhqr_form_q_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp],
     "dhqr_form_q_c64": [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp],
+    "dhqr_forwardsolve_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
+    "dhqr_forwardsolve_c64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
+    "dhqr_solve_adj_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
+    "dhqr_solve_adj_c64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

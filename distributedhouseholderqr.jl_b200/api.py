@@ -278,6 +278,9 @@ class DistributedHouseholderQRStruct:
 
     solve = ldiv
 
+    def ldiv_adjoint(self, c):
+        return ldiv_adjoint(self, c)
+
 
 def _dev_args(A):
     if isinstance(A, ColumnBlockMatrix):
@@ -432,6 +435,56 @@ def backsolve_(b: torch.Tensor, A, alpha: torch.Tensor, handle: Optional[Handle]
         _lib.call("dhqr_backsolve_" + _sfx(loc), h.raw, m, n, col0, loc.shape[1], C.c_void_p(loc.data_ptr()), _lda(loc),
                   C.c_void_p(alpha.data_ptr()), C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(loc.device))
     return b[:n]
+
+
+def _adj(fn: str, b: torch.Tensor, A, alpha: torch.Tensor, handle: Optional[Handle]) -> int:
+    if isinstance(A, np.ndarray):
+        raise TypeError("the adjoint solves work on a device-resident factorisation (a CUDA tensor), not a numpy array")
+    loc, n, _, h = _dev_args(A)
+    h = handle or h
+    m = loc.shape[0]
+    if alpha.dtype != loc.dtype:
+        raise TypeError("alpha must have the element type of A")
+    ldb, nrhs = _rhs_args(b, m, loc.dtype)
+    with torch.cuda.device(loc.device):
+        _lib.call(fn + _sfx(loc), h.raw, m, n, C.c_void_p(loc.data_ptr()), _lda(loc), C.c_void_p(alpha.data_ptr()),
+                  C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(loc.device))
+    return n
+
+
+def forwardsolve_(b: torch.Tensor, A, alpha: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
+    """b[0:n] <- R^{-H} b[0:n] (R^{-T} for Float64) with R = triu(A,1) + diag(alpha): forward substitution with the lower-triangular
+    R^H, the adjoint of backsolve_.  ``b``: length-m vector or (m, k) column-major block; rows n..m-1 are left as they are.
+    Returns b[0:n].  Single GPU."""
+    return b[:_adj("dhqr_forwardsolve_", b, A, alpha, handle)]
+
+
+def solve_adjoint_(b: torch.Tensor, A, alpha: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
+    """The minimum-norm solution of A^H y = c (LAPACK ?gels, TRANS = 'C'): rows [0, n) of ``b`` hold c on entry, all m rows hold
+    y = Q [R^{-H} c; 0] on return.  ``b``: length-m vector or (m, k) column-major block.  Returns b.  Single GPU."""
+    _adj("dhqr_solve_adj_", b, A, alpha, handle)
+    return b
+
+
+def ldiv_adjoint(H: DistributedHouseholderQRStruct, c):
+    """H^H \\ c: the minimum-norm solution y of A^H y = c for the factored A (length n, or (n, k)).  Neither H nor c is modified;
+    returns a new length-m vector or (m, k) tensor."""
+    if isinstance(H.A, np.ndarray):
+        raise TypeError("ldiv_adjoint works on a device-resident factorisation (a CUDA tensor), not a numpy array")
+    loc = H.A.local if isinstance(H.A, ColumnBlockMatrix) else H.A
+    m, n = loc.shape[0], H.α.shape[0]
+    c = torch.as_tensor(c)
+    if c.is_complex() != loc.is_complex():
+        raise TypeError(f"c must have the element type of A ({loc.dtype})")
+    if c.dim() not in (1, 2) or c.shape[0] != n:
+        raise ValueError(f"c must have {n} rows (a length-n vector or an (n, k) block)")
+    if c.dim() == 1:
+        y = torch.empty(m, dtype=loc.dtype, device=loc.device)
+        y[:n] = c.to(device=loc.device, dtype=loc.dtype)
+    else:
+        y = colmajor_empty(m, c.shape[1], loc.device, dtype=loc.dtype)
+        y[:n] = c.to(device=loc.device, dtype=loc.dtype)
+    return solve_adjoint_(y, H.A, H.α, H.handle)
 
 
 def ldiv(H: DistributedHouseholderQRStruct, b):

@@ -138,7 +138,8 @@ struct dhqr_context {
     int panel_fast = 1;
     int bs_wave = 1;                                                    // back-substitution as one wavefront launch per right-hand side
     int bs_wave_max_ctas = 0;                                           // co-residency limit of k_backsolve_wave on this device
-    unsigned long long* bs_cells = nullptr; size_t bs_cells_blocks = 0; // x cells of the wavefront ([block][32][2 words])
+    int fs_wave_max_ctas = 0;                                           // ... and of k_forwardsolve_wave
+    unsigned long long* bs_cells = nullptr; size_t bs_cells_blocks = 0; // x cells of the wavefronts ([block][32][2 words])
     uint32_t bs_epoch = 0;
     int unblocked_wave = 1;                                             // nb = 1, m <= 8192: the column loop as one persistent launch
     unsigned int* uw_flags = nullptr; size_t uw_flags_n = 0; unsigned int uw_epoch = 0;
@@ -1315,6 +1316,37 @@ static int apply_qt_local_vec(dhqr_context* c, cudaStream_t st, int64_t m, int64
 }
 static bool qt_vec_ok(const dhqr_context* c, int64_t m, int nrhs) { return c->qt_vec && nrhs == 1 && m <= (int64_t)QT_MAXG * QT_MAXROWS; }
 
+// Set-up shared by both wavefront substitutions: the x cells for nl local unknowns (zeroed in stream order when they grow)
+// and the co-residency limit of each wave kernel on this device.
+static int wave_prepare(dhqr_context* c, cudaStream_t st, int64_t nl) {
+    if (c->bs_cells_blocks < (size_t)(nl + 31) / 32 + 1) {
+        if (c->bs_cells) CU(cudaFree(c->bs_cells));
+        c->bs_cells = nullptr;
+        c->bs_cells_blocks = (size_t)(nl + 31) / 32 + 64;
+        CU(cudaMalloc((void**)&c->bs_cells, c->bs_cells_blocks * 32 * 16));
+        CU(cudaMemsetAsync(c->bs_cells, 0, c->bs_cells_blocks * 32 * 16, st));
+        c->bs_epoch = 0;
+    }
+    if (!c->bs_wave_max_ctas) {
+        int per_sm = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_backsolve_wave, BW_THREADS, 0));
+        c->bs_wave_max_ctas = std::max(1, per_sm * c->sms);
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_forwardsolve_wave, BW_THREADS, 0));
+        c->fs_wave_max_ctas = std::max(1, per_sm * c->sms);
+    }
+    return 0;
+}
+
+// Tag of the next wave launch; the cells are cleared before the 32-bit tag could come round to a value they still hold.
+static int wave_tag(dhqr_context* c, cudaStream_t st, uint32_t* tag) {
+    if (c->bs_epoch > 0xFFFFFFF0u) {
+        CU(cudaMemsetAsync(c->bs_cells, 0, (size_t)c->bs_cells_blocks * 32 * 16, st));
+        c->bs_epoch = 0;
+    }
+    *tag = ++c->bs_epoch;
+    return 0;
+}
+
 static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64_t nl, const double* A, int64_t lda,
                            const double* alpha, double* y, int64_t ldy, int nrhs, double* x, int64_t ldx) {
     if (nl <= 0) return 0;
@@ -1322,12 +1354,10 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
     const int64_t nbk = (nl + 31) / 32, nlow = (col0 + 31) / 32;
     if (c->bs_wave && nbk + nlow <= c->bs_wave_max_ctas && nbk <= (int64_t)c->bs_cells_blocks) {
         for (int rhs = 0; rhs < nrhs; ++rhs) {
-            if (c->bs_epoch > 0xFFFFFFF0u) {
-                CU(cudaMemsetAsync(c->bs_cells, 0, (size_t)c->bs_cells_blocks * 32 * 16, st));
-                c->bs_epoch = 0;
-            }
+            uint32_t tag;
+            TRY(wave_tag(c, st, &tag));
             k_backsolve_wave<<<(unsigned)(nbk + nlow), BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx, col0, nl,
-                                                                          (int)nlow, c->bs_cells, ++c->bs_epoch);
+                                                                          (int)nlow, c->bs_cells, tag);
             TRY(post(c, st, "k_backsolve_wave"));
         }
         return 0;
@@ -1340,6 +1370,38 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
         k_backsolve_step<<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs);
         TRY(post(c, st, "k_backsolve_step"));
     }
+    return 0;
+}
+
+// y[0:n] <- R^{-T} y[0:n] on one GPU, through c->xbuf: the wavefront of k_forwardsolve_wave (first strip to last) when every CTA
+// fits on the device at once, otherwise (or with "bs_wave" = 0) blocks of BS_BLK columns, first to last, one k_forwardsolve_step
+// each.  Every CTA of a step reads the block's y, so z goes to xbuf and is copied back at the end, as in the back-substitution.
+static int forwardsolve_local(dhqr_context* c, cudaStream_t st, int64_t n, const double* A, int64_t lda, const double* alpha,
+                              double* y, int64_t ldy, int nrhs) {
+    if (n <= 0 || nrhs <= 0) return 0;
+    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n * nrhs, st));
+    TRY(wave_prepare(c, st, n));
+    double* x = c->xbuf;
+    const int64_t ldx = n, nbk = (n + 31) / 32;
+    if (c->bs_wave && nbk <= c->fs_wave_max_ctas && nbk <= (int64_t)c->bs_cells_blocks) {
+        for (int rhs = 0; rhs < nrhs; ++rhs) {
+            uint32_t tag;
+            TRY(wave_tag(c, st, &tag));
+            pre(c, st);
+            k_forwardsolve_wave<<<(unsigned)nbk, BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx, n,
+                                                                     c->bs_cells, tag);
+            TRY(post(c, st, "k_forwardsolve_wave"));
+        }
+    } else {
+        for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
+            const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
+            const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
+            pre(c, st);
+            k_forwardsolve_step<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs, n);
+            TRY(post(c, st, "k_forwardsolve_step"));
+        }
+    }
+    CU(cudaMemcpy2DAsync(y, (size_t)ldy * 8, x, (size_t)ldx * 8, (size_t)n * 8, nrhs, cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 
@@ -1665,19 +1727,7 @@ int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     TRY(gather_partition(c, st, col0, n_local, col0s, nls));
     TRY(check_partition(col0s, nls, n_global));
     TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n_global * nrhs, st));
-    if (c->bs_cells_blocks < (size_t)(n_local + 31) / 32 + 1) {
-        if (c->bs_cells) CU(cudaFree(c->bs_cells));
-        c->bs_cells = nullptr;
-        c->bs_cells_blocks = (size_t)(n_local + 31) / 32 + 64;
-        CU(cudaMalloc((void**)&c->bs_cells, c->bs_cells_blocks * 32 * 16));
-        CU(cudaMemsetAsync(c->bs_cells, 0, c->bs_cells_blocks * 32 * 16, st));
-        c->bs_epoch = 0;
-    }
-    if (!c->bs_wave_max_ctas) {
-        int per_sm = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_backsolve_wave, BW_THREADS, 0));
-        c->bs_wave_max_ctas = std::max(1, per_sm * c->sms);
-    }
+    TRY(wave_prepare(c, st, n_local));
     // C4 (S:260-267), column oriented: the last owner solves its block of unknowns and removes their
     // contribution from the rows above; the partially reduced right-hand side then moves one rank down.
     const size_t cnt = (size_t)ldb * (nrhs - 1) + n_global;
@@ -1917,6 +1967,105 @@ int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t
                                   false, nullptr, 0, 1));
     }
     return 0;
+}
+
+// ---- solves with the adjoint (LAPACK ?gels, TRANS = 'C') ------------------------------------------------------------------
+// forwardsolve: b[0:n] <- R^{-H} b[0:n].  solve_adj: the minimum-norm solution of A^H y = c, y = Q [R^{-H} c; 0]: forward
+// substitution on rows [0, n), zero rows [n, m), then b <- H_1 ... H_n b.  Single GPU.
+static int check_adj(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* alpha, const void* b, int64_t ldb,
+                     int nrhs, bool cplx) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the adjoint solves are single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (n > 0 && !A) return set_err(-4, "null A");
+    if (cplx) TRY(check_c64_ptr(A, -4, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
+    if (n > 0 && !alpha) return set_err(-6, "null alpha");
+    if (cplx) TRY(check_c64_ptr(alpha, -6, "alpha"));
+    if (nrhs > 0 && !b) return set_err(-7, "null b");
+    if (cplx) TRY(check_c64_ptr(b, -7, "b"));
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-8, "ldb < max(1,m)");
+    if (nrhs < 0) return set_err(-9, "nrhs < 0");
+    return 0;
+}
+
+// complex y[0:n] <- R^{-H} y[0:n], blocks of BS_BLK columns first to last, through c->xbuf
+static int forwardsolve_c64_local(dhqr_context* c, cudaStream_t st, int64_t n, const double2* A, int64_t lda, const double2* alpha,
+                                  double2* y, int64_t ldy, int nrhs) {
+    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)2 * n * nrhs, st));
+    double2* x = (double2*)c->xbuf;
+    for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
+        const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
+        pre(c, st);
+        k_forwardsolve_step_c<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, n, c0, bs, n);
+        TRY(post(c, st, "k_forwardsolve_step_c"));
+    }
+    CU(cudaMemcpy2DAsync(y, (size_t)ldy * 16, x, (size_t)n * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+// complex b <- Q b = H_1 ... H_n b: the panel loop of dhqr_apply_qt_c64 run backwards, each panel as I - V T V' (T, not T')
+static int apply_q_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b,
+                             int64_t ldb, int nrhs) {
+    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
+    for (int64_t c0 = ((n - 1) / CPW) * CPW; c0 >= 0; c0 -= CPW) {
+        const int kb = (int)std::min<int64_t>(CPW, n - c0);
+        const int64_t mpc = m - c0, rows = 2 * mpc, vrows = rup(rows, 128);
+        TRY(pack_complex_panel(c, st, A + c0 * lda + c0, lda, mpc, kb, vrows));
+        TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, (double*)(b + c0), 2 * ldb, nrhs, false, nullptr, 0, 1));
+    }
+    return 0;
+}
+
+int dhqr_forwardsolve_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
+                          int64_t ldb, int nrhs, void* stream) {
+    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, false));
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return forwardsolve_local(c, (cudaStream_t)stream, n, dA, lda, d_alpha, d_b, ldb, nrhs);
+}
+
+int dhqr_forwardsolve_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b,
+                          int64_t ldb, int nrhs, void* stream) {
+    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, true));
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return forwardsolve_c64_local(c, (cudaStream_t)stream, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs);
+}
+
+int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
+                       int64_t ldb, int nrhs, void* stream) {
+    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, false));
+    if (m == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(forwardsolve_local(c, st, n, dA, lda, d_alpha, d_b, ldb, nrhs));
+    if (m > n) CU(cudaMemset2DAsync(d_b + n, (size_t)ldb * 8, 0, (size_t)(m - n) * 8, nrhs, st));    // n = 0: y = 0, as in ?gels
+    if (n == 0) return 0;
+    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
+    if (qt_vec_ok(c, m, nrhs)) {
+        TRY(qt_prepare(c, st, m, 0, n, dA, lda));
+        TRY(apply_qt_local_vec(c, st, m, 0, n, dA, lda, d_b, 1));
+    } else {
+        TRY(apply_qt_local(c, st, m, 0, n, dA, lda, d_b, ldb, nrhs, 1));
+    }
+    return 0;
+}
+
+int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
+                       int nrhs, void* stream) {
+    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, true));
+    if (m == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    const double2* A = (const double2*)dA;
+    double2* b = (double2*)d_b;
+    if (n > 0) TRY(forwardsolve_c64_local(c, st, n, A, lda, (const double2*)d_alpha, b, ldb, nrhs));
+    if (m > n) CU(cudaMemset2DAsync(b + n, (size_t)ldb * 16, 0, (size_t)(m - n) * 16, nrhs, st));
+    if (n == 0) return 0;
+    return apply_q_c64_local(c, st, m, n, A, lda, b, ldb, nrhs);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

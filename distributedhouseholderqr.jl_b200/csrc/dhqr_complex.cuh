@@ -146,6 +146,61 @@ __global__ void __launch_bounds__(256) k_backsolve_step_c(const double2* __restr
     }
 }
 
+// n / conj(a) by Smith's algorithm: the ratio of the smaller to the larger part of a is formed first, so neither |a|^2 nor a
+// partial product overflows or underflows when n and a lie many decades apart (columns scaled by 10^+-120).  a = 0 gives NaN.
+__device__ __forceinline__ double2 cdiv_conj(double2 n, double2 a) {
+    const double p = a.x, q = -a.y;                                          // conj(a) = p + i q
+    if (fabs(p) >= fabs(q)) {
+        const double r = q / p, d = p + q * r;
+        return make_double2((n.x + n.y * r) / d, (n.y - n.x * r) / d);
+    }
+    const double r = p / q, d = q + p * r;
+    return make_double2((n.x * r + n.y) / d, (n.y * r - n.x) / d);
+}
+
+// forward substitution with R^H (z = R^{-H} y) for complex R = triu(A,1) + diag(alpha): like k_forwardsolve_step, with the
+// conjugated products z_i = (y_i - sum_{j<i} conj(R[j,i]) z_j) / conj(alpha_i)
+__global__ void __launch_bounds__(256, 1) k_forwardsolve_step_c(const double2* __restrict__ A, int64_t lda, const double2* __restrict__ alpha,
+                                                             double2* __restrict__ y, int64_t ldy, int nrhs, double2* __restrict__ x,
+                                                             int64_t ldx, int64_t c0, int bs, int64_t n) {
+    __shared__ double2 sx[BS_BLK], sD[BS_BLK][BS_BLK + 1];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int e = tid; e < BS_BLK * BS_BLK; e += 256) {                      // sD[j][i] = R[c0 + i, c0 + j], i < j: column j of A
+        const int i = e & 31, j = e >> 5;
+        sD[j][i] = (i < j && j < bs) ? A[(c0 + j) * lda + c0 + i] : make_double2(0.0, 0.0);
+    }
+    __syncthreads();
+    for (int rhs = 0; rhs < nrhs; ++rhs) {
+        double2* yr = y + (int64_t)rhs * ldy;
+        if (tid < 32) {
+            double2 yk = lane < bs ? yr[c0 + lane] : make_double2(0.0, 0.0);
+            for (int i = 0; i < bs; ++i) {
+                const double nx = __shfl_sync(0xffffffffu, yk.x, i), ny = __shfl_sync(0xffffffffu, yk.y, i);
+                const double2 zi = cdiv_conj(make_double2(nx, ny), alpha[c0 + i]);
+                if (lane == i) yk = zi;
+                if (lane > i) {
+                    const double2 t = cmulc(sD[lane][i], zi);
+                    yk.x -= t.x;
+                    yk.y -= t.y;
+                }
+            }
+            sx[lane] = yk;
+        }
+        __syncthreads();
+        if (blockIdx.x == 0 && tid < bs) x[(int64_t)rhs * ldx + c0 + tid] = sx[tid];
+        const double2 zl = lane < bs ? sx[lane] : make_double2(0.0, 0.0);
+        for (int64_t r = c0 + bs + (int64_t)blockIdx.x * 8 + warp; r < n; r += (int64_t)gridDim.x * 8) {
+            const double2 t = lane < bs ? cmulc(A[r * lda + c0 + lane], zl) : make_double2(0.0, 0.0);
+            const double sre = warp_sum(t.x), sim = warp_sum(t.y);
+            if (lane == 0) {
+                yr[r].x -= sre;
+                yr[r].y -= sim;
+            }
+        }
+        __syncthreads();
+    }
+}
+
 // partialdot(a, b, is, ::Type{<:Complex}) (S:51-59): sum conj(a[i]) b[i] over [i0, i1); one CTA.
 __global__ void __launch_bounds__(1024, 1) k_partialdot_c(const double2* __restrict__ x, const double2* __restrict__ y, int64_t i0,
                                                           int64_t i1, double2* __restrict__ out) {

@@ -172,4 +172,40 @@ function apply_q!(b::CuVecOrMat{Float64}, A::CuMatrix{Float64})
     return b
 end
 
+# ---- solves with the adjoint (LAPACK ?gels with TRANS = 'C'; not in the reference), single GPU ----
+for (T, fs, sa) in ((Float64, :dhqr_forwardsolve_f64, :dhqr_solve_adj_f64), (ComplexF64, :dhqr_forwardsolve_c64, :dhqr_solve_adj_c64))
+    @eval begin
+        adj_call(::Val{:forward}, A::CuMatrix{$T}, α::CuVector{$T}, b::CuVecOrMat{$T}) =
+            GC.@preserve A α b check($(QuoteNode(fs)), ccall(($(QuoteNode(fs)), libdhqr), Cint,
+                (Ptr{Cvoid}, Int64, Int64, CuPtr{$T}, Int64, CuPtr{$T}, CuPtr{$T}, Int64, Cint, Ptr{Cvoid}),
+                handle().ptr, size(A, 1), size(A, 2), pointer(A), stride(A, 2), pointer(α), pointer(b), max(stride(b, 2), size(A, 1)),
+                size(b, 2), stream_ptr()))
+        adj_call(::Val{:solve}, A::CuMatrix{$T}, α::CuVector{$T}, b::CuVecOrMat{$T}) =
+            GC.@preserve A α b check($(QuoteNode(sa)), ccall(($(QuoteNode(sa)), libdhqr), Cint,
+                (Ptr{Cvoid}, Int64, Int64, CuPtr{$T}, Int64, CuPtr{$T}, CuPtr{$T}, Int64, Cint, Ptr{Cvoid}),
+                handle().ptr, size(A, 1), size(A, 2), pointer(A), stride(A, 2), pointer(α), pointer(b), max(stride(b, 2), size(A, 1)),
+                size(b, 2), stream_ptr()))
+    end
+end
+
+# b[1:n, :] <- R^{-H} b[1:n, :] (rows n+1:m untouched); returns that view
+function forwardsolve!(b::CuVecOrMat{T}, A::CuMatrix{T}, α::CuVector{T}) where {T<:Union{Float64,ComplexF64}}
+    adj_call(Val(:forward), A, α, b)
+    return b isa CuVector ? view(b, 1:size(A, 2)) : view(b, 1:size(A, 2), :)
+end
+
+# H' \ c: the minimum-norm solution y = Q [R^{-H} c; 0] of A^H y = c (dhqr_solve_adj_*); c (length n, or n x k) is not modified
+struct AdjointQR{S<:DistributedHouseholderQRStruct}
+    parent::S
+end
+Base.adjoint(H::DistributedHouseholderQRStruct{<:CuMatrix}) = AdjointQR(H)
+function LinearAlgebra.:(\)(Ha::AdjointQR, c::AbstractVecOrMat)
+    A = Ha.parent.A; T = eltype(A); m, n = size(A)
+    size(c, 1) == n || throw(DimensionMismatch("c must have $n rows"))
+    y = CUDA.zeros(T, m, size(c, 2))
+    y[1:n, :] .= CuArray{T}(reshape(c, n, :))
+    adj_call(Val(:solve), A, Ha.parent.α, y)
+    return c isa AbstractVector ? vec(y) : y
+end
+
 end # module

@@ -27,7 +27,8 @@
  *     (iv) workspace growth (first call, or a larger problem than any before) allocates device memory.
  *     Everything else returns without synchronising.  Any caller stream works, non-blocking and prioritised ones
  *     included: the library depends on no stream but the caller's (workspace zero fills included; its internal streams
- *     fork from and join back to the caller's stream with events).  tests/test_gpu_streams.py holds every entry point to this.
+ *     fork from and join back to the caller's stream with events).  tests/test_gpu_streams.py and tests/test_gpu_adjoint.py
+ *     (the adjoint solves) hold every entry point to this.
  *   - no pointer to caller memory is retained after return; workspace lives in the handle.
  *   - a handle is not thread-safe and its calls share one workspace: one handle per host thread, and
  *     consecutive calls on one handle must be on the same stream or ordered by the caller (events);
@@ -86,9 +87,10 @@ int dhqr_destroy(dhqr_handle h);
  *                 "host_trace" 1: stage timeline on stderr.  A wrong assumption costs idle time, never correctness
  *   "sync"        1: cudaStreamSynchronize + error check after every kernel launch (debugging; implies serial)
  *   "profile"     1: CUDA-event bracket per launch (implies serial), read with dhqr_profile_get
- *   "bs_wave", "unblocked_wave", "fuse_house"  1 (default): back-substitution as one wavefront launch, nb = 1 as one persistent
- *                 launch (m <= 8192), nb = 1 with the next reflector formed inside the apply kernel, where the shape allows;
- *                 0: the per-block / per-column launches those paths otherwise take
+ *   "bs_wave", "unblocked_wave", "fuse_house"  1 (default): back-substitution (and the Float64 forward substitution of
+ *                 dhqr_forwardsolve_f64 / dhqr_solve_adj_f64) as one wavefront launch per right-hand side where all its CTAs fit
+ *                 on the device, nb = 1 as one persistent launch (m <= 8192), nb = 1 with the next reflector formed inside the
+ *                 apply kernel, where the shape allows; 0: the per-block / per-column launches those paths otherwise take
  *   "wide_kappa"  guard of the 128-column chain on ||D R1^{-1}||_F of its first Cholesky factor (default 1000)
  *   traces:       "panel_trace", "la_trace", "wide_trace" (timestamps read with dhqr_debug_copy_f64)
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
@@ -174,6 +176,28 @@ int dhqr_form_q_f64(dhqr_handle h, int64_t m, int64_t n, const double *dA, int64
 /* ComplexF64: interleaved (re, im); lda, ldq in complex elements.  Q = H_1 ... H_n with H_j = I - v_j v_j^H. */
 int dhqr_form_q_c64(dhqr_handle h, int64_t m, int64_t n, const void *dA, int64_t lda, void *dQ, int64_t ldq,
                     void *stream);
+
+/* ---- solves with the adjoint (not in the reference; SURVEY 8f-3: LAPACK ?gels with TRANS = 'C', full rank) -------------------
+ * From a factorisation A = QR (dA, lda, d_alpha) in the library's storage format, R = triu(A, 1) + diag(alpha), any path.
+ * d_b: m x nrhs, ldb >= max(1, m), in place.  Single GPU (a handle with nranks > 1 returns -1).  Stream-ordered, no
+ * synchronisation apart from workspace growth (point (iv)).  Nothing outside the m x nrhs operand b is written; A and alpha
+ * never are.  A zero entry of alpha divides by zero and propagates Inf / NaN, as in dhqr_backsolve_*.
+ * Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 null A with n > 0, -5 lda < max(1, m), -6 null alpha
+ * with n > 0, -7 null b with nrhs > 0, -8 ldb < max(1, m), -9 nrhs < 0; the _c64 functions also return -4 / -6 / -7 for an A,
+ * alpha or b that is only 8 B aligned.  Every check runs before anything is enqueued.
+ *
+ * b[0:n, :] <- R^{-H} b[0:n, :] (R^{-T} for Float64): forward substitution with the lower-triangular R^H.  Rows n..m-1 of b are
+ * neither read nor written.  n = 0 is a no-op. */
+int dhqr_forwardsolve_f64(dhqr_handle h, int64_t m, int64_t n, const double *dA, int64_t lda, const double *d_alpha,
+                          double *d_b, int64_t ldb, int nrhs, void *stream);
+int dhqr_forwardsolve_c64(dhqr_handle h, int64_t m, int64_t n, const void *dA, int64_t lda, const void *d_alpha, void *d_b,
+                          int64_t ldb, int nrhs, void *stream);
+/* Minimum-norm solution of A^H y = c: on entry c = b[0:n, :]; on return y = b[0:m, :] = Q [R^{-H} c; 0].  n = 0 sets the
+ * m x nrhs block of b to zero (the minimum-norm solution of an empty system, as in ?gels). */
+int dhqr_solve_adj_f64(dhqr_handle h, int64_t m, int64_t n, const double *dA, int64_t lda, const double *d_alpha, double *d_b,
+                       int64_t ldb, int nrhs, void *stream);
+int dhqr_solve_adj_c64(dhqr_handle h, int64_t m, int64_t n, const void *dA, int64_t lda, const void *d_alpha, void *d_b,
+                       int64_t ldb, int nrhs, void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
