@@ -41,6 +41,8 @@ SIGNATURES = {
     "dhqr_forwardsolve_c64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
     "dhqr_solve_adj_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
     "dhqr_solve_adj_c64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _int, _vp],
+    "dhqr_qrcp_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
+    "dhqr_solve_qrcp_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _int, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

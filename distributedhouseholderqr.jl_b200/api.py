@@ -507,6 +507,85 @@ def ldiv(H: DistributedHouseholderQRStruct, b):
     return x.clone()                                                              # S:320
 
 
+# --------------------------------------------------------------------------------------------
+# QR with column pivoting (LAPACK dgeqp3) and the basic least-squares solution (dgelsy without the complete orthogonal
+# decomposition); scipy.linalg.qr(pivoting=True) / Julia's qr(A, ColumnNorm())
+# --------------------------------------------------------------------------------------------
+class PivotedHouseholderQRStruct:
+    """A P = Q R from ``qrcp_``: ``.A`` (the caller's storage, factored in place) and ``.α`` (``.alpha``) are the factorisation of
+    ``A[:, p]`` in the library's storage format, so every other entry point (apply_qt_, apply_q_, backsolve_, form_q,
+    forwardsolve_) takes them as that; ``.p`` is an int64 device tensor, ``p[k]`` = original index of the k-th column."""
+
+    def __init__(self, A, alpha, p, handle: Optional[Handle] = None):
+        self.A = A
+        self.α = alpha
+        self.p = p
+        self.handle = handle
+
+    @property
+    def alpha(self):
+        return self.α
+
+    def rank(self, rcond: Optional[float] = None) -> int:
+        """Numerical rank: the first k with |α_k| <= rcond |α_0| (n if there is none).  Default rcond = max(m, n) eps.  Reads α,
+        so it synchronises with the stream the factorisation ran on."""
+        m, n = self.A.shape[0], self.α.shape[0]
+        if n == 0:
+            return 0
+        if rcond is None:
+            rcond = max(m, n) * float(np.finfo(np.float64).eps)
+        a = self.α.abs().cpu().numpy()
+        small = np.nonzero(~(a > rcond * a[0]))[0]
+        return int(small[0]) if small.size else n
+
+    def ldiv(self, b, rcond: Optional[float] = None):
+        """The basic solution x of min ||A x - b|| at rank ``self.rank(rcond)``; returns (x, rank).  Neither the factorisation nor
+        b is modified.  ``b``: length m, or (m, k)."""
+        r = self.rank(rcond)
+        loc = self.A
+        if b.dim() == 1:
+            s = b.to(device=loc.device, dtype=loc.dtype).clone()
+        else:
+            s = to_colmajor(b, device=loc.device)
+        solve_qrcp_(s, self.A, self.α, self.p, r, self.handle)
+        return s[:loc.shape[1]].clone(), r
+
+    solve = ldiv
+
+
+def qrcp_(A: torch.Tensor, handle: Optional[Handle] = None) -> PivotedHouseholderQRStruct:
+    """A P = Q R with column pivoting (LAPACK dgeqp3; scipy.linalg.qr(pivoting=True)), in place, on a column-major float64 CUDA
+    tensor with n <= m.  Single GPU, stream-ordered, no synchronisation."""
+    if not isinstance(A, torch.Tensor) or not A.is_cuda:
+        raise TypeError("qrcp_ works on a column-major float64 CUDA tensor")
+    if A.dtype != torch.float64:
+        raise TypeError("qrcp_ is Float64 only")
+    h = handle or default_handle(A.device.index)
+    m, n = A.shape
+    alpha = torch.zeros(n, dtype=torch.float64, device=A.device)
+    p = torch.zeros(n, dtype=torch.int64, device=A.device)
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_qrcp_f64", h.raw, m, n, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+                  C.c_void_p(p.data_ptr()), _stream_ptr(A.device))
+    return PivotedHouseholderQRStruct(A, alpha, p, h)
+
+
+def solve_qrcp_(b: torch.Tensor, A: torch.Tensor, alpha: torch.Tensor, p: torch.Tensor, rank: int,
+                handle: Optional[Handle] = None) -> torch.Tensor:
+    """x = P [R11^{-1} (Q'b)[0:rank]; 0], the basic solution at the given rank, from a factorisation made by ``qrcp_``.  ``b``:
+    length m, or (m, k) column-major; on return b[0:n] = x (returned as a view) and rows n..m-1 hold rows n..m-1 of
+    H_rank ... H_1 b."""
+    h = handle or default_handle(A.device.index)
+    m, n = A.shape
+    if alpha.dtype != torch.float64 or p.dtype != torch.int64:
+        raise TypeError("alpha must be float64 and p int64")
+    ldb, nrhs = _rhs_args(b, m, A.dtype)
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_solve_qrcp_f64", h.raw, m, n, int(rank), C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+                  C.c_void_p(p.data_ptr()), C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(A.device))
+    return b[:n]
+
+
 def partialdot(a: torch.Tensor, b: torch.Tensor, rng, handle: Optional[Handle] = None):
     """partialdot(a, b, is, ::Type{<:Real}) (S:42-49) / ::Type{<:Complex} (S:51-59: sum conj(a[i]) b[i]); ``rng`` is a
     0-based Python range."""

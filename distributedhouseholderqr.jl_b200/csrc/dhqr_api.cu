@@ -17,6 +17,7 @@
 #include "dhqr_kernels.cuh"
 #include "dhqr_wide.cuh"
 #include "dhqr_complex.cuh"
+#include "dhqr_qrcp.cuh"
 
 using namespace dhqr;
 
@@ -160,6 +161,11 @@ struct dhqr_context {
     int qt_vec = 1;                                                     // option: use it (0: the GEMM-shaped block update also for one right-hand side)
     double* v1 = nullptr;    size_t v1_elems = 0;                       // unblocked path: v
     double* xbuf = nullptr;  size_t xbuf_elems = 0;                     // back-substitution output
+    // pivoted factorisation (dhqr_qrcp.cuh): vn1, vn2, F, the column in flight and the partials of both reductions; renorm
+    // flags; scalars of the reflector in flight, the pivot ticket and the renorm counter
+    double* qp_buf = nullptr; size_t qp_buf_elems = 0;
+    int* qp_flag = nullptr;  size_t qp_flag_elems = 0;
+    QrcpCtl* qp_ctl = nullptr;
     double* hostA = nullptr; size_t hostA_elems = 0;                    // device staging for _host_ entry points
     double* hostB = nullptr; size_t hostB_elems = 0;
     int64_t* d_i64 = nullptr;                                           // small int64 scratch (partition exchange)
@@ -356,6 +362,9 @@ static int pick_splits(int tiles, int nchunks, int sms, int64_t cap_tiles) {
     return best;
 }
 
+static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int voff, int nbp, const double* ypk, int64_t rows,
+                      int64_t row_lo, double* C, int64_t ldc, int ncols, int gate);
+
 // block-reflector application  C <- (I - V T' V') C  on window rows >= row_lo
 //   V = packed columns [voff, voff + nbp) of `vpk` (columns beyond the live ones are zero); T from the
 //   Gram matrix; `w` = the workspace set of the calling chain.
@@ -410,10 +419,19 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
         else k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans);
         TRY(post(c, st, small ? "k_ymake32" : "k_ymake128"));
     }
+    return launch_cvy(c, st, vpk, voff, nbp, w.ypk, rows, row_lo, C, ldc, ncols, gate);
+}
+
+// C += V Y on window rows >= row_lo, Y packed in the ypk layout (nbp <= 32: one k-chunk per column tile; else NBMAX / KC):
+// the second half of a block-reflector application, also fed a Y made elsewhere (the pivoted factorisation's -F')
+static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int voff, int nbp, const double* ypk, int64_t rows,
+                      int64_t row_lo, double* C, int64_t ldc, int ncols, int gate) {
+    const bool small = (nbp <= 32);
+    const int NBPK = small ? 32 : 128;
     pre(c, st);
     GemmCvyArgs g2;
     g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.row_lo = row_lo; g2.ncols = ncols;
-    g2.vpk = vpk; g2.voff = voff; g2.ypk = w.ypk;
+    g2.vpk = vpk; g2.voff = voff; g2.ypk = ypk;
     g2.nkq = small ? 1 : (int)(rup(nbp, KC) / KC); g2.nkq_alloc = NBPK / KC;
     g2.ctl = c->wctl; g2.gate = gate;
     dim3 grid2((unsigned)((rows + G2_BM - 1) / G2_BM), (unsigned)((ncols + G2_BN - 1) / G2_BN));
@@ -1492,6 +1510,7 @@ int dhqr_destroy(dhqr_handle c) {
     if (c->aux_stream) cudaStreamDestroy(c->aux_stream);
     for (int i = 0; i < 4; ++i)
         if (c->ev_aux[i]) cudaEventDestroy(c->ev_aux[i]);
+    cudaFree(c->qp_buf); cudaFree(c->qp_flag); cudaFree(c->qp_ctl);
     cudaFree(c->v1); cudaFree(c->xbuf); cudaFree(c->hostA); cudaFree(c->hostB); cudaFree(c->d_i64);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     if (c->d2h_stream) cudaStreamDestroy(c->d2h_stream);
@@ -1594,6 +1613,11 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
     else if (!strcmp(key, "wide_panels")) *value = c->wide_panels;
     else if (!strcmp(key, "wide_redone")) *value = c->wide_redone;
     else if (!strcmp(key, "pair_units")) *value = c->pair_units;
+    else if (!strcmp(key, "qrcp_renorms")) {
+        unsigned long long r = 0;
+        if (c->qp_ctl) CU(cudaMemcpy(&r, &c->qp_ctl->renorms, sizeof(r), cudaMemcpyDeviceToHost));
+        *value = (int64_t)r;
+    }
     else if (!strcmp(key, "panels_fast") || !strcmp(key, "panels_fallback")) {
         int st2[2] = {0, 0};
         if (c->fast_stats) CU(cudaMemcpy(st2, c->fast_stats, sizeof(st2), cudaMemcpyDeviceToHost));
@@ -2066,6 +2090,138 @@ int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int6
     if (m > n) CU(cudaMemset2DAsync(b + n, (size_t)ldb * 16, 0, (size_t)(m - n) * 16, nrhs, st));
     if (n == 0) return 0;
     return apply_q_c64_local(c, st, m, n, A, lda, b, ldb, nrhs);
+}
+
+// ---- QR with column pivoting (LAPACK dgeqp3 / dlaqps, dhqr_qrcp.cuh) -------------------------------------------------------
+// Panels of QP_NB columns, four launches per column, then the trailing update A[k0+32:, k0+32:] -= V F' through the 32-wide
+// C += V Y kernel.  A column whose norm downdate fails LAPACK's tol3z test is renormed exactly inside the panel, before the
+// next pivot is chosen, instead of ending the panel early: every panel has its static width and the host never needs a device
+// value, so the driver is one static loop and the call does not synchronise.  Single GPU, n <= m, no row limit.
+static int check_qrcp_ptr(const void* p, int arg, const char* name) {
+    if (((uintptr_t)p & 7) != 0) return set_err(arg, "%s must be 8 B aligned", name);
+    return 0;
+}
+
+static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double* A, int64_t lda, double* alpha, int64_t* jpvt) {
+    TRY(ensure_workspace(c, st, m, n));
+    const int64_t p1 = (m + QP_PROWS - 1) / QP_PROWS;                                    // k_qrcp_pivot CTAs
+    const int64_t smax = std::max<int64_t>(1, std::min<int64_t>((m + QP_THREADS - 1) / QP_THREADS, 8 * c->sms));
+    const size_t need = (size_t)2 * n + (size_t)QP_NB * n + (size_t)m + (size_t)p1 + (size_t)smax * n;
+    TRY(ensure(&c->qp_buf, &c->qp_buf_elems, need, st));
+    TRY(ensure(&c->qp_flag, &c->qp_flag_elems, (size_t)n, st));
+    if (!c->qp_ctl) {
+        CU(cudaMalloc((void**)&c->qp_ctl, sizeof(QrcpCtl)));
+        CU(cudaMemsetAsync(c->qp_ctl, 0, sizeof(QrcpCtl), st));
+    }
+    QrcpArgs a;
+    a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
+    a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = a.vn2 + n; a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
+    a.part1 = a.x + m; a.part2 = a.part1 + p1; a.ldp = n;
+    pre(c, st);
+    k_qrcp_init<<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
+    TRY(post(c, st, "k_qrcp_init", 8.0 * (double)m * n));
+    for (int64_t k0 = 0; k0 < n; k0 += QP_NB) {
+        const int kb = (int)std::min<int64_t>(QP_NB, n - k0);
+        const int tiles = (int)((n - k0 + QP_GCOLS - 1) / QP_GCOLS);
+        for (int jj = 0; jj < kb; ++jj) {
+            const int64_t j = k0 + jj, rows = m - j;
+            a.j = j; a.k0 = k0; a.jj = jj;
+            pre(c, st);
+            k_qrcp_pivot<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
+            TRY(post(c, st, "k_qrcp_pivot", 8.0 * ((double)m * 4 + (double)rows * (jj + 1) + (double)(n - j))));
+            // row splits: about eight CTAs per SM in all, at least QP_THREADS rows each
+            const int64_t s = std::max<int64_t>(1, std::min<int64_t>((rows + QP_THREADS - 1) / QP_THREADS,
+                                                                     (8 * (int64_t)c->sms + tiles - 1) / tiles));
+            a.split_rows = rup((rows + s - 1) / s, QP_THREADS);
+            a.nsplit = (int)((rows + a.split_rows - 1) / a.split_rows);
+            pre(c, st);
+            k_qrcp_gemv<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
+            TRY(post(c, st, "k_qrcp_gemv", 8.0 * (double)rows * (double)(n - k0)));
+            if (j + 1 >= n) continue;
+            pre(c, st);
+            k_qrcp_finish<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
+            TRY(post(c, st, "k_qrcp_finish"));
+            pre(c, st);
+            k_qrcp_renorm<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
+            TRY(post(c, st, "k_qrcp_renorm"));
+        }
+        const int64_t c1 = k0 + kb;
+        if (c1 >= n) break;
+        // A[c1:, c1:] -= V F'  on the window starting at row k0 (a multiple of 32), rows >= c1 only
+        const int64_t wrows = m - k0, vrows = rup(wrows, 128);
+        const int ncols = (int)(n - c1);
+        pre(c, st);
+        dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), QP_NB);
+        k_pack<<<grid, 256, 0, st>>>(A + k0 * lda + k0, lda, wrows, kb, 1, c->vpk2[0], 0, 0, vrows);
+        TRY(post(c, st, "k_pack"));
+        const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * YT * LDK;
+        pre(c, st);
+        k_qrcp_ypack<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(a.F, a.ldf, c1, ncols, kb, c->ws[0].ypk);
+        TRY(post(c, st, "k_qrcp_ypack"));
+        TRY(launch_cvy(c, st, c->vpk2[0], 0, QP_NB, c->ws[0].ypk, wrows, kb, A + c1 * lda + k0, lda, ncols, 0));
+    }
+    return 0;
+}
+
+int dhqr_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, double* dA, int64_t lda, double* d_alpha, int64_t* d_jpvt, void* stream) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the pivoted factorisation is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (n > 0 && !dA) return set_err(-4, "null A");
+    TRY(check_qrcp_ptr(dA, -4, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
+    if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
+    TRY(check_qrcp_ptr(d_alpha, -6, "alpha"));
+    if (n > 0 && !d_jpvt) return set_err(-7, "null jpvt");
+    TRY(check_qrcp_ptr(d_jpvt, -7, "jpvt"));
+    if (n == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return qrcp_local(c, (cudaStream_t)stream, m, n, dA, lda, d_alpha, d_jpvt);
+}
+
+int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha,
+                        const int64_t* d_jpvt, double* d_b, int64_t ldb, int nrhs, void* stream) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the pivoted solve is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
+    if (n > 0 && !dA) return set_err(-5, "null A");
+    TRY(check_qrcp_ptr(dA, -5, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
+    if (n > 0 && !d_alpha) return set_err(-7, "null alpha");
+    TRY(check_qrcp_ptr(d_alpha, -7, "alpha"));
+    if (n > 0 && !d_jpvt) return set_err(-8, "null jpvt");
+    TRY(check_qrcp_ptr(d_jpvt, -8, "jpvt"));
+    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
+    TRY(check_qrcp_ptr(d_b, -9, "b"));
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
+    if (nrhs < 0) return set_err(-11, "nrhs < 0");
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
+    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n * nrhs, st));
+    if (rank > 0) {
+        // (Q'b)[0:rank] needs only the first `rank` reflectors
+        if (qt_vec_ok(c, m, nrhs)) {
+            TRY(qt_prepare(c, st, m, 0, rank, dA, lda));
+            TRY(apply_qt_local_vec(c, st, m, 0, rank, dA, lda, d_b, 0));
+        } else {
+            TRY(apply_qt_local(c, st, m, 0, rank, dA, lda, d_b, ldb, nrhs));
+        }
+        TRY(wave_prepare(c, st, rank));
+        TRY(backsolve_local(c, st, 0, rank, dA, lda, d_alpha, d_b, ldb, nrhs, c->xbuf, rank));
+    }
+    for (int r0 = 0; r0 < nrhs; r0 += 65535) {
+        const int nr = std::min(nrhs - r0, 65535);
+        pre(c, st);
+        k_qrcp_scatter<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(c->xbuf + (size_t)r0 * rank, rank, d_jpvt, n, rank,
+                                                                                     d_b + (size_t)r0 * ldb, ldb);
+        TRY(post(c, st, "k_qrcp_scatter"));
+    }
+    return 0;
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

@@ -208,4 +208,40 @@ function LinearAlgebra.:(\)(Ha::AdjointQR, c::AbstractVecOrMat)
     return c isa AbstractVector ? vec(y) : y
 end
 
+# ---- QR with column pivoting (LAPACK dgeqp3; not in the reference), Float64, single GPU ----
+# A[:, p] = Q R: (A, α) is the factorisation of A[:, p] in the storage format above; p is 1-based here, 0-based on the device
+struct PivotedHouseholderQRStruct{T1, T2, T3}
+    A::T1
+    α::T2
+    jpvt::T3          # CuVector{Int64}, 0-based
+end
+function qr!(A::CuMatrix{Float64}, ::ColumnNorm)
+    m, n = size(A)
+    α = CUDA.zeros(Float64, n); jpvt = CUDA.zeros(Int64, n)
+    GC.@preserve A α jpvt check(:dhqr_qrcp_f64, ccall((:dhqr_qrcp_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Int64}, Ptr{Cvoid}),
+        handle().ptr, m, n, pointer(A), stride(A, 2), pointer(α), pointer(jpvt), stream_ptr()))
+    return PivotedHouseholderQRStruct(A, α, jpvt)
+end
+Base.getproperty(H::PivotedHouseholderQRStruct, s::Symbol) = s === :p ? Array(getfield(H, :jpvt)) .+ 1 : getfield(H, s)
+# numerical rank: the first k with |α_k| <= rtol |α_1| (reads α: synchronises)
+function LinearAlgebra.rank(H::PivotedHouseholderQRStruct; rtol::Real = max(size(H.A)...) * eps(Float64))
+    a = abs.(Array(H.α))
+    isempty(a) && return 0
+    k = findfirst(x -> !(x > rtol * a[1]), a)
+    return k === nothing ? length(a) : k - 1
+end
+# H \ b: the basic solution x = P [R11^{-1} (Q'b)[1:r]; 0] at r = rank(H; rtol) (dhqr_solve_qrcp_f64); b is not modified
+function LinearAlgebra.ldiv!(x::AbstractVector, H::PivotedHouseholderQRStruct, b::AbstractVector; rtol::Real = max(size(H.A)...) * eps(Float64))
+    A = H.A; m, n = size(A)
+    r = rank(H; rtol)
+    s = CuVector{Float64}(b)
+    GC.@preserve A s check(:dhqr_solve_qrcp_f64, ccall((:dhqr_solve_qrcp_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Int64}, CuPtr{Float64}, Int64, Cint, Ptr{Cvoid}),
+        handle().ptr, m, n, r, pointer(A), stride(A, 2), pointer(H.α), pointer(H.jpvt), pointer(s), m, 1, stream_ptr()))
+    copyto!(x, Array(s[1:n]))
+    return x
+end
+LinearAlgebra.:(\)(H::PivotedHouseholderQRStruct, b::AbstractVector) = ldiv!(Vector{Float64}(undef, size(H.A, 2)), H, b)
+
 end # module

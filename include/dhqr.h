@@ -95,7 +95,8 @@ int dhqr_destroy(dhqr_handle h);
  *   traces:       "panel_trace", "la_trace", "wide_trace" (timestamps read with dhqr_debug_copy_f64)
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
- *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal)
+ *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
+ *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64; device-side, read after synchronising)
  *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
  *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys.
  *   Any other key returns -2 (unknown option). */
@@ -198,6 +199,32 @@ int dhqr_solve_adj_f64(dhqr_handle h, int64_t m, int64_t n, const double *dA, in
                        int64_t ldb, int nrhs, void *stream);
 int dhqr_solve_adj_c64(dhqr_handle h, int64_t m, int64_t n, const void *dA, int64_t lda, const void *d_alpha, void *d_b,
                        int64_t ldb, int nrhs, void *stream);
+
+/* ---- QR with column pivoting (not in the reference; LAPACK dgeqp3 + dgelsy's basic solution) ---------------------------------
+ * A P = Q R: Householder QR with Businger-Golub pivoting on the largest remaining column norm, blocked as in LAPACK dlaqps
+ * (panels of 32 columns, partial norms downdated with LAPACK's tol3z = sqrt(eps) test; a column that fails it is renormed exactly
+ * before the next pivot is chosen).  Float64, single GPU (a handle with nranks > 1 returns -1), n <= m, no row limit.
+ * Stream-ordered, no synchronisation apart from workspace growth (point (iv)).  Two calls on the same input give bitwise
+ * identical results.  Nothing outside A (m x n), alpha (n) or jpvt (n) is written, and no pointer may be less than 8 B aligned.
+ *
+ * dhqr_qrcp_f64: factors in place.  On return A[:, jpvt] = Q R in the library's storage format, so (dA, lda, d_alpha) is the
+ * factorisation of the permuted matrix for every other entry point (apply_qt / apply_q / backsolve / form_q / forwardsolve);
+ * jpvt is 0-based: jpvt[k] = original index of the k-th column.  Pivot k is the remaining column with the largest partial norm;
+ * a tie goes to the smallest index, a NaN norm beats every number (so NaN input shows up in alpha[0]).  alpha_k = -sign(x0) ||x||
+ * with a zero x0 counted as positive.  Once the largest remaining norm is exactly 0, every remaining column is zero in working
+ * precision and every remaining step stores v = 0 and alpha = 0 (H = I).  Read-only option "qrcp_renorms": exact renorms so far.
+ * Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 null (n > 0) or misaligned A, -5 lda < max(1, m),
+ * -6 null or misaligned alpha, -7 null or misaligned jpvt.  Every check runs before anything is enqueued.  n = 0 is a no-op. */
+int dhqr_qrcp_f64(dhqr_handle h, int64_t m, int64_t n, double *dA, int64_t lda, double *d_alpha, int64_t *d_jpvt, void *stream);
+/* x = P [R11^{-1} (Q'b)[0:rank]; 0]: the basic solution of min ||A x - b|| at the given rank (LAPACK dgelsy without the complete
+ * orthogonal decomposition), from a factorisation made by dhqr_qrcp_f64.  Choosing the rank needs alpha on the host, so it is an
+ * argument.  d_b: m x nrhs, ldb >= max(1, m), in place: on return b[0:n] = x, and rows n..m-1 hold rows n..m-1 of
+ * H_rank ... H_1 b.  Only the first `rank` reflectors run.  rank = 0 gives x = 0.  jpvt entries outside [0, n) are skipped, so
+ * nothing is ever written outside b.  Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 rank < 0 or
+ * rank > n, -5 null or misaligned A, -6 lda < max(1, m), -7 null or misaligned alpha, -8 null or misaligned jpvt, -9 null or
+ * misaligned b, -10 ldb < max(1, m), -11 nrhs < 0.  n = 0 or nrhs = 0 is a no-op. */
+int dhqr_solve_qrcp_f64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const double *dA, int64_t lda, const double *d_alpha,
+                        const int64_t *d_jpvt, double *d_b, int64_t ldb, int nrhs, void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
