@@ -208,7 +208,8 @@ static constexpr int G2_BM = 128, G2_BN = YT;               // gemm_cvy: 128 x 6
 
 static size_t smem_g1(int nbp, int bn) { return (size_t)2 * (nbp + bn) * LD1 * 8 + 4 * 8; }
 static size_t smem_g2() { return (size_t)2 * (2 * KC * LD1 + G2_BN * LDK) * 8 + 4 * 8; }
-static size_t smem_g2p() { return (size_t)(2 * (2 * KC * LD1 + G2_BN * LDK) + G2_BN * LDCT) * 8 + 6 * 8; }   // + the C tile: 169 KB
+// the operand ring, the C tile, 2 barriers per stage + cfull, cdone and the gate word: 226 KB (one CTA per SM)
+static size_t smem_g2p() { return (size_t)(CVYP_STAGES * (2 * KC * LD1 + G2_BN * LDK) + G2_BN * LDCT) * 8 + (2 * CVYP_STAGES + 3) * 8; }
 static size_t smem_tinv(int nbp) { return ((size_t)nbp * (nbp + 1) + 4 * 32 * 33 + (nbp == 128 ? 64 * 65 : 0)) * 8; }
 static size_t smem_ymake(int nbp) { return ((size_t)nbp * nbp + YCOLS * nbp) * 8; }
 
@@ -422,6 +423,13 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     return launch_cvy(c, st, vpk, voff, nbp, w.ypk, rows, row_lo, C, ldc, ncols, gate);
 }
 
+// k_gemm_cvy_p: one CTA pair per `tiles_per_cta` consecutive pair-tiles (a row tile by two adjacent column tiles)
+static void launch_cvy_p(const GemmCvyArgs& g2, cudaStream_t st) {
+    const int npairs = g2.tiles_m * ((g2.tiles_n + 1) / 2);
+    const int clusters = (npairs + g2.tiles_per_cta - 1) / g2.tiles_per_cta;
+    k_gemm_cvy_p<<<clusters * CVYP_CLUSTER, CVYP_THREADS, smem_g2p(), st>>>(g2);
+}
+
 // C += V Y on window rows >= row_lo, Y packed in the ypk layout (nbp <= 32: one k-chunk per column tile; else NBMAX / KC):
 // the second half of a block-reflector application, also fed a Y made elsewhere (the pivoted factorisation's -F')
 static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int voff, int nbp, const double* ypk, int64_t rows,
@@ -439,8 +447,7 @@ static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int v
     g2.tiles_per_cta = std::max(c->cvy_persist, 1);   // cvy_persist = 0: one tile per CTA
     g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
     g2.nks = 4; g2.vpk2 = nullptr;
-    if (g2.nkq == 4)
-        k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, CVYP_THREADS, smem_g2p(), st>>>(g2);
+    if (g2.nkq == 4) launch_cvy_p(g2, st);
     else k_gemm_cvy<<<grid2, 9 * 32, smem_g2(), st>>>(g2);
     TRY(post(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols));
     return 0;
@@ -512,7 +519,7 @@ static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const
     g2.tiles_m = (int)((rows + G2_BM - 1) / G2_BM); g2.tiles_n = (ncols + G2_BN - 1) / G2_BN;
     g2.tiles_per_cta = std::max(c->cvy_persist, 1);
     g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
-    k_gemm_cvy_p<<<(g2.tiles_m * g2.tiles_n + g2.tiles_per_cta - 1) / g2.tiles_per_cta, CVYP_THREADS, smem_g2p(), st>>>(g2);
+    launch_cvy_p(g2, st);
     return post(c, st, "k_gemm_cvy256", 2.0 * ((double)rows * WP + (double)(rows - WP) * WP) * (double)ncols);
 }
 
