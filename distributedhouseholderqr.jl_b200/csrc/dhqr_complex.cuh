@@ -32,8 +32,12 @@ __device__ __forceinline__ double2 block_sum2(double2 v, double2* red, int tid, 
     return t;
 }
 
-// S:129-135 for one complex column (one CTA): s = |x|, alpha = -exp(i angle(x0)) s  (S:9; angle(0) = 0 -> -s),
-// f = 1 / sqrt(s (s + |x0|)), x0 -= alpha, x *= f.
+// sin(pi) in Float64 (Julia's sin(pi), numpy's np.sin(np.pi)): written out rather than left to the device sin
+constexpr double SIN_PI = 1.2246467991473532e-16;
+
+// S:129-135 for one complex column (one CTA): s = |x|, alpha = -exp(i angle(x0)) s  (S:9), f = 1 / sqrt(s (s + |x0|)),
+// x0 -= alpha, x *= f.  angle = atan2(im, re) sees the signs of a zero pivot: angle(+0 +- 0i) = +-0 gives alpha = -s,
+// angle(-0 +- 0i) = +-pi gives alpha = -s (cos pi, +-sin pi) = s (1, -+1.2246e-16).
 __global__ void __launch_bounds__(1024, 1) k_house1_c(double2* __restrict__ col, int64_t len, double2* __restrict__ alpha) {
     __shared__ double2 red[32];
     __shared__ double sc[3];
@@ -48,8 +52,18 @@ __global__ void __launch_bounds__(1024, 1) k_house1_c(double2* __restrict__ col,
         const double2 x0 = col[0];
         const double s = sqrt(acc.x);
         const double a0 = hypot(x0.x, x0.y);
-        // -exp(i angle(x0)) = -(x0 / |x0|); angle(0) = 0 -> -1
-        const double ux = a0 > 0.0 ? x0.x / a0 : 1.0, uy = a0 > 0.0 ? x0.y / a0 : 0.0;
+        // -exp(i angle(x0)) = -(x0 / |x0|); exp(i angle(x0)) = (cos, sin) of +-0 or +-pi for a zero x0
+        double ux, uy;
+        if (a0 > 0.0) {
+            ux = x0.x / a0;
+            uy = x0.y / a0;
+        } else if (!signbit(x0.x)) {
+            ux = 1.0;
+            uy = x0.y;
+        } else {
+            ux = -1.0;
+            uy = copysign(SIN_PI, x0.y);
+        }
         const double2 al = make_double2(-ux * s, -uy * s);
         *alpha = al;
         sc[0] = al.x;

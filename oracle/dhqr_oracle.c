@@ -392,9 +392,12 @@ int dhqr_oracle_qr_ext_c(int64_t m, int64_t n, double *a, int64_t lda, double *a
         for (int64_t i = j; i < m; ++i) s += cr[i] * cr[i] + ci[i] * ci[i];
         s = sqrtl(s);                                                  /* S:129 */
         const ldbl xr = cr[j], xi = ci[j], ax = hypotl(xr, xi);
-        /* S:130, S:9: alpha = -exp(im*angle(x)) * s; angle(0) = 0 */
-        ar[j] = ax > 0.0L ? -s * (xr / ax) : -s;
-        ai[j] = ax > 0.0L ? -s * (xi / ax) : 0.0L;
+        /* S:130, S:9: alpha = -exp(im*angle(x)) * s.  angle = atan2(im, re) sees the signs of a zero x: +-0 for +0 +- 0i,
+         * +-pi for -0 +- 0i, whose (cos, sin) is (-1, +-sin(pi)) with Float64's sin(pi), as in the reference */
+        const ldbl ux = ax > 0.0L ? xr / ax : (signbit(xr) ? -1.0L : 1.0L);
+        const ldbl uy = ax > 0.0L ? xi / ax : (signbit(xr) ? copysignl((ldbl)1.2246467991473532e-16, xi) : xi);
+        ar[j] = -s * ux;
+        ai[j] = -s * uy;
         const ldbl f = 1.0L / sqrtl(s * (s + ax));                    /* S:131 */
         cr[j] -= ar[j];                                                /* S:132 */
         ci[j] -= ai[j];

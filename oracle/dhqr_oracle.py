@@ -305,7 +305,7 @@ def np_ldiv(h, alpha, b):
 # ComplexF64 restatement (SURVEY section 8f "next": oracle first; no CUDA path yet)
 # ---------------------------------------------------------------------------
 def np_alphafactor_c(x: complex) -> complex:
-    """S:9: alphafactor(x::Complex) = -exp(im * angle(x))   (angle(0) = 0 -> -1)."""
+    """S:9: alphafactor(x::Complex) = -exp(im * angle(x))   (angle(+0 +- 0i) = +-0 -> -1, angle(-0 +- 0i) = +-pi -> 1 -+ sin(pi) i)."""
     return -np.exp(1j * np.angle(x))
 
 

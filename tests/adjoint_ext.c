@@ -23,9 +23,9 @@ static void factor(int64_t m, int64_t n, ldbl *wr, ldbl *wi, ldbl *ar, ldbl *ai,
         for (int64_t i = j; i < m; ++i) s += cr[i] * cr[i] + (ci ? ci[i] * ci[i] : 0.0L);
         s = sqrtl(s);                                                   /* S:129 */
         const ldbl xr = cr[j], xi = ci ? ci[j] : 0.0L, ax = ci ? hypotl(xr, xi) : fabsl(xr);
-        if (ci) {                                                       /* S:9: -exp(i angle(x)) s, angle(0) = 0 */
-            ar[j] = ax > 0.0L ? -s * (xr / ax) : -s;
-            ai[j] = ax > 0.0L ? -s * (xi / ax) : 0.0L;
+        if (ci) {                                                       /* S:9: -exp(i angle(x)) s, angle(-0 +- 0i) = +-pi */
+            ar[j] = -s * (ax > 0.0L ? xr / ax : (signbit(xr) ? -1.0L : 1.0L));
+            ai[j] = -s * (ax > 0.0L ? xi / ax : (signbit(xr) ? copysignl((ldbl)1.2246467991473532e-16, xi) : xi));
         } else {                                                        /* S:8: -sign(x) s, sign(0) = 0 */
             ar[j] = s * (xr > 0.0L ? -1.0L : (xr < 0.0L ? 1.0L : -0.0L * 0.0L));
         }

@@ -1,5 +1,5 @@
 """The extended-precision acceptance rule shared by the GPU accuracy modules (test_gpu_ext.py: every path on hard families;
-test_gpu_shapes.py: the same rule at the shape edges).
+test_gpu_shapes.py: the same rule at the shape edges; test_gpu_complex_ext.py: every ComplexF64 path on the complex families).
 
 The reference is oracle/dhqr_oracle.c's loop in long double (COracle.qr_ext): the reference's recurrences with a forward error
 of about kappa * 1e-19.  The fp64 oracle runs the same loop in double, so its error against the extended reference on the
@@ -38,6 +38,10 @@ TOL_BWD = 1e-13      # column-wise backward error: Householder QR is column-wise
 TOL_ORTH = 1e-13     # |v_j|^2 = 2 exactly in exact arithmetic (S:131-135)
 COUNTERS = ("wide_panels", "wide_redone", "panels_fast", "panels_fallback")
 RHS = 4              # default right-hand-side block of a real Ref: column 0 the single right-hand side, 1..3 an nrhs = 3 block
+# Ref.check_oracles_agree: err_fp64 <= AGREE kappa eps.  Worst measured on the complex families at 1024 x 384 and 777 x 321:
+# 781 kappa eps (imag: a pivot whose real part is exactly 0 in extended precision and rounding in fp64, divided by a pivot
+# 6e-4 of its column's norm); an oracle pair that disagrees on a convention is off by O(1)
+AGREE = 4096
 
 
 @contextlib.contextmanager
@@ -78,20 +82,21 @@ def qb_sweep(h, b):
 class Ref:
     """Extended and fp64 results for one input.  ``k`` leading columns are compared (the leading-column identity: H[:, :k] and
     alpha[:k] depend on A[:, :k] only); for the zero-column families k is the zero column, and the NaN pattern of the whole
-    fp64 oracle is kept for comparison.
+    fp64 oracle (COracle.qr, or np_qr_c for complex input) is kept for comparison.
 
     ``nrhs`` right-hand sides (default: RHS for real input, one length-m vector for complex) go through both references;
     b, qtb_e, qb_e, x_e, qtb64, qb64 and x64 are then (m or n, nrhs) blocks, except for the complex single vector.  Solves are
-    skipped (``solve`` False) for the zero-column families and where the family is singular at the shape (F.singular)."""
+    skipped (``solve`` False) for the zero-column families and where the family is singular at the shape (F.singular), for
+    real and complex input alike."""
 
-    def __init__(self, coracle, oracle, family, m, n, k=None, cplx=False, solve=True, nrhs=None):
+    def __init__(self, coracle, oracle, family, m, n, k=None, cplx=False, solve=True, nrhs=None, keep_h64=False):
         self.family, self.m, self.n = family, m, n
         A = F.make_complex(family, m, n) if cplx else F.make(family, m, n)
         self.A = A
         self.nan_cols = self.nan_alpha = None
-        if family in F.NAN_FAMILIES:
+        if family in (F.COMPLEX_NAN_FAMILIES if cplx else F.NAN_FAMILIES):
             with np.errstate(all="ignore"):
-                H64, a64 = coracle.qr(A.copy(order="F"))
+                H64, a64 = oracle.np_qr_c(A) if cplx else coracle.qr(A.copy(order="F"))
             self.nan_cols, self.nan_alpha = np.isnan(H64).any(0), np.isnan(a64)
             k, solve = F.zero_column(family, n), False
         k = n if k is None else k
@@ -99,7 +104,10 @@ class Ref:
         self.k, self.solve = k, solve
         Ak = np.asfortranarray(A[:, :k])
         self.cn = np.linalg.norm(Ak, axis=0)
-        if cplx and nrhs is None:
+        if cplx and not solve:
+            self.He, self.ae = coracle.qr_ext_c(Ak)
+            self.H64, self.a64 = oracle.np_qr_c(Ak)
+        elif cplx and nrhs is None:
             self.b = F.rhs(m, 1, cplx=True)
             self.He, self.ae, qtb, x = coracle.qr_ext_c(Ak, self.b)
             self.qtb_e, self.x_e = qtb[:, 0], x[:, 0]
@@ -124,7 +132,20 @@ class Ref:
             self.He, self.ae = coracle.qr_ext(Ak)
             self.H64, self.a64 = coracle.qr(Ak.copy(order="F"))
         self.e64 = factor_errors(self.H64, self.a64, self)
-        del self.H64                                     # only its errors (and solves, above) are needed from here on
+        if not keep_h64:
+            del self.H64                                 # only its errors (and solves, above) are needed from here on
+
+    def check_oracles_agree(self, c=AGREE):
+        """Both oracles describe the same factorisation: err_fp64 <= c kappa eps on V and R, kappa the 2-norm condition number
+        of the leading columns scaled to unit norm.  A convention on which the two differ (the phase of a zero pivot, say)
+        makes err_fp64 O(1), and every rule measured against it would pass whatever the library returns."""
+        Ak = self.A[:, :self.k] / np.where(self.cn > 0, self.cn, 1.0)
+        kappa = float(np.linalg.cond(Ak))
+        for key in ("V", "R"):
+            assert self.e64[key] <= c * kappa * EPS, \
+                f"the fp64 and extended oracles disagree on {key}: {self.e64[key]:.3e} > {c} x kappa {kappa:.3e} x eps; " \
+                f"family {self.family}, {self.m}x{self.n}"
+        return kappa
 
     def solve_errors(self, key, got, r):
         """(err_gpu, err_fp64) of right-hand side ``r`` for metric ``key`` in qtb, qb, x; ``got`` is the library's result."""

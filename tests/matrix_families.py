@@ -22,6 +22,18 @@ Families:
   zerocol_wide     N(0,1) with one exactly zero column in the middle of a 128-column panel
   zerocol_narrow   N(0,1) with one exactly zero column in the middle of a 32-column panel
 A zero column makes the reference's f = 1/sqrt(0) = Inf (S:131): that column and everything it touches afterwards is NaN.
+
+``make_complex`` has a twin of every family above except the two zero-column ones (both parts N(0,1) where the real family is
+N(0,1), U[0,1) where it is uniform; kahan with random unit-modulus row and column phases, which keep its singular values) and:
+  zerocol_first / zerocol_mid / zerocol_last
+                   N(0,1) + i N(0,1) with one exactly zero column: the first, a middle or the last column of a 64-column
+                   complex panel (CPW of dhqr_complex.cuh)
+  imag             i N(0,1): every real part exactly +0
+  zerolead         m >= 2n: rows [0, n) exactly +0, rows [n, 2n) diag(d) with complex |d| in [1, 2), the rest N(0,1) + i N(0,1).
+                   Step j leaves rows j+1..n-1 of every later column exactly +0 (v_j is zero there), so every pivot is an
+                   exact +0 and takes the angle(0) branch of S:9 (alpha_j = -s), in every panel and through the blocked update
+  zerolead_neg / zerolead_negneg
+                   zerolead with A[0, 0] = -0 + 0i / -0 - 0i: angle = +pi / -pi, alpha_0 = s (1, -+sin(pi))
 """
 from __future__ import annotations
 
@@ -32,6 +44,10 @@ FAMILIES = (("uniform", "centered", "normal") + tuple(f"graded{k}" for k in GRAD
             ("colscale", "tiny", "huge", "rowscale", "triangular", "zerorows", "kahan", "zerocol_wide", "zerocol_narrow"))
 COMPLEX_FAMILIES = ("centered", "graded6", "colscale")
 NAN_FAMILIES = ("zerocol_wide", "zerocol_narrow")
+CPW = 64                                                  # complex panel width of the library
+COMPLEX_NAN_FAMILIES = ("zerocol_first", "zerocol_mid", "zerocol_last")
+ZEROLEAD = ("zerolead", "zerolead_neg", "zerolead_negneg")
+COMPLEX_ALL = (tuple(f for f in FAMILIES if f not in NAN_FAMILIES) + ("imag",) + ZEROLEAD + COMPLEX_NAN_FAMILIES)
 
 
 def _rng(family: str, m: int, n: int, seed: int) -> np.random.Generator:
@@ -49,10 +65,14 @@ def _orth(rng, m, n, cplx=False):
 
 
 def zero_column(family: str, n: int) -> int:
-    """Index of the exactly zero column of the zerocol families."""
+    """Index of the exactly zero column of the zerocol families (real and complex)."""
     if family == "zerocol_wide":
         return 128 * (n // 256) + 61 if n >= 128 else n // 2
-    return 32 * (n // 64) + 16 if n >= 32 else n // 2
+    if family == "zerocol_narrow":
+        return 32 * (n // 64) + 16 if n >= 32 else n // 2
+    if n < 2 * CPW:
+        return n // 2
+    return CPW * (n // (2 * CPW)) + {"zerocol_first": 0, "zerocol_mid": 29, "zerocol_last": CPW - 1}[family]
 
 
 def zero_rows(m: int, n: int) -> int:
@@ -65,7 +85,7 @@ def singular(family: str, m: int, n: int) -> bool:
     zero block leaves fewer than n non-zero rows (m = n, for one), and the zero-column families."""
     if family == "zerorows":
         return m - zero_rows(m, n) < n
-    return family in NAN_FAMILIES
+    return family in NAN_FAMILIES or family in COMPLEX_NAN_FAMILIES
 
 
 def make(family: str, m: int, n: int, seed: int = 0) -> np.ndarray:
@@ -110,13 +130,50 @@ def make(family: str, m: int, n: int, seed: int = 0) -> np.ndarray:
 def make_complex(family: str, m: int, n: int, seed: int = 0) -> np.ndarray:
     assert m >= n >= 1
     rng = _rng("c" + family, m, n, seed)
-    if family == "centered":
+
+    def cnormal(r=m, c=n):
+        return rng.standard_normal((r, c)) + 1j * rng.standard_normal((r, c))
+
+    if family == "uniform":
+        a = rng.random((m, n)) + 1j * rng.random((m, n))
+    elif family == "centered":
         a = (rng.random((m, n)) - 0.5) + 1j * (rng.random((m, n)) - 0.5)
+    elif family == "normal":
+        a = cnormal()
     elif family.startswith("graded"):
         k = int(family[6:])
         a = (_orth(rng, m, n, True) * np.logspace(0, -k, n)) @ _orth(rng, n, n, True).conj().T
     elif family == "colscale":
         a = (rng.standard_normal((m, n)) + 1j * rng.standard_normal((m, n))) * 10.0 ** rng.uniform(-120, 120, n)
+    elif family == "tiny":
+        a = cnormal() * 1e-150
+    elif family == "huge":
+        a = cnormal() * 1e150
+    elif family == "rowscale":
+        a = cnormal() * 10.0 ** rng.uniform(-8, 8, m)[:, None]
+    elif family == "triangular":
+        a = np.zeros((m, n), dtype=np.complex128)
+        a[:n] = np.triu(cnormal(n, n))
+    elif family == "zerorows":
+        a = cnormal()
+        a[m - zero_rows(m, n):] = 0.0
+    elif family == "kahan":
+        phase = lambda k: np.exp(2j * np.pi * rng.random(k))
+        a = phase(m)[:, None] * make("kahan", m, n) * phase(n)
+    elif family in COMPLEX_NAN_FAMILIES:
+        a = cnormal()
+        a[:, zero_column(family, n)] = 0.0
+    elif family == "imag":
+        a = np.zeros((m, n), dtype=np.complex128)       # real parts +0 (1j * x would give -0 where x < 0)
+        a.imag = rng.standard_normal((m, n))
+    elif family in ZEROLEAD:
+        if m < 2 * n:
+            raise ValueError(f"{family} needs m >= 2n, got {m} x {n}")
+        a = np.zeros((m, n), dtype=np.complex128)
+        a[n + np.arange(n), np.arange(n)] = (1.0 + rng.random(n)) * np.exp(2j * np.pi * rng.random(n))
+        a[2 * n:] = cnormal(m - 2 * n, n)
+        if family != "zerolead":
+            a[0, 0] = complex(-0.0, 0.0 if family == "zerolead_neg" else -0.0)
     else:
         raise ValueError(f"unknown complex family {family!r}")
     return np.asfortranarray(a, dtype=np.complex128)

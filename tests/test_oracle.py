@@ -229,6 +229,29 @@ def test_ext_mirrors_zero_column_and_zero_pivot(oracle, coracle):
     assert coracle.qr_ext(P)[1][0] == 0.0
 
 
+SIGNED_ZERO_PIVOTS = [(complex(0.0, 0.0), -1.0), (complex(0.0, -0.0), -1.0),
+                      (complex(-0.0, 0.0), 1.0 - 1.2246467991473532e-16j), (complex(-0.0, -0.0), 1.0 + 1.2246467991473532e-16j)]
+
+
+@pytest.mark.parametrize("x0,af", SIGNED_ZERO_PIVOTS, ids=["+0+0i", "+0-0i", "-0+0i", "-0-0i"])
+def test_complex_zero_pivot_follows_the_signs_of_its_zeros(oracle, coracle, x0, af):
+    # alphafactor(x::Complex) = -exp(im * angle(x)) (S:9) and angle = atan2(imag, real) sees the sign of a zero: angle(-0 +- 0i)
+    # = +-pi.  The numpy oracle, the long double oracle (qr_ext_c and the adjoint reference) and dhqr_b200.alphafactor agree
+    import adjoint_oracle as AO
+    import dhqr_b200
+    assert oracle.np_alphafactor_c(x0) == af and dhqr_b200.alphafactor(x0) == af
+    A = np.asfortranarray(np.array([[x0, 1.0], [3.0 - 4.0j, 2.0j], [0.0, 1.0 + 1.0j]], dtype=np.complex128))
+    s = 5.0
+    Hn, an = oracle.np_qr_c(A)
+    He, ae = coracle.qr_ext_c(A)
+    assert an[0] == s * af and ae[0] == s * af
+    assert np.abs(He - Hn).max() < 1e-15 and np.abs(ae - an).max() < 1e-14
+    assert abs(Hn[0, 0] - (x0 - s * af) / s) < 1e-16                                     # f = 1 / s: |x0| = 0 (S:131)
+    # adj_ext factors in long double with the same convention: z_0 = c_0 / conj(alpha_0)
+    z, _ = AO.adj_ext(A, np.array([1.0 + 0j, 0.0]))
+    assert abs(z[0] - 1.0 / np.conj(s * af)) < 1e-16
+
+
 @pytest.mark.parametrize("family,h_err,a_err", [("uniform", 2.5e-14, 1.6e-16), ("normal", 1.3e-14, 3.5e-16),
                                                 ("graded6", 5.4e-12, 2.6e-12), ("graded12", 3.5e-6, 1.2e-6)])
 def test_fp64_oracle_forward_error_against_ext(family, h_err, a_err, oracle, coracle):
