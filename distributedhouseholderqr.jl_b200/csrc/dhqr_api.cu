@@ -67,11 +67,18 @@ struct NcclApi {
 static NcclApi g_nccl;
 static int load_nccl() {
     if (g_nccl.lib) return 0;
-    // An already-loaded libnccl.so.2 (e.g. the one bundled with torch) is reused by soname.
+    // DHQR_NCCL_LIBRARY names the library to use.  It is opened privately (RTLD_LOCAL), so its symbols never take the place
+    // of those of a libnccl.so.2 the process already has (torch's), and the library resolves its ten entry points in it alone.
+    const char* path = getenv("DHQR_NCCL_LIBRARY");
+    if (path && *path) {
+        g_nccl.lib = dlopen(path, RTLD_NOW | RTLD_LOCAL);
+        if (!g_nccl.lib) return set_err(2001, "cannot dlopen DHQR_NCCL_LIBRARY=%s: %s", path, dlerror());
+    }
+    // Otherwise an already-loaded libnccl.so.2 (e.g. the one bundled with torch) is reused by soname.
     const char* names[] = {"libnccl.so.2", "libnccl.so"};
     for (const char* nm : names) {
-        g_nccl.lib = dlopen(nm, RTLD_NOW | RTLD_GLOBAL);
         if (g_nccl.lib) break;
+        g_nccl.lib = dlopen(nm, RTLD_NOW | RTLD_GLOBAL);
     }
     if (!g_nccl.lib) return set_err(2001, "cannot dlopen libnccl.so.2: %s", dlerror());
 #define SYM(field, name)                                                       \
@@ -161,6 +168,7 @@ struct dhqr_context {
     int qt_vec = 1;                                                     // option: use it (0: the GEMM-shaped block update also for one right-hand side)
     double* v1 = nullptr;    size_t v1_elems = 0;                       // unblocked path: v
     double* xbuf = nullptr;  size_t xbuf_elems = 0;                     // back-substitution output
+    double* xfer = nullptr;  size_t xfer_elems = 0;                     // a right-hand-side block packed for the rank-to-rank hand-over
     // pivoted factorisation (dhqr_qrcp.cuh): vn1, vn2, F, the column in flight and the partials of both reductions; renorm
     // flags; scalars of the reflector in flight, the pivot ticket and the renorm counter
     double* qp_buf = nullptr; size_t qp_buf_elems = 0;
@@ -1518,7 +1526,7 @@ int dhqr_destroy(dhqr_handle c) {
     for (int i = 0; i < 4; ++i)
         if (c->ev_aux[i]) cudaEventDestroy(c->ev_aux[i]);
     cudaFree(c->qp_buf); cudaFree(c->qp_flag); cudaFree(c->qp_ctl);
-    cudaFree(c->v1); cudaFree(c->xbuf); cudaFree(c->hostA); cudaFree(c->hostB); cudaFree(c->d_i64);
+    cudaFree(c->v1); cudaFree(c->xbuf); cudaFree(c->xfer); cudaFree(c->hostA); cudaFree(c->hostB); cudaFree(c->d_i64);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     if (c->d2h_stream) cudaStreamDestroy(c->d2h_stream);
     if (c->h2d_stream) cudaStreamDestroy(c->h2d_stream);
@@ -1690,6 +1698,22 @@ int dhqr_qr_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
     return qr_blocked(c, st, m, n_global, col0, n_local, dA, lda, d_alpha, nb);
 }
 
+// The rows x nrhs block of b as one contiguous message for the rank-to-rank hand-over.  With ldb > rows and nrhs > 1 the rows
+// between its columns are the caller's padding, which must neither travel nor be overwritten by another rank's: the block is
+// then packed into handle workspace (*msg = c->xfer) and unpacked after.  Otherwise *msg = b.
+static int rhs_message(dhqr_context* c, cudaStream_t st, double* b, int64_t ldb, int64_t rows, int nrhs, double** msg) {
+    *msg = b;
+    if (ldb == rows || nrhs == 1) return 0;
+    TRY(ensure(&c->xfer, &c->xfer_elems, (size_t)rows * nrhs, st));
+    *msg = c->xfer;
+    return 0;
+}
+static int rhs_copy(cudaStream_t st, double* dst, int64_t lddst, const double* src, int64_t ldsrc, int64_t rows, int nrhs) {
+    if (dst == src) return 0;
+    CU(cudaMemcpy2DAsync(dst, (size_t)lddst * 8, src, (size_t)ldsrc * 8, (size_t)rows * 8, nrhs, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
 int dhqr_apply_qt_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
                       int64_t lda, double* d_b, int64_t ldb, int nrhs, void* stream) {
     TRY(check_common(c, m, n_global, col0, n_local, dA, lda));
@@ -1704,15 +1728,22 @@ int dhqr_apply_qt_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
     TRY(check_partition(col0s, nls, n_global));
     TRY(ensure_workspace(c, st, m, std::max<int64_t>(n_local, nrhs)));
     // C3 (S:227-229): owners act on b one after the other; b travels rank -> rank
-    const size_t cnt = (size_t)ldb * (nrhs - 1) + m;
+    const size_t cnt = (size_t)m * nrhs;
+    double* msg = d_b;
+    if (c->nranks > 1) TRY(rhs_message(c, st, d_b, ldb, m, nrhs, &msg));
     const bool vec = qt_vec_ok(c, m, nrhs);
     if (vec) TRY(qt_prepare(c, st, m, col0, n_local, dA, lda));
-    if (c->nranks > 1 && c->rank > 0) NC(g_nccl.Recv(d_b, cnt, ncclFloat64, c->rank - 1, c->comm, st));
+    if (c->nranks > 1 && c->rank > 0) {
+        NC(g_nccl.Recv(msg, cnt, ncclFloat64, c->rank - 1, c->comm, st));
+        TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
+    }
     if (vec) TRY(apply_qt_local_vec(c, st, m, col0, n_local, dA, lda, d_b, 0));
     else TRY(apply_qt_local(c, st, m, col0, n_local, dA, lda, d_b, ldb, nrhs));
     if (c->nranks > 1) {
-        if (c->rank + 1 < c->nranks) NC(g_nccl.Send(d_b, cnt, ncclFloat64, c->rank + 1, c->comm, st));
-        NC(g_nccl.Broadcast(d_b, d_b, cnt, ncclFloat64, c->nranks - 1, c->comm, st));
+        TRY(rhs_copy(st, msg, m, d_b, ldb, m, nrhs));
+        if (c->rank + 1 < c->nranks) NC(g_nccl.Send(msg, cnt, ncclFloat64, c->rank + 1, c->comm, st));
+        NC(g_nccl.Broadcast(msg, msg, cnt, ncclFloat64, c->nranks - 1, c->comm, st));
+        if (c->rank + 1 < c->nranks) TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
     }
     return 0;
 }
@@ -1731,15 +1762,22 @@ int dhqr_apply_q_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, i
     TRY(check_partition(col0s, nls, n_global));
     TRY(ensure_workspace(c, st, m, std::max<int64_t>(n_local, nrhs)));
     // b <- H_1 ... H_n b: the owners act in reverse rank order, b travels rank -> rank - 1
-    const size_t cnt = (size_t)ldb * (nrhs - 1) + m;
+    const size_t cnt = (size_t)m * nrhs;
+    double* msg = d_b;
+    if (c->nranks > 1) TRY(rhs_message(c, st, d_b, ldb, m, nrhs, &msg));
     const bool vec = qt_vec_ok(c, m, nrhs);
     if (vec) TRY(qt_prepare(c, st, m, col0, n_local, dA, lda));
-    if (c->nranks > 1 && c->rank + 1 < c->nranks) NC(g_nccl.Recv(d_b, cnt, ncclFloat64, c->rank + 1, c->comm, st));
+    if (c->nranks > 1 && c->rank + 1 < c->nranks) {
+        NC(g_nccl.Recv(msg, cnt, ncclFloat64, c->rank + 1, c->comm, st));
+        TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
+    }
     if (vec) TRY(apply_qt_local_vec(c, st, m, col0, n_local, dA, lda, d_b, 1));
     else TRY(apply_qt_local(c, st, m, col0, n_local, dA, lda, d_b, ldb, nrhs, 1));
     if (c->nranks > 1) {
-        if (c->rank > 0) NC(g_nccl.Send(d_b, cnt, ncclFloat64, c->rank - 1, c->comm, st));
-        NC(g_nccl.Broadcast(d_b, d_b, cnt, ncclFloat64, 0, c->comm, st));
+        TRY(rhs_copy(st, msg, m, d_b, ldb, m, nrhs));
+        if (c->rank > 0) NC(g_nccl.Send(msg, cnt, ncclFloat64, c->rank - 1, c->comm, st));
+        NC(g_nccl.Broadcast(msg, msg, cnt, ncclFloat64, 0, c->comm, st));
+        if (c->rank > 0) TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
     }
     return 0;
 }
@@ -1761,15 +1799,19 @@ int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     TRY(wave_prepare(c, st, n_local));
     // C4 (S:260-267), column oriented: the last owner solves its block of unknowns and removes their
     // contribution from the rows above; the partially reduced right-hand side then moves one rank down.
-    const size_t cnt = (size_t)ldb * (nrhs - 1) + n_global;
+    const size_t cnt = (size_t)n_global * nrhs;
+    double* msg = d_b;
+    if (c->nranks > 1) TRY(rhs_message(c, st, d_b, ldb, n_global, nrhs, &msg));
     if (c->nranks > 1 && c->rank + 1 < c->nranks) {
-        NC(g_nccl.Recv(d_b, cnt, ncclFloat64, c->rank + 1, c->comm, st));
+        NC(g_nccl.Recv(msg, cnt, ncclFloat64, c->rank + 1, c->comm, st));
         NC(g_nccl.Recv(c->xbuf, (size_t)n_global * nrhs, ncclFloat64, c->rank + 1, c->comm, st));
+        TRY(rhs_copy(st, d_b, ldb, msg, n_global, n_global, nrhs));
     }
     TRY(backsolve_local(c, st, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs, c->xbuf, n_global));
     if (c->nranks > 1) {
         if (c->rank > 0) {
-            NC(g_nccl.Send(d_b, cnt, ncclFloat64, c->rank - 1, c->comm, st));
+            TRY(rhs_copy(st, msg, n_global, d_b, ldb, n_global, nrhs));
+            NC(g_nccl.Send(msg, cnt, ncclFloat64, c->rank - 1, c->comm, st));
             NC(g_nccl.Send(c->xbuf, (size_t)n_global * nrhs, ncclFloat64, c->rank - 1, c->comm, st));
         }
         NC(g_nccl.Broadcast(c->xbuf, c->xbuf, (size_t)n_global * nrhs, ncclFloat64, 0, c->comm, st));
