@@ -1,5 +1,6 @@
 """The extended-precision acceptance rule shared by the GPU accuracy modules (test_gpu_ext.py: every path on hard families;
-test_gpu_shapes.py: the same rule at the shape edges; test_gpu_complex_ext.py: every ComplexF64 path on the complex families).
+test_gpu_shapes.py: the same rule at the shape edges; test_gpu_complex_ext.py: every ComplexF64 path on the complex families;
+test_gpu_host_ext.py: the pipelined host entry in pinned memory).
 
 The reference is oracle/dhqr_oracle.c's loop in long double (COracle.qr_ext): the reference's recurrences with a forward error
 of about kappa * 1e-19.  The fp64 oracle runs the same loop in double, so its error against the extended reference on the
@@ -87,11 +88,16 @@ class Ref:
     ``nrhs`` right-hand sides (default: RHS for real input, one length-m vector for complex) go through both references;
     b, qtb_e, qb_e, x_e, qtb64, qb64 and x64 are then (m or n, nrhs) blocks, except for the complex single vector.  Solves are
     skipped (``solve`` False) for the zero-column families and where the family is singular at the shape (F.singular), for
-    real and complex input alike."""
+    real and complex input alike.
 
-    def __init__(self, coracle, oracle, family, m, n, k=None, cplx=False, solve=True, nrhs=None, keep_h64=False):
+    ``A`` replaces the family's matrix with a given (m, n) one (a pivoted matrix, a panel made nearly rank deficient); ``family``
+    then only labels it.  ``b`` (real input) replaces the default right-hand sides with a given length-m vector or (m, k) block."""
+
+    def __init__(self, coracle, oracle, family, m, n, k=None, cplx=False, solve=True, nrhs=None, keep_h64=False, A=None, b=None):
         self.family, self.m, self.n = family, m, n
-        A = F.make_complex(family, m, n) if cplx else F.make(family, m, n)
+        if A is None:
+            A = F.make_complex(family, m, n) if cplx else F.make(family, m, n)
+        assert A.shape == (m, n), (A.shape, m, n)
         self.A = A
         self.nan_cols = self.nan_alpha = None
         if family in (F.COMPLEX_NAN_FAMILIES if cplx else F.NAN_FAMILIES):
@@ -121,8 +127,11 @@ class Ref:
             self.qtb64 = np.stack([oracle.np_apply_qt_c(self.H64, self.b[:, r]) for r in range(nrhs)], 1)
             self.x64 = np.stack([oracle.np_ldiv_c(self.H64, self.a64, self.b[:, r]) for r in range(nrhs)], 1)
         elif solve:
-            nrhs = RHS if nrhs is None else nrhs
-            self.b = np.asfortranarray(F.rhs(m, nrhs).reshape(m, nrhs))
+            if b is None:
+                nrhs = RHS if nrhs is None else nrhs
+                b = F.rhs(m, nrhs)
+            self.b = np.asfortranarray(np.reshape(b, (m, -1)))
+            nrhs = self.b.shape[1]
             self.He, self.ae, self.qtb_e, self.qb_e, self.x_e = coracle.qr_ext(Ak, self.b, want_qb=True)
             self.H64, self.a64 = coracle.qr(Ak.copy(order="F"))
             self.qtb64 = np.stack([coracle.apply_qt(self.H64, self.b[:, r].copy()) for r in range(nrhs)], 1)

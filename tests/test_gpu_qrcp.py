@@ -46,27 +46,10 @@ def qrcp(D, h, A0, lda=None):
     return st, np.asfortranarray(A.cpu().numpy()), st.α.cpu().numpy(), st.p.cpu().numpy()
 
 
-class PRef(E.Ref):
+def PRef(coracle, A, family, k=None, b=None):
     """ext_rule.Ref of a given matrix (A[:, p]): extended and fp64 factorisations of its leading k columns, optionally with
     right-hand sides b (the extended least-squares solution of the leading k columns)."""
-
-    def __init__(self, coracle, A, family, k=None, b=None):
-        self.family, (self.m, self.n) = family, A.shape
-        self.A = A
-        self.nan_cols = self.nan_alpha = None
-        self.k = k = self.n if k is None else k
-        self.solve = b is not None
-        Ak = np.asfortranarray(A[:, :k])
-        self.cn = np.linalg.norm(Ak, axis=0)
-        if b is not None:
-            self.b = np.asfortranarray(b.reshape(self.m, -1))
-            self.He, self.ae, _, _, self.x_e = coracle.qr_ext(Ak, self.b)
-        else:
-            self.He, self.ae = coracle.qr_ext(Ak)
-        H64, a64 = coracle.qr(Ak.copy(order="F"))
-        if b is not None:
-            self.x64 = np.stack([coracle.ldiv(H64, a64, self.b[:, r].copy()) for r in range(self.b.shape[1])], 1)
-        self.e64 = E.factor_errors(H64, a64, self)
+    return E.Ref(coracle, None, family, *A.shape, k=k, solve=b is not None, A=A, b=b)
 
 
 def check_factor(coracle, path, family, A0, H, alpha, p, k=None):
