@@ -233,6 +233,7 @@ static int set_attrs(dhqr_context* c) {
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2p()));
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(k_gram_sym, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_GRAM_SYM));
+    CU(cudaFuncSetAttribute(k_pack_gram, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_GRAM_SYM));
     CU(cudaFuncSetAttribute(k_tinv<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(128)));
     CU(cudaFuncSetAttribute(k_tinv<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(32)));
     CU(cudaFuncSetAttribute(k_ymake<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(128)));
@@ -651,14 +652,24 @@ static int factor_outer_panel_narrow(dhqr_context* c, cudaStream_t st, double* v
     return 0;
 }
 
+// The split of a panel's Gram matrix over CTAs: k_gram_sym, k_pack_gram and the Gram mode of k_vpk_rmul all run on this many
+// CTAs, so that they sum the same chunks in the same order.
+static int panel_gram_split(dhqr_context* c, const dhqr_context::WSet& w, int64_t rows, int* nchunks_out, int* nsplit_out) {
+    const int nchunks = (int)((rows + KC1 - 1) / KC1);
+    const int cps = std::max(1, (nchunks + c->sms - 1) / c->sms);                           // chunks per CTA: whole waves of equal CTAs
+    const int nsplit = (nchunks + cps - 1) / cps;
+    if ((size_t)nsplit * WP * WP > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
+    *nchunks_out = nchunks;
+    *nsplit_out = nsplit;
+    return 0;
+}
+
 // Partial Gram matrices of the packed panel in `vpk` (window rows `rows`) -> w.wpart; returns the number of partials and their stride.
 static int launch_panel_gram(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_context::WSet& w, int64_t rows, int* nsplit_out,
                              int64_t* pstride_out) {
-    const int nchunks = (int)((rows + KC1 - 1) / KC1);
     const int64_t pstride = (int64_t)WP * WP;
-    const int cps = std::max(1, (nchunks + c->sms - 1) / c->sms);                           // chunks per CTA: whole waves of equal CTAs
-    const int nsplit = (nchunks + cps - 1) / cps;
-    if ((size_t)nsplit * pstride > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
+    int nchunks, nsplit;
+    TRY(panel_gram_split(c, w, rows, &nchunks, &nsplit));
     GramSymArgs g;
     g.vpk = vpk; g.nchunks = nchunks; g.Wp = w.wpart; g.pstride = pstride;
     pre(c, st);
@@ -681,32 +692,35 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     double* vflag = vpk + KC1;                  // padding row 64 of packed column 0: travels with the V buffer
     const int nq = (int)(g.vrows / KC1);
     long long* stamps = c->wide_trace ? c->wstamps : nullptr;
+    // Gram matrices of the panel: partials over the window rows, split over CTAs as launch_panel_gram splits them
+    int nchunks = 0, nsplit = 0;
+    const int64_t pstride = (int64_t)WP * WP;
+    TRY(panel_gram_split(c, w, g.rows, &nchunks, &nsplit));
     RmulArgs r;
     r.vpk = vpk; r.ctl = c->wctl; r.step = step; r.P = nullptr; r.ldp = lda; r.mp = g.rows;
-    auto rmul = [&](int q0, int n, const double* Z, double* Pout) -> int {
+    r.Wp = nullptr; r.nchunks = nchunks; r.pstride = pstride;
+    auto rmul = [&](int q0, int n, const double* Z, double* Pout, bool with_gram) -> int {
         if (n <= 0) return 0;
-        r.q0 = q0; r.nq = n; r.ZL = Z; r.P = Pout;
+        r.q0 = q0; r.nq = n; r.ZL = Z; r.P = Pout; r.Wp = with_gram ? w.wpart : nullptr;
         pre(c, st);
-        k_vpk_rmul<<<std::min(n, c->sms), 256, SMEM_RMUL, st>>>(r);
+        k_vpk_rmul<<<with_gram ? nsplit : std::min(n, c->sms), 256, SMEM_RMUL, st>>>(r);
+        if (with_gram) return post(c, st, "k_rmul_gram", 2.0 * 64.0 * n * WP * 80.0 + 2.0 * (double)g.rows * WP * WP);
         return post(c, st, "k_vpk_rmul", 2.0 * 64.0 * n * WP * 80.0);
     };
-    // Gram matrix of the packed panel: partials of vpk' vpk over the window rows
-    int nsplit = 0;
-    int64_t pstride = 0;
-    auto gram = [&]() -> int { return launch_panel_gram(c, st, vpk, w, g.rows, &nsplit, &pstride); };
+    // pack + first Gram: the chunks go from the caller's matrix into the Gram kernel's tiles, and from there to vpk
+    PackGramArgs pg;
+    pg.P = P; pg.ldp = lda; pg.rows = g.rows; pg.p_bulk = ((reinterpret_cast<uintptr_t>(P) & 15) == 0) && ((lda & 1) == 0);
+    pg.vpk = vpk; pg.nq = nq; pg.nchunks = nchunks; pg.Wp = w.wpart; pg.pstride = pstride;
     pre(c, st);
-    dim3 pgrid((unsigned)std::min<int64_t>((g.vrows / 4 + 255) / 256, 4 * c->sms), WP);
-    k_pack<<<pgrid, 256, 0, st>>>(P, lda, g.rows, WP, 0, vpk, 0, 0, g.vrows);
-    TRY(post(c, st, "k_pack"));
-    TRY(gram());
+    k_pack_gram<<<nsplit, (GS_MMA_WARPS + PG_PROD_WARPS) * 32, SMEM_GRAM_SYM, st>>>(pg);
+    TRY(post(c, st, "k_gram128", 2.0 * (double)g.rows * WP * WP));
     pre(c, st);
     k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum);
     TRY(post(c, st, "k_wreduce"));
     pre(c, st);
     k_chol128<<<1, 512, SMEM_WIDE1, st>>>(w.wsum, R1, Z1, c->wctl, step, vflag, c->wide_kappa, stamps);
     TRY(post(c, st, "k_chol128"));
-    TRY(rmul(0, nq, Z1, nullptr));
-    TRY(gram());
+    TRY(rmul(0, nq, Z1, nullptr, true));    // Q1, and the partials of the second Gram matrix Q1'Q1
     pre(c, st);
     k_gram2_finish<<<256, 256, 0, st>>>(w.wpart, pstride, nsplit, w.wsum, R2, Z2, c->wctl, step, vflag);
     TRY(post(c, st, "k_gram2_finish"));
@@ -718,7 +732,7 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     k_trimm128<<<10, 256, SMEM_TRIMM, sx>>>(R2, R1, Rt, c->wctl, step);
     TRY(post(c, sx, "k_trimm128"));
     if (sx != st) CU(cudaEventRecord(c->ev_aux[1], sx));
-    TRY(rmul(0, 2, Z2, nullptr));
+    TRY(rmul(0, 2, Z2, nullptr, false));
     if (sx != st) CU(cudaStreamWaitEvent(st, c->ev_aux[1], 0));
     pre(c, st);
     k_hr128<<<1, 512, SMEM_WIDE1, st>>>(vpk, Rt, P, lda, alpha + p.c, Rr, MT, c->wctl, step, stamps ? stamps + 16 : nullptr);
@@ -733,7 +747,7 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     pre(c, st);
     k_trimm_z<<<10, 256, SMEM_TRIMM, st>>>(Rr, R2, Z23, c->wctl, step);
     TRY(post(c, st, "k_trimm_z"));
-    TRY(rmul(2, nq - 2, Z23, P));
+    TRY(rmul(2, nq - 2, Z23, P, false));
     if (linv_out && sx != st) CU(cudaStreamWaitEvent(st, c->ev_aux[3], 0));   // T' is part of the panel's result
     c->wide_panels++;
     return 0;
