@@ -139,6 +139,16 @@ struct dhqr_context {
     int lookahead = 1;
     int la_trace = 0;                                                   // keep timing events of the look-ahead schedule
     std::vector<float> la_times;                                        // [k][3]: panel k done (hp), next k signalled (st), bulk k done (st), ms since start
+    // option chain_wait_trace (look-ahead schedule): CUDA events right before and after every launch on hp, hp2 and aux, and
+    // the CwtScope stamps of the same launch, so that the time a launch was ready but had no SM can be told from its run time
+    int chain_wait_trace = 0;
+    unsigned long long* cwt_stamps = nullptr;                           // [CWT_MAX][2]: first CTA start, last warp end (%globaltimer ns)
+    unsigned long long* cwt_cur = nullptr;                              // slot of the launch between pre() and post(); null: not traced
+    cudaEvent_t cwt_e0 = nullptr;
+    int cwt_unit = 0, cwt_stream = 0;
+    struct CwtRec { int unit, stream, cls; cudaEvent_t e0, e1; };
+    std::vector<CwtRec> cwt_recs;
+    std::vector<double> cwt_rows;                                       // [launch][6]: unit, stream, class, event span, stamp span, wait (ms)
     unsigned long long* cells = nullptr;                                // panel exchange cells [IB+1][MAXG+1][IB][2]
     uint32_t ll_epoch = 0;
     unsigned long long* cells2 = nullptr;                               // exchange cells of the panel kernel's fast path
@@ -207,6 +217,7 @@ struct dhqr_context {
 };
 
 static constexpr int NBMAX = 128;
+static constexpr int CWT_MAX = 8192;   // traced launches per factorisation (option chain_wait_trace)
 static constexpr int MAXCTAS_FACTOR = 3;
 
 // gemm tile configurations
@@ -325,14 +336,34 @@ static int prof_slot(dhqr_context* c, const char* name) {
     c->prof_slots.push_back(s);
     return (int)c->prof_slots.size() - 1;
 }
-// pre(): open a CUDA-event bracket on the launching stream when profiling is on
+// chain_wait_trace: open an event bracket around the next launch when `st` is one of the chain's streams; its kernel gets the
+// stamp slot c->cwt_cur, and post() closes the bracket
+static void cwt_open(dhqr_context* c, cudaStream_t st) {
+    c->cwt_cur = nullptr;
+    if (!c->chain_wait_trace || !c->cwt_stamps || c->cwt_recs.size() >= (size_t)CWT_MAX) return;
+    const int s = st == c->hp_stream ? 0 : st == c->hp2_stream ? 1 : st == c->aux_stream ? 2 : -1;
+    if (s >= 0 && cudaEventCreate(&c->cwt_e0) == cudaSuccess) {
+        cudaEventRecord(c->cwt_e0, st);
+        c->cwt_stream = s;
+        c->cwt_cur = c->cwt_stamps + 2 * c->cwt_recs.size();
+    }
+}
+// pre(): open a CUDA-event bracket on the launching stream when profiling is on (and the chain_wait_trace one)
 static void pre(dhqr_context* c, cudaStream_t st) {
+    cwt_open(c, st);
     if (!c->profile) return;
     cudaEventCreate(&c->prof_open);
     cudaEventRecord(c->prof_open, st);
 }
 static int post(dhqr_context* c, cudaStream_t st, const char* what, double work = 0.0) {
     c->launches++;
+    if (c->cwt_cur) {
+        dhqr_context::CwtRec r{c->cwt_unit, c->cwt_stream, prof_slot(c, what), c->cwt_e0, nullptr};
+        cudaEventCreate(&r.e1);
+        cudaEventRecord(r.e1, st);
+        c->cwt_recs.push_back(r);
+        c->cwt_cur = nullptr;
+    }
     if (c->profile && c->prof_open) {
         dhqr_context::ProfRec r;
         r.slot = prof_slot(c, what);
@@ -402,6 +433,7 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     g1.Wp = w.wpart; g1.pstride = pstride;
     dim3 grid1(tiles, nsplit);
     pre(c, st);
+    g1.cwt = c->cwt_cur;
     if (small) {
         K_G1_32<<<grid1, (1 * 4 + G1S_NPW) * 32, smem_g1(32, G1S_BN), st>>>(g1);
     } else {
@@ -416,17 +448,17 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     } else {
         pre(c, st);
         const int64_t nelem = (int64_t)next * NBPK;
-        k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, w.wsum);
+        k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, w.wsum, c->cwt_cur);
         TRY(post(c, st, "k_wreduce"));
         if (!reuse_T) {
             pre(c, st);
-            if (small) k_tinv<32><<<1, 512, smem_tinv(32), st>>>(w.wsum, linv);
-            else k_tinv<128><<<1, 512, smem_tinv(128), st>>>(w.wsum, linv);
+            if (small) k_tinv<32><<<1, 512, smem_tinv(32), st>>>(w.wsum, linv, 0, c->cwt_cur);
+            else k_tinv<128><<<1, 512, smem_tinv(128), st>>>(w.wsum, linv, 0, c->cwt_cur);
             TRY(post(c, st, small ? "k_tinv32" : "k_tinv128"));
         }
         pre(c, st);
-        if (small) k_ymake<32><<<ygrid, 256, smem_ymake(32), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans);
-        else k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans);
+        if (small) k_ymake<32><<<ygrid, 256, smem_ymake(32), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans, c->cwt_cur);
+        else k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans, c->cwt_cur);
         TRY(post(c, st, small ? "k_ymake32" : "k_ymake128"));
     }
     return launch_cvy(c, st, vpk, voff, nbp, w.ypk, rows, row_lo, C, ldc, ncols, gate);
@@ -447,6 +479,7 @@ static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int v
     const int NBPK = small ? 32 : 128;
     pre(c, st);
     GemmCvyArgs g2;
+    g2.cwt = c->cwt_cur;
     g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.row_lo = row_lo; g2.ncols = ncols;
     g2.vpk = vpk; g2.voff = voff; g2.ypk = ypk;
     g2.nkq = small ? 1 : (int)(rup(nbp, KC) / KC); g2.nkq_alloc = NBPK / KC;
@@ -476,6 +509,7 @@ static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* v
     g1.a_aligned = (((uintptr_t)B & 15) == 0 && (ldb & 1) == 0) ? 1 : 0;
     g1.Wp = w.wpart; g1.pstride = pstride;
     pre(c, st);
+    g1.cwt = c->cwt_cur;
     K_G1_128<<<dim3(tiles, nsplit), (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
     *nsplit_out = nsplit;
     *pstride_out = pstride;
@@ -490,7 +524,7 @@ static int block_w(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_con
     TRY(launch_vta_partials(c, st, vpk, w, C, ldc, rows, ncols, "k_gemm_vta128", &nsplit, &pstride));
     pre(c, st);
     const int64_t nelem = (int64_t)ncols * NBMAX;
-    k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, Ws);
+    k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, Ws, c->cwt_cur);
     return post(c, st, "k_wreduce");
 }
 
@@ -502,7 +536,7 @@ static int form_pair_gram(dhqr_context* c, cudaStream_t st, const double* vpk_b,
     int64_t pstride = 0;
     TRY(launch_vta_partials(c, st, vpk_b, w, A + (ca - col0) * lda + ca + WP, lda, m - ca - WP, WP, "k_gram_pair", &nsplit, &pstride));
     pre(c, st);
-    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, gout);
+    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, gout, c->cwt_cur);
     return post(c, st, "k_wreduce");
 }
 
@@ -517,10 +551,11 @@ static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const
     TRY(block_w(c, st, vpa, w, C, ldc, rows, ncols, Wa));
     TRY(block_w(c, st, vpb, w, C + WP, ldc, rows - WP, ncols, Wb));
     pre(c, st);
-    k_ymake2<<<(ncols + YCOLS - 1) / YCOLS, 256, SMEM_YMAKE2, st>>>(Wa, Wb, ncols, Ta, Tb, G, w.ypk);
+    k_ymake2<<<(ncols + YCOLS - 1) / YCOLS, 256, SMEM_YMAKE2, st>>>(Wa, Wb, ncols, Ta, Tb, G, w.ypk, c->cwt_cur);
     TRY(post(c, st, "k_ymake2"));
     pre(c, st);
     GemmCvyArgs g2;
+    g2.cwt = c->cwt_cur;
     g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.row_lo = 0; g2.ncols = ncols;
     g2.vpk = vpa; g2.voff = 0; g2.vpk2 = vpb; g2.ypk = w.ypk;
     g2.nkq = 8; g2.nkq_alloc = 8; g2.nks = 8;
@@ -703,6 +738,7 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
         if (n <= 0) return 0;
         r.q0 = q0; r.nq = n; r.ZL = Z; r.P = Pout; r.Wp = with_gram ? w.wpart : nullptr;
         pre(c, st);
+        r.cwt = c->cwt_cur;
         k_vpk_rmul<<<with_gram ? nsplit : std::min(n, c->sms), 256, SMEM_RMUL, st>>>(r);
         if (with_gram) return post(c, st, "k_rmul_gram", 2.0 * 64.0 * n * WP * 80.0 + 2.0 * (double)g.rows * WP * WP);
         return post(c, st, "k_vpk_rmul", 2.0 * 64.0 * n * WP * 80.0);
@@ -712,40 +748,41 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     pg.P = P; pg.ldp = lda; pg.rows = g.rows; pg.p_bulk = ((reinterpret_cast<uintptr_t>(P) & 15) == 0) && ((lda & 1) == 0);
     pg.vpk = vpk; pg.nq = nq; pg.nchunks = nchunks; pg.Wp = w.wpart; pg.pstride = pstride;
     pre(c, st);
+    pg.cwt = c->cwt_cur;
     k_pack_gram<<<nsplit, (GS_MMA_WARPS + PG_PROD_WARPS) * 32, SMEM_GRAM_SYM, st>>>(pg);
     TRY(post(c, st, "k_gram128", 2.0 * (double)g.rows * WP * WP));
     pre(c, st);
-    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum);
+    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum, c->cwt_cur);
     TRY(post(c, st, "k_wreduce"));
     pre(c, st);
-    k_chol128<<<1, 512, SMEM_WIDE1, st>>>(w.wsum, R1, Z1, c->wctl, step, vflag, c->wide_kappa, stamps);
+    k_chol128<<<1, 512, SMEM_WIDE1, st>>>(w.wsum, R1, Z1, c->wctl, step, vflag, c->wide_kappa, stamps, c->cwt_cur);
     TRY(post(c, st, "k_chol128"));
     TRY(rmul(0, nq, Z1, nullptr, true));    // Q1, and the partials of the second Gram matrix Q1'Q1
     pre(c, st);
-    k_gram2_finish<<<256, 256, 0, st>>>(w.wpart, pstride, nsplit, w.wsum, R2, Z2, c->wctl, step, vflag);
+    k_gram2_finish<<<256, 256, 0, st>>>(w.wpart, pstride, nsplit, w.wsum, R2, Z2, c->wctl, step, vflag, c->cwt_cur);
     TRY(post(c, st, "k_gram2_finish"));
     // Two small kernels sit beside the chain, not in it (their own high-priority stream, unless the per-launch profile or the
     // debug sync asks for plain stream order): Rt = R2 R1 overlaps the solve of the top chunks, k_trecon the last pass
     cudaStream_t sx = (!c->profile && !c->sync) ? c->aux_stream : st;
     if (sx != st) { CU(cudaEventRecord(c->ev_aux[0], st)); CU(cudaStreamWaitEvent(sx, c->ev_aux[0], 0)); }
     pre(c, sx);
-    k_trimm128<<<10, 256, SMEM_TRIMM, sx>>>(R2, R1, Rt, c->wctl, step);
+    k_trimm128<<<10, 256, SMEM_TRIMM, sx>>>(R2, R1, Rt, c->wctl, step, c->cwt_cur);
     TRY(post(c, sx, "k_trimm128"));
     if (sx != st) CU(cudaEventRecord(c->ev_aux[1], sx));
     TRY(rmul(0, 2, Z2, nullptr, false));
     if (sx != st) CU(cudaStreamWaitEvent(st, c->ev_aux[1], 0));
     pre(c, st);
-    k_hr128<<<1, 512, SMEM_WIDE1, st>>>(vpk, Rt, P, lda, alpha + p.c, Rr, MT, c->wctl, step, stamps ? stamps + 16 : nullptr);
+    k_hr128<<<1, 512, SMEM_WIDE1, st>>>(vpk, Rt, P, lda, alpha + p.c, Rr, MT, c->wctl, step, stamps ? stamps + 16 : nullptr, c->cwt_cur);
     TRY(post(c, st, "k_hr128"));
     if (linv_out) {     // T' of the panel from the reconstruction: the owner's next block update needs neither V'V nor k_tinv
         if (sx != st) { CU(cudaEventRecord(c->ev_aux[2], st)); CU(cudaStreamWaitEvent(sx, c->ev_aux[2], 0)); }
         pre(c, sx);
-        k_trecon<<<4, 256, SMEM_TRECON, sx>>>(vpk, MT, linv_out, c->wctl, step);
+        k_trecon<<<4, 256, SMEM_TRECON, sx>>>(vpk, MT, linv_out, c->wctl, step, c->cwt_cur);
         TRY(post(c, sx, "k_trecon"));
         if (sx != st) CU(cudaEventRecord(c->ev_aux[3], sx));
     }
     pre(c, st);
-    k_trimm_z<<<10, 256, SMEM_TRIMM, st>>>(Rr, R2, Z23, c->wctl, step);
+    k_trimm_z<<<10, 256, SMEM_TRIMM, st>>>(Rr, R2, Z23, c->wctl, step, c->cwt_cur);
     TRY(post(c, st, "k_trimm_z"));
     TRY(rmul(2, nq - 2, Z23, P, false));
     if (linv_out && sx != st) CU(cudaStreamWaitEvent(st, c->ev_aux[3], 0));   // T' is part of the panel's result
@@ -756,7 +793,8 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
 static int factor_outer_panel(dhqr_context* c, cudaStream_t st, double* vpk, dhqr_context::WSet& w, const Panel& p, int64_t m,
                               int64_t col0, double* A, int64_t lda, double* alpha, int step, bool wide, double* linv_out = nullptr) {
     if (c->wctl) {   // clear the guards of the previous panel and the verdict that travels with this V buffer
-        k_wide_begin<<<1, 32, 0, st>>>(c->wctl, vpk + KC1);
+        cwt_open(c, st);
+        k_wide_begin<<<1, 32, 0, st>>>(c->wctl, vpk + KC1, c->cwt_cur);
         TRY(post(c, st, "k_wide_begin"));
     }
     if (wide) return factor_outer_panel_wide(c, st, vpk, w, p, m, col0, A, lda, alpha, step, linv_out);
@@ -954,6 +992,14 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     int rc = 0;
     cudaEvent_t fork = nullptr, hpdone = nullptr;
     do {
+        if (c->chain_wait_trace && c->cwt_stamps) {   // starts to ~0 (atomicMin), ends to 0 (atomicMax), in stream order
+            for (auto& r : c->cwt_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
+            c->cwt_recs.clear();
+            c->cwt_rows.clear();
+            c->cwt_unit = 0;
+            if (cudaMemset2DAsync(c->cwt_stamps, 16, 0xFF, 8, CWT_MAX, st) != cudaSuccess ||
+                cudaMemset2DAsync(c->cwt_stamps + 1, 16, 0, 8, CWT_MAX, st) != cudaSuccess) { rc = set_err(1002, "chain_wait_trace reset failed"); break; }
+        }
         if (cudaEventCreateWithFlags(&fork, evflags) != cudaSuccess) { rc = set_err(1001, "event create failed"); break; }
         cudaEventRecord(fork, st);
         cudaStreamWaitEvent(hp, fork, 0);                          // hp starts after everything already queued on st
@@ -969,6 +1015,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             const Panel& p = P(k);
             const PanelGeom g = panel_geom(p, m);
             const double* vk = c->vpk2[k % 3];
+            c->cwt_unit = k + 1;   // chain launches of this step end with unit k + 1 factored (unit 0: before the loop)
             const int pk = units[k].a;                                                   // first panel of the unit
             const int64_t t0 = uend(k);                                                  // first trailing column
             const int64_t t1 = k + 1 < K ? uend(k + 1) : t0;                             // end of unit k+1
@@ -1003,6 +1050,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             }
             double* lk = c->tslot(pk);
             bool haveT = ownT[k];                                        // T'_k in lk (this rank)
+            bool hp2_gate = false;                                       // evA2[k] already marks where hp2 may start on hp
             if (k + 1 < K) {
                 // vpk[(k+1)%3] was last read by the bulk update k-2 (and, on the owner of panel k-2, by its broadcast)
                 if (k - 2 >= K0) {
@@ -1019,6 +1067,9 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
                         haveT = true;
                         if (!hadT) cudaEventRecord(evNext[k], hp);       // T'_k is in the ring: the bulk update may start
                     }
+                    // hp2 needs nothing of the factorisation of unit k+1 below: it neither touches nor gates on its columns
+                    cudaEventRecord(evA2[k], hp);
+                    hp2_gate = true;
                     bool widen = false;
                     if ((rc = factor_unit(c, hp, units[k + 1], c->vpk2[(k + 1) % 3], c->vpkb[(k + 1) % 3], c->ws[1], panels, pl, m, col0, A,
                                           lda, alpha, c->tslot(units[k + 1].a), &widen))) break;
@@ -1027,12 +1078,12 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
                 if ((rc = publish(k + 1))) break;
             }
             // columns of panel k+2: their V_0..V_{k-1} come from the bulk updates up to k-1.  This apply is off the chain's
-            // stream (it overlaps the factorisation of panel k+1); the chain picks it up through evA2[k] before it applies
+            // stream and overlaps the factorisation of panel k+1; the chain picks it up through evA2[k] before it applies
             // V_{k+1} to the same columns.
             if (clip(t1, t2, lo, hi)) {
                 cudaStream_t s2 = c->hp2_stream;
-                cudaEventRecord(evA2[k], hp);                            // (used as a scratch event first: order s2 behind hp so far,
-                cudaStreamWaitEvent(s2, evA2[k], 0);                     //  i.e. behind T'_k and behind the last reader of workspace set 2)
+                if (!hp2_gate) cudaEventRecord(evA2[k], hp);             // (used as a scratch event first: order s2 behind hp's
+                cudaStreamWaitEvent(s2, evA2[k], 0);                     //  work up to T'_k, not behind the factorisation of k+1)
                 if (k - 1 >= K0) cudaStreamWaitEvent(s2, evBulk[k - 1], 0);
                 wait_panel(s2, k);
                 const bool hadT = haveT;
@@ -1063,6 +1114,23 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
         if (c->nranks > 1) {
             cudaEventRecord(evHp[K - 1], hp);                      // (re-recorded: everything queued on hp)
             cudaStreamWaitEvent(st, evHp[K - 1], 0);
+        }
+        if (c->chain_wait_trace && c->cwt_stamps) {
+            for (cudaStream_t s : {st, hp, c->hp2_stream, c->aux_stream}) cudaStreamSynchronize(s);
+            std::vector<unsigned long long> t(2 * c->cwt_recs.size());
+            if (!t.empty() && cudaMemcpy(t.data(), c->cwt_stamps, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) {
+                rc = set_err(1002, "chain_wait_trace read-back failed");
+                break;
+            }
+            for (size_t i = 0; i < c->cwt_recs.size(); ++i) {
+                const auto& r = c->cwt_recs[i];
+                float span = 0.f;
+                cudaEventElapsedTime(&span, r.e0, r.e1);
+                const bool stamped = t[2 * i] != ~0ull && t[2 * i + 1] >= t[2 * i];   // kernels without a CwtScope: -1
+                const double run = stamped ? (double)(t[2 * i + 1] - t[2 * i]) * 1e-6 : -1.0;
+                const double row[6] = {(double)r.unit, (double)r.stream, (double)r.cls, (double)span, run, stamped ? span - run : -1.0};
+                c->cwt_rows.insert(c->cwt_rows.end(), row, row + 6);
+            }
         }
         if (c->la_trace) {
             cudaStreamSynchronize(st);
@@ -1532,7 +1600,7 @@ int dhqr_destroy(dhqr_handle c) {
     cudaFree(c->uw_flags);
     cudaFree(c->qt_T); cudaFree(c->qt_part); cudaFree(c->qt_ticket);
     cudaFree(c->wctl); cudaFree(c->wbuf); cudaFree(c->wstamps); cudaFree(c->bs_cells);
-    cudaFree(c->cells); cudaFree(c->cells2); cudaFree(c->fast_stats); cudaFree(c->panel_trace);
+    cudaFree(c->cells); cudaFree(c->cells2); cudaFree(c->fast_stats); cudaFree(c->panel_trace); cudaFree(c->cwt_stamps);
     if (c->hp_stream) cudaStreamDestroy(c->hp_stream);
     if (c->comm_stream) cudaStreamDestroy(c->comm_stream);
     if (c->hp2_stream) cudaStreamDestroy(c->hp2_stream);
@@ -1597,6 +1665,9 @@ int dhqr_set_option(dhqr_handle c, const char* key, int64_t value) {
         c->cvy_persist = (int)value;
     } else if (!strcmp(key, "la_trace")) {
         c->la_trace = value ? 1 : 0;
+    } else if (!strcmp(key, "chain_wait_trace")) {
+        if (value && !c->cwt_stamps) CU(cudaMalloc((void**)&c->cwt_stamps, sizeof(unsigned long long) * 2 * CWT_MAX));
+        c->chain_wait_trace = value ? 1 : 0;
     } else if (!strcmp(key, "panel_fast")) {
         c->panel_fast = value ? 1 : 0;
     } else if (!strcmp(key, "wide_panel")) {
@@ -2519,6 +2590,13 @@ int dhqr_debug_copy_f64(dhqr_handle c, const char* which, double* d_dst, int64_t
     if (!d_dst) return set_err(-3, "null destination");
     if (!strcmp(which, "la_times")) {   // host-side list: converted to doubles and copied to the device buffer
         std::vector<double> t(c->la_times.begin(), c->la_times.end());
+        if ((size_t)nelems < t.size()) return set_err(-4, "need %zu elements", t.size());
+        CU(cudaMemcpy(d_dst, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice));
+        return 0;
+    }
+    if (!strcmp(which, "chain_wait")) {   // [0] = launches of the last look-ahead factorisation, then 6 doubles per launch
+        std::vector<double> t(1, (double)(c->cwt_rows.size() / 6));
+        t.insert(t.end(), c->cwt_rows.begin(), c->cwt_rows.end());
         if ((size_t)nelems < t.size()) return set_err(-4, "need %zu elements", t.size());
         CU(cudaMemcpy(d_dst, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice));
         return 0;

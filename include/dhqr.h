@@ -95,7 +95,11 @@ int dhqr_destroy(dhqr_handle h);
  *                 on the device, nb = 1 as one persistent launch (m <= 8192), nb = 1 with the next reflector formed inside the
  *                 apply kernel, where the shape allows; 0: the per-block / per-column launches those paths otherwise take
  *   "wide_kappa"  guard of the 128-column chain on ||D R1^{-1}||_F of its first Cholesky factor (default 1000)
- *   traces:       "panel_trace", "la_trace", "wide_trace" (timestamps read with dhqr_debug_copy_f64)
+ *   traces:       "panel_trace", "la_trace", "wide_trace" (timestamps read with dhqr_debug_copy_f64); "chain_wait_trace" 1:
+ *                 under the look-ahead schedule, CUDA events around every launch on the chain's streams and %globaltimer
+ *                 stamps of its first CTA start and last warp end ("chain_wait": [0] = launches, then per launch unit,
+ *                 stream (0 chain, 1 second apply, 2 side kernels), class index for dhqr_profile_get, event span, stamp
+ *                 span, their difference, in ms; -1 for a launch without stamps)
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
