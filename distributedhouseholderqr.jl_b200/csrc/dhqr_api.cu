@@ -12,6 +12,7 @@
 #include <time.h>
 
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "dhqr_kernels.cuh"
@@ -143,9 +144,7 @@ struct dhqr_context {
     // the CwtScope stamps of the same launch, so that the time a launch was ready but had no SM can be told from its run time
     int chain_wait_trace = 0;
     unsigned long long* cwt_stamps = nullptr;                           // [CWT_MAX][2]: first CTA start, last warp end (%globaltimer ns)
-    unsigned long long* cwt_cur = nullptr;                              // slot of the launch between pre() and post(); null: not traced
-    cudaEvent_t cwt_e0 = nullptr;
-    int cwt_unit = 0, cwt_stream = 0;
+    int cwt_unit = 0;                                                   // unit of the look-ahead step being enqueued
     struct CwtRec { int unit, stream, cls; cudaEvent_t e0, e1; };
     std::vector<CwtRec> cwt_recs;
     std::vector<double> cwt_rows;                                       // [launch][6]: unit, stream, class, event span, stamp span, wait (ms)
@@ -213,7 +212,6 @@ struct dhqr_context {
     struct ProfSlot { const char* name; double ms = 0.0; int64_t count = 0; double work = 0.0; };
     std::vector<ProfRec> prof_pending;
     std::vector<ProfSlot> prof_slots;
-    cudaEvent_t prof_open = nullptr;
 };
 
 static constexpr int NBMAX = 128;
@@ -261,6 +259,62 @@ static int set_attrs(dhqr_context* c) {
     c->attrs_set = true;
     return 0;
 }
+
+static int prof_slot(dhqr_context* c, const char* name) {
+    for (size_t i = 0; i < c->prof_slots.size(); ++i)
+        if (!strcmp(c->prof_slots[i].name, name)) return (int)i;
+    dhqr_context::ProfSlot s;
+    s.name = name;
+    c->prof_slots.push_back(s);
+    return (int)c->prof_slots.size() - 1;
+}
+
+// chain_wait_trace: where a launch's kernel leaves its stamps (null: the launch is not traced)
+using CwtSlot = unsigned long long*;
+
+// Every kernel launch goes through here.  `enqueue(cwt)` launches on `st`: a <<<>>> launch returns nothing (its error is read
+// here, with cudaGetLastError), a launch through the runtime API returns its error.  Kernels without a CwtScope ignore the stamp
+// slot `cwt`.  Around the launch go the CUDA-event brackets of option chain_wait_trace (on the chain's streams) and of option
+// "profile" (class `what`, credited with `work`); the launch is counted, and under option "sync" waited for.  A failed launch
+// leaves no bracket behind.
+template <typename Enqueue>
+static int launch(dhqr_context* c, cudaStream_t st, const char* what, double work, Enqueue&& enqueue) {
+    cudaEvent_t cw0 = nullptr, cw1 = nullptr, pf0 = nullptr, pf1 = nullptr;
+    CwtSlot cwt = nullptr;
+    const int cws = st == c->hp_stream ? 0 : st == c->hp2_stream ? 1 : st == c->aux_stream ? 2 : -1;
+    if (c->chain_wait_trace && c->cwt_stamps && c->cwt_recs.size() < (size_t)CWT_MAX && cws >= 0 && cudaEventCreate(&cw0) == cudaSuccess) {
+        cudaEventRecord(cw0, st);
+        cwt = c->cwt_stamps + 2 * c->cwt_recs.size();
+    }
+    if (c->profile && cudaEventCreate(&pf0) == cudaSuccess) cudaEventRecord(pf0, st);
+    cudaError_t e = cudaSuccess;
+    if constexpr (std::is_void_v<decltype(enqueue(cwt))>) enqueue(cwt);
+    else e = enqueue(cwt);
+    c->launches++;
+    if (cw0) { cudaEventCreate(&cw1); cudaEventRecord(cw1, st); }
+    if (pf0) { cudaEventCreate(&pf1); cudaEventRecord(pf1, st); }
+    const cudaError_t e2 = cudaGetLastError();
+    if (e == cudaSuccess) e = e2;
+    if (e != cudaSuccess) {
+        for (cudaEvent_t ev : {cw0, cw1, pf0, pf1})
+            if (ev) cudaEventDestroy(ev);
+        return set_err(1000 + (int)e, "launch of %s failed: %s", what, cudaGetErrorString(e));
+    }
+    if (cw0) c->cwt_recs.push_back({c->cwt_unit, cws, prof_slot(c, what), cw0, cw1});
+    if (pf0) {
+        const int s = prof_slot(c, what);
+        c->prof_pending.push_back({s, pf0, pf1});
+        c->prof_slots[s].work += work;
+    }
+    if (c->sync) {
+        e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return set_err(1000 + (int)e, "%s failed: %s", what, cudaGetErrorString(e));
+    }
+    return 0;
+}
+
+// Every column of `p` starts 16 B aligned (bulk copies legal): `p` itself is, and the leading dimension is even.
+static bool bulk_ok(const void* p, int64_t ld) { return ((uintptr_t)p & 15) == 0 && (ld & 1) == 0; }
 
 // Grows a workspace buffer.  The zero fill goes on `st`, the stream of the call that needs the buffer: a synchronous
 // cudaMemset would run on the legacy default stream, which a non-blocking caller stream is not ordered after.
@@ -315,9 +369,8 @@ static int ensure_workspace(dhqr_context* c, cudaStream_t st, int64_t m, int64_t
     if (!c->wctl) {
         CU(cudaMalloc((void**)&c->wctl, sizeof(WideCtl)));
         CU(cudaMemsetAsync(c->wctl, 0, sizeof(WideCtl), st));
-        k_wide_reset<<<1, 32, 0, st>>>(c->wctl);              // initial state {W_NOFAIL, 0}, in the caller's stream order
-        c->launches++;
-        CU(cudaGetLastError());
+        // initial state {W_NOFAIL, 0}, in the caller's stream order
+        TRY(launch(c, st, "k_wide_reset", 0.0, [&](CwtSlot) { k_wide_reset<<<1, 32, 0, st>>>(c->wctl); }));
         size_t o3 = 0;
         TRY(ensure(&c->wbuf, &o3, (size_t)5 * WP * WP + 3 * XL_ELEMS, st));
         CU(cudaMalloc((void**)&c->wstamps, 32 * sizeof(long long)));
@@ -325,61 +378,6 @@ static int ensure_workspace(dhqr_context* c, cudaStream_t st, int64_t m, int64_t
     }
     TRY(ensure(&c->v1, &c->v1_elems, (size_t)2 * rup(m + 4, 2), st));
     TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)1, st));
-    return 0;
-}
-
-static int prof_slot(dhqr_context* c, const char* name) {
-    for (size_t i = 0; i < c->prof_slots.size(); ++i)
-        if (!strcmp(c->prof_slots[i].name, name)) return (int)i;
-    dhqr_context::ProfSlot s;
-    s.name = name;
-    c->prof_slots.push_back(s);
-    return (int)c->prof_slots.size() - 1;
-}
-// chain_wait_trace: open an event bracket around the next launch when `st` is one of the chain's streams; its kernel gets the
-// stamp slot c->cwt_cur, and post() closes the bracket
-static void cwt_open(dhqr_context* c, cudaStream_t st) {
-    c->cwt_cur = nullptr;
-    if (!c->chain_wait_trace || !c->cwt_stamps || c->cwt_recs.size() >= (size_t)CWT_MAX) return;
-    const int s = st == c->hp_stream ? 0 : st == c->hp2_stream ? 1 : st == c->aux_stream ? 2 : -1;
-    if (s >= 0 && cudaEventCreate(&c->cwt_e0) == cudaSuccess) {
-        cudaEventRecord(c->cwt_e0, st);
-        c->cwt_stream = s;
-        c->cwt_cur = c->cwt_stamps + 2 * c->cwt_recs.size();
-    }
-}
-// pre(): open a CUDA-event bracket on the launching stream when profiling is on (and the chain_wait_trace one)
-static void pre(dhqr_context* c, cudaStream_t st) {
-    cwt_open(c, st);
-    if (!c->profile) return;
-    cudaEventCreate(&c->prof_open);
-    cudaEventRecord(c->prof_open, st);
-}
-static int post(dhqr_context* c, cudaStream_t st, const char* what, double work = 0.0) {
-    c->launches++;
-    if (c->cwt_cur) {
-        dhqr_context::CwtRec r{c->cwt_unit, c->cwt_stream, prof_slot(c, what), c->cwt_e0, nullptr};
-        cudaEventCreate(&r.e1);
-        cudaEventRecord(r.e1, st);
-        c->cwt_recs.push_back(r);
-        c->cwt_cur = nullptr;
-    }
-    if (c->profile && c->prof_open) {
-        dhqr_context::ProfRec r;
-        r.slot = prof_slot(c, what);
-        r.e0 = c->prof_open;
-        cudaEventCreate(&r.e1);
-        cudaEventRecord(r.e1, st);
-        c->prof_pending.push_back(r);
-        c->prof_slots[r.slot].work += work;
-        c->prof_open = nullptr;
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_err(1000 + (int)e, "launch of %s failed: %s", what, cudaGetErrorString(e));
-    if (c->sync) {
-        e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) return set_err(1000 + (int)e, "%s failed: %s", what, cudaGetErrorString(e));
-    }
     return 0;
 }
 
@@ -403,6 +401,44 @@ static int pick_splits(int tiles, int nchunks, int sms, int64_t cap_tiles) {
     return best;
 }
 
+// The kb columns (mp rows) of a Householder block at A -> the first `width` packed columns of vpk, the block's row 0 at window row
+// vtop, zero-filled to vrows rows (k_pack; tril: the block is stored in place in A, zeros above its diagonal)
+static int pack_v(dhqr_context* c, cudaStream_t st, const double* A, int64_t lda, int64_t mp, int kb, int tril, double* vpk, int64_t vtop,
+                  int64_t vrows, int width) {
+    const dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), width);
+    return launch(c, st, "k_pack", 0.0, [&](CwtSlot) { k_pack<<<grid, 256, 0, st>>>(A, lda, mp, kb, tril, vpk, 0, vtop, vrows); });
+}
+
+// Partials of W = V' B -> w.wpart.  V = packed columns [voff, voff + nbp) of vpk, through the 32- or the 128-column kernel as nbp
+// asks; nv > 0: W starts with the nv columns of V'V itself (for T), then come the ncols columns of B (`rows` rows).
+static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_context::WSet& w, int voff, int nbp, int nv,
+                               const double* B, int64_t ldb, int64_t rows, int ncols, const char* what, int* nsplit_out,
+                               int64_t* pstride_out) {
+    const bool small = (nbp <= 32);
+    const int NBPK = small ? 32 : 128;          // kernel instantiation
+    const int bn = small ? G1S_BN : G1_BN;
+    const int tiles = (nv + ncols + bn - 1) / bn;
+    const int nchunks = (int)((rows + KC1 - 1) / KC1);
+    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart_elems / ((size_t)bn * NBPK)));
+    const int64_t pstride = (int64_t)tiles * bn * NBPK;
+    if ((size_t)(pstride * nsplit) > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
+    GemmVtaArgs g1;
+    g1.vpk = vpk; g1.voff = voff; g1.nv = nv;
+    g1.A = B; g1.lda = ldb; g1.rows = rows; g1.na = ncols; g1.nchunks = nchunks;
+    g1.a_aligned = bulk_ok(B, ldb);
+    g1.Wp = w.wpart; g1.pstride = pstride;
+    *nsplit_out = nsplit;
+    *pstride_out = pstride;
+    return launch(c, st, what, 2.0 * (double)rows * nbp * ((double)ncols + nv), [&](CwtSlot cwt) {
+        g1.cwt = cwt;
+        if (small) K_G1_32<<<dim3(tiles, nsplit), (1 * 4 + G1S_NPW) * 32, smem_g1(32, G1S_BN), st>>>(g1);
+        else K_G1_128<<<dim3(tiles, nsplit), (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
+    });
+}
+
+// k_wreduce: one thread per element, at most eight CTAs per SM
+static unsigned wreduce_grid(const dhqr_context* c, int64_t nelem) { return (unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms); }
+
 static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int voff, int nbp, const double* ypk, int64_t rows,
                       int64_t row_lo, double* C, int64_t ldc, int ncols, int gate);
 
@@ -417,58 +453,54 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     if (ncols <= 0 || rows <= 0) return 0;
     const bool small = (nbp <= 32);
     const int NBPK = small ? 32 : 128;          // kernel instantiation
-    const int bn = small ? G1S_BN : G1_BN;
     const int nv = reuse_T ? 0 : NBPK;
     const int next = nv + ncols;
-    const int tiles = (next + bn - 1) / bn;
-    const int nchunks = (int)((rows + KC1 - 1) / KC1);
-    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart_elems / ((size_t)bn * NBPK)));
-    const int64_t pstride = (int64_t)tiles * bn * NBPK;
-    if ((size_t)(pstride * nsplit) > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
     if ((size_t)next * NBPK > w.wsum_elems) return set_err(4003, "internal: W workspace too small");
-    GemmVtaArgs g1;
-    g1.vpk = vpk; g1.voff = voff; g1.nv = nv;
-    g1.A = C; g1.lda = ldc; g1.rows = rows; g1.na = ncols; g1.nchunks = nchunks;
-    g1.a_aligned = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
-    g1.Wp = w.wpart; g1.pstride = pstride;
-    dim3 grid1(tiles, nsplit);
-    pre(c, st);
-    g1.cwt = c->cwt_cur;
-    if (small) {
-        K_G1_32<<<grid1, (1 * 4 + G1S_NPW) * 32, smem_g1(32, G1S_BN), st>>>(g1);
-    } else {
-        K_G1_128<<<grid1, (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
-    }
-    TRY(post(c, st, small ? "k_gemm_vta32" : "k_gemm_vta128", 2.0 * (double)rows * nbp * ((double)ncols + nv)));
+    int nsplit = 0;
+    int64_t pstride = 0;
+    TRY(launch_vta_partials(c, st, vpk, w, voff, nbp, nv, C, ldc, rows, ncols, small ? "k_gemm_vta32" : "k_gemm_vta128", &nsplit,
+                            &pstride));
     const int ygrid = (ncols + YCOLS - 1) / YCOLS;
     if (small && !reuse_T) {
-        pre(c, st);
-        k_mid32<<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, linv, trans);
-        TRY(post(c, st, "k_mid32"));
+        TRY(launch(c, st, "k_mid32", 0.0, [&](CwtSlot) {
+            k_mid32<<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, linv, trans);
+        }));
     } else {
-        pre(c, st);
         const int64_t nelem = (int64_t)next * NBPK;
-        k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, w.wsum, c->cwt_cur);
-        TRY(post(c, st, "k_wreduce"));
+        TRY(launch(c, st, "k_wreduce", 0.0, [&](CwtSlot cwt) {
+            k_wreduce<<<wreduce_grid(c, nelem), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, w.wsum, cwt);
+        }));
         if (!reuse_T) {
-            pre(c, st);
-            if (small) k_tinv<32><<<1, 512, smem_tinv(32), st>>>(w.wsum, linv, 0, c->cwt_cur);
-            else k_tinv<128><<<1, 512, smem_tinv(128), st>>>(w.wsum, linv, 0, c->cwt_cur);
-            TRY(post(c, st, small ? "k_tinv32" : "k_tinv128"));
+            TRY(launch(c, st, small ? "k_tinv32" : "k_tinv128", 0.0, [&](CwtSlot cwt) {
+                if (small) k_tinv<32><<<1, 512, smem_tinv(32), st>>>(w.wsum, linv, 0, cwt);
+                else k_tinv<128><<<1, 512, smem_tinv(128), st>>>(w.wsum, linv, 0, cwt);
+            }));
         }
-        pre(c, st);
-        if (small) k_ymake<32><<<ygrid, 256, smem_ymake(32), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans, c->cwt_cur);
-        else k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans, c->cwt_cur);
-        TRY(post(c, st, small ? "k_ymake32" : "k_ymake128"));
+        TRY(launch(c, st, small ? "k_ymake32" : "k_ymake128", 0.0, [&](CwtSlot cwt) {
+            if (small) k_ymake<32><<<ygrid, 256, smem_ymake(32), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans, cwt);
+            else k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, nv, ncols, linv, w.ypk, trans, cwt);
+        }));
     }
     return launch_cvy(c, st, vpk, voff, nbp, w.ypk, rows, row_lo, C, ldc, ncols, gate);
 }
 
+// The arguments of C += V Y that come from C and the schedule: the 128 x 64 tiles over C, how many of them one CTA of the
+// persistent variant walks through, whether C moves by bulk copies, and the gate of the speculative panel chain
+static GemmCvyArgs cvy_args(const dhqr_context* c, double* C, int64_t ldc, int64_t rows, int ncols, int gate) {
+    GemmCvyArgs g2;
+    g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.ncols = ncols;
+    g2.tiles_m = (int)((rows + G2_BM - 1) / G2_BM); g2.tiles_n = (ncols + G2_BN - 1) / G2_BN;
+    g2.tiles_per_cta = std::max(c->cvy_persist, 1);   // cvy_persist = 0: one tile per CTA
+    g2.c_bulk = bulk_ok(C, ldc);
+    g2.ctl = c->wctl; g2.gate = gate;
+    return g2;
+}
+
 // k_gemm_cvy_p: one CTA pair per `tiles_per_cta` consecutive pair-tiles (a row tile by two adjacent column tiles)
-static void launch_cvy_p(const GemmCvyArgs& g2, cudaStream_t st) {
+static unsigned cvy_p_grid(const GemmCvyArgs& g2) {
     const int npairs = g2.tiles_m * ((g2.tiles_n + 1) / 2);
     const int clusters = (npairs + g2.tiles_per_cta - 1) / g2.tiles_per_cta;
-    k_gemm_cvy_p<<<clusters * CVYP_CLUSTER, CVYP_THREADS, smem_g2p(), st>>>(g2);
+    return clusters * CVYP_CLUSTER;
 }
 
 // C += V Y on window rows >= row_lo, Y packed in the ypk layout (nbp <= 32: one k-chunk per column tile; else NBMAX / KC):
@@ -477,43 +509,17 @@ static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int v
                       int64_t row_lo, double* C, int64_t ldc, int ncols, int gate) {
     const bool small = (nbp <= 32);
     const int NBPK = small ? 32 : 128;
-    pre(c, st);
-    GemmCvyArgs g2;
-    g2.cwt = c->cwt_cur;
-    g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.row_lo = row_lo; g2.ncols = ncols;
+    GemmCvyArgs g2 = cvy_args(c, C, ldc, rows, ncols, gate);
+    g2.row_lo = row_lo;
     g2.vpk = vpk; g2.voff = voff; g2.ypk = ypk;
     g2.nkq = small ? 1 : (int)(rup(nbp, KC) / KC); g2.nkq_alloc = NBPK / KC;
-    g2.ctl = c->wctl; g2.gate = gate;
-    dim3 grid2((unsigned)((rows + G2_BM - 1) / G2_BM), (unsigned)((ncols + G2_BN - 1) / G2_BN));
-    g2.tiles_m = (int)grid2.x; g2.tiles_n = (int)grid2.y;
-    g2.tiles_per_cta = std::max(c->cvy_persist, 1);   // cvy_persist = 0: one tile per CTA
-    g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
     g2.nks = 4; g2.vpk2 = nullptr;
-    if (g2.nkq == 4) launch_cvy_p(g2, st);
-    else k_gemm_cvy<<<grid2, 9 * 32, smem_g2(), st>>>(g2);
-    TRY(post(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols));
-    return 0;
-}
-
-// Partials of W = V' B (V: the 128 packed columns of vpk, B: ncols columns of user storage, `rows` rows) -> w.wpart.
-static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_context::WSet& w, const double* B, int64_t ldb,
-                               int64_t rows, int ncols, const char* what, int* nsplit_out, int64_t* pstride_out) {
-    const int tiles = (ncols + G1_BN - 1) / G1_BN;
-    const int nchunks = (int)((rows + KC1 - 1) / KC1);
-    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart_elems / ((size_t)G1_BN * NBMAX)));
-    const int64_t pstride = (int64_t)tiles * G1_BN * NBMAX;
-    if ((size_t)(pstride * nsplit) > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
-    GemmVtaArgs g1;
-    g1.vpk = vpk; g1.voff = 0; g1.nv = 0;
-    g1.A = B; g1.lda = ldb; g1.rows = rows; g1.na = ncols; g1.nchunks = nchunks;
-    g1.a_aligned = (((uintptr_t)B & 15) == 0 && (ldb & 1) == 0) ? 1 : 0;
-    g1.Wp = w.wpart; g1.pstride = pstride;
-    pre(c, st);
-    g1.cwt = c->cwt_cur;
-    K_G1_128<<<dim3(tiles, nsplit), (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
-    *nsplit_out = nsplit;
-    *pstride_out = pstride;
-    return post(c, st, what, 2.0 * (double)rows * NBMAX * ncols);
+    return launch(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols,
+                  [&](CwtSlot cwt) {
+                      g2.cwt = cwt;
+                      if (g2.nkq == 4) k_gemm_cvy_p<<<cvy_p_grid(g2), CVYP_THREADS, smem_g2p(), st>>>(g2);
+                      else k_gemm_cvy<<<dim3(g2.tiles_m, g2.tiles_n), 9 * 32, smem_g2(), st>>>(g2);
+                  });
 }
 
 // W = V' C for one 128-column block -> Ws (128 x ncols, col-major), T' reused
@@ -521,11 +527,11 @@ static int block_w(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_con
                    int ncols, double* Ws) {
     int nsplit = 0;
     int64_t pstride = 0;
-    TRY(launch_vta_partials(c, st, vpk, w, C, ldc, rows, ncols, "k_gemm_vta128", &nsplit, &pstride));
-    pre(c, st);
+    TRY(launch_vta_partials(c, st, vpk, w, 0, NBMAX, 0, C, ldc, rows, ncols, "k_gemm_vta128", &nsplit, &pstride));
     const int64_t nelem = (int64_t)ncols * NBMAX;
-    k_wreduce<<<(unsigned)std::min<int64_t>((nelem + 255) / 256, 8 * c->sms), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, Ws, c->cwt_cur);
-    return post(c, st, "k_wreduce");
+    return launch(c, st, "k_wreduce", 0.0, [&](CwtSlot cwt) {
+        k_wreduce<<<wreduce_grid(c, nelem), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, Ws, cwt);
+    });
 }
 
 // G = V_b' V_a of a panel pair (a = panel at column ca, b = the next 128 columns) into gout.  Below row ca + 128 the columns of
@@ -534,10 +540,11 @@ static int form_pair_gram(dhqr_context* c, cudaStream_t st, const double* vpk_b,
                           int64_t col0, int64_t ca, int64_t m, double* gout) {
     int nsplit = 0;
     int64_t pstride = 0;
-    TRY(launch_vta_partials(c, st, vpk_b, w, A + (ca - col0) * lda + ca + WP, lda, m - ca - WP, WP, "k_gram_pair", &nsplit, &pstride));
-    pre(c, st);
-    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, gout, c->cwt_cur);
-    return post(c, st, "k_wreduce");
+    TRY(launch_vta_partials(c, st, vpk_b, w, 0, NBMAX, 0, A + (ca - col0) * lda + ca + WP, lda, m - ca - WP, WP, "k_gram_pair", &nsplit,
+                            &pstride));
+    return launch(c, st, "k_wreduce", 0.0, [&](CwtSlot cwt) {
+        k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, gout, cwt);
+    });
 }
 
 // Two 128-column blocks a then b in one pass over C:  C <- (I - V_b T_b' V_b')(I - V_a T_a' V_a') C,  i.e.  C += [V_a V_b] [Y_a; Y_b]
@@ -550,21 +557,17 @@ static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const
     double* Wa = w.wsum, *Wb = w.wsum + (size_t)ncols * NBMAX;
     TRY(block_w(c, st, vpa, w, C, ldc, rows, ncols, Wa));
     TRY(block_w(c, st, vpb, w, C + WP, ldc, rows - WP, ncols, Wb));
-    pre(c, st);
-    k_ymake2<<<(ncols + YCOLS - 1) / YCOLS, 256, SMEM_YMAKE2, st>>>(Wa, Wb, ncols, Ta, Tb, G, w.ypk, c->cwt_cur);
-    TRY(post(c, st, "k_ymake2"));
-    pre(c, st);
-    GemmCvyArgs g2;
-    g2.cwt = c->cwt_cur;
-    g2.C = C; g2.ldc = ldc; g2.rows = rows; g2.row_lo = 0; g2.ncols = ncols;
+    TRY(launch(c, st, "k_ymake2", 0.0, [&](CwtSlot cwt) {
+        k_ymake2<<<(ncols + YCOLS - 1) / YCOLS, 256, SMEM_YMAKE2, st>>>(Wa, Wb, ncols, Ta, Tb, G, w.ypk, cwt);
+    }));
+    GemmCvyArgs g2 = cvy_args(c, C, ldc, rows, ncols, gate);
+    g2.row_lo = 0;
     g2.vpk = vpa; g2.voff = 0; g2.vpk2 = vpb; g2.ypk = w.ypk;
     g2.nkq = 8; g2.nkq_alloc = 8; g2.nks = 8;
-    g2.ctl = c->wctl; g2.gate = gate;
-    g2.tiles_m = (int)((rows + G2_BM - 1) / G2_BM); g2.tiles_n = (ncols + G2_BN - 1) / G2_BN;
-    g2.tiles_per_cta = std::max(c->cvy_persist, 1);
-    g2.c_bulk = (((uintptr_t)C & 15) == 0 && (ldc & 1) == 0) ? 1 : 0;
-    launch_cvy_p(g2, st);
-    return post(c, st, "k_gemm_cvy256", 2.0 * ((double)rows * WP + (double)(rows - WP) * WP) * (double)ncols);
+    return launch(c, st, "k_gemm_cvy256", 2.0 * ((double)rows * WP + (double)(rows - WP) * WP) * (double)ncols, [&](CwtSlot cwt) {
+        g2.cwt = cwt;
+        k_gemm_cvy_p<<<cvy_p_grid(g2), CVYP_THREADS, smem_g2p(), st>>>(g2);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -597,11 +600,11 @@ static int launch_panel(dhqr_context* c, cudaStream_t st, double* vpk, double* P
     a.cells2 = c->cells2; a.fast = c->panel_fast; a.fast_stats = c->fast_stats;
     a.ctl = c->wctl; a.gate = gate;
     void* args[] = {&a};
-    pre(c, st);
-    cudaError_t e = cudaLaunchCooperativeKernel((void*)k_panel, dim3(G), dim3(PANEL_THREADS), args, smem, st);
-    if (e != cudaSuccess) return set_err(1000 + (int)e, "cooperative launch of k_panel failed: %s", cudaGetErrorString(e));
-    c->ll_epoch += IB + 8;
-    return post(c, st, "k_panel", 16.0 * (double)mp * ncols);   // work = bytes: panel read once + written once
+    return launch(c, st, "k_panel", 16.0 * (double)mp * ncols, [&](CwtSlot) {   // work = bytes: panel read once + written once
+        const cudaError_t e = cudaLaunchCooperativeKernel((void*)k_panel, dim3(G), dim3(PANEL_THREADS), args, smem, st);
+        if (e == cudaSuccess) c->ll_epoch += IB + 8;   // the launch has used the tags up to here
+        return e;
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -681,8 +684,9 @@ static int factor_outer_panel_narrow(dhqr_context* c, cudaStream_t st, double* v
                                       nullptr, step));
     }
     if (g.nbp > IB && g.nbp < NBMAX) {   // zero the V columns the 128-wide kernels read beyond nbp
-        k_vpk_zero_cols<<<2 * c->sms, 256, 0, st>>>(vpk, g.vrows / KC1, g.nbp, NBMAX);
-        TRY(post(c, st, "k_vpk_zero_cols"));
+        TRY(launch(c, st, "k_vpk_zero_cols", 0.0, [&](CwtSlot) {
+            k_vpk_zero_cols<<<2 * c->sms, 256, 0, st>>>(vpk, g.vrows / KC1, g.nbp, NBMAX);
+        }));
     }
     return 0;
 }
@@ -707,11 +711,11 @@ static int launch_panel_gram(dhqr_context* c, cudaStream_t st, const double* vpk
     TRY(panel_gram_split(c, w, rows, &nchunks, &nsplit));
     GramSymArgs g;
     g.vpk = vpk; g.nchunks = nchunks; g.Wp = w.wpart; g.pstride = pstride;
-    pre(c, st);
-    k_gram_sym<<<nsplit, (GS_MMA_WARPS + 1) * 32, SMEM_GRAM_SYM, st>>>(g);
     *nsplit_out = nsplit;
     *pstride_out = pstride;
-    return post(c, st, "k_gram128", 2.0 * (double)rows * WP * WP);
+    return launch(c, st, "k_gram128", 2.0 * (double)rows * WP * WP, [&](CwtSlot) {
+        k_gram_sym<<<nsplit, (GS_MMA_WARPS + 1) * 32, SMEM_GRAM_SYM, st>>>(g);
+    });
 }
 
 // the 128-column chain (dhqr_wide.cuh): CholeskyQR2 + Householder reconstruction of a full aligned outer panel
@@ -737,53 +741,49 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     auto rmul = [&](int q0, int n, const double* Z, double* Pout, bool with_gram) -> int {
         if (n <= 0) return 0;
         r.q0 = q0; r.nq = n; r.ZL = Z; r.P = Pout; r.Wp = with_gram ? w.wpart : nullptr;
-        pre(c, st);
-        r.cwt = c->cwt_cur;
-        k_vpk_rmul<<<with_gram ? nsplit : std::min(n, c->sms), 256, SMEM_RMUL, st>>>(r);
-        if (with_gram) return post(c, st, "k_rmul_gram", 2.0 * 64.0 * n * WP * 80.0 + 2.0 * (double)g.rows * WP * WP);
-        return post(c, st, "k_vpk_rmul", 2.0 * 64.0 * n * WP * 80.0);
+        const double work = 2.0 * 64.0 * n * WP * 80.0 + (with_gram ? 2.0 * (double)g.rows * WP * WP : 0.0);
+        return launch(c, st, with_gram ? "k_rmul_gram" : "k_vpk_rmul", work, [&](CwtSlot cwt) {
+            r.cwt = cwt;
+            k_vpk_rmul<<<with_gram ? nsplit : std::min(n, c->sms), 256, SMEM_RMUL, st>>>(r);
+        });
     };
     // pack + first Gram: the chunks go from the caller's matrix into the Gram kernel's tiles, and from there to vpk
     PackGramArgs pg;
-    pg.P = P; pg.ldp = lda; pg.rows = g.rows; pg.p_bulk = ((reinterpret_cast<uintptr_t>(P) & 15) == 0) && ((lda & 1) == 0);
+    pg.P = P; pg.ldp = lda; pg.rows = g.rows; pg.p_bulk = bulk_ok(P, lda);
     pg.vpk = vpk; pg.nq = nq; pg.nchunks = nchunks; pg.Wp = w.wpart; pg.pstride = pstride;
-    pre(c, st);
-    pg.cwt = c->cwt_cur;
-    k_pack_gram<<<nsplit, (GS_MMA_WARPS + PG_PROD_WARPS) * 32, SMEM_GRAM_SYM, st>>>(pg);
-    TRY(post(c, st, "k_gram128", 2.0 * (double)g.rows * WP * WP));
-    pre(c, st);
-    k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum, c->cwt_cur);
-    TRY(post(c, st, "k_wreduce"));
-    pre(c, st);
-    k_chol128<<<1, 512, SMEM_WIDE1, st>>>(w.wsum, R1, Z1, c->wctl, step, vflag, c->wide_kappa, stamps, c->cwt_cur);
-    TRY(post(c, st, "k_chol128"));
+    TRY(launch(c, st, "k_gram128", 2.0 * (double)g.rows * WP * WP, [&](CwtSlot cwt) {
+        pg.cwt = cwt;
+        k_pack_gram<<<nsplit, (GS_MMA_WARPS + PG_PROD_WARPS) * 32, SMEM_GRAM_SYM, st>>>(pg);
+    }));
+    TRY(launch(c, st, "k_wreduce", 0.0, [&](CwtSlot cwt) {
+        k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum, cwt);
+    }));
+    TRY(launch(c, st, "k_chol128", 0.0, [&](CwtSlot cwt) {
+        k_chol128<<<1, 512, SMEM_WIDE1, st>>>(w.wsum, R1, Z1, c->wctl, step, vflag, c->wide_kappa, stamps, cwt);
+    }));
     TRY(rmul(0, nq, Z1, nullptr, true));    // Q1, and the partials of the second Gram matrix Q1'Q1
-    pre(c, st);
-    k_gram2_finish<<<256, 256, 0, st>>>(w.wpart, pstride, nsplit, w.wsum, R2, Z2, c->wctl, step, vflag, c->cwt_cur);
-    TRY(post(c, st, "k_gram2_finish"));
+    TRY(launch(c, st, "k_gram2_finish", 0.0, [&](CwtSlot cwt) {
+        k_gram2_finish<<<256, 256, 0, st>>>(w.wpart, pstride, nsplit, w.wsum, R2, Z2, c->wctl, step, vflag, cwt);
+    }));
     // Two small kernels sit beside the chain, not in it (their own high-priority stream, unless the per-launch profile or the
     // debug sync asks for plain stream order): Rt = R2 R1 overlaps the solve of the top chunks, k_trecon the last pass
     cudaStream_t sx = (!c->profile && !c->sync) ? c->aux_stream : st;
     if (sx != st) { CU(cudaEventRecord(c->ev_aux[0], st)); CU(cudaStreamWaitEvent(sx, c->ev_aux[0], 0)); }
-    pre(c, sx);
-    k_trimm128<<<10, 256, SMEM_TRIMM, sx>>>(R2, R1, Rt, c->wctl, step, c->cwt_cur);
-    TRY(post(c, sx, "k_trimm128"));
+    TRY(launch(c, sx, "k_trimm128", 0.0, [&](CwtSlot cwt) { k_trimm128<<<10, 256, SMEM_TRIMM, sx>>>(R2, R1, Rt, c->wctl, step, cwt); }));
     if (sx != st) CU(cudaEventRecord(c->ev_aux[1], sx));
     TRY(rmul(0, 2, Z2, nullptr, false));
     if (sx != st) CU(cudaStreamWaitEvent(st, c->ev_aux[1], 0));
-    pre(c, st);
-    k_hr128<<<1, 512, SMEM_WIDE1, st>>>(vpk, Rt, P, lda, alpha + p.c, Rr, MT, c->wctl, step, stamps ? stamps + 16 : nullptr, c->cwt_cur);
-    TRY(post(c, st, "k_hr128"));
+    TRY(launch(c, st, "k_hr128", 0.0, [&](CwtSlot cwt) {
+        k_hr128<<<1, 512, SMEM_WIDE1, st>>>(vpk, Rt, P, lda, alpha + p.c, Rr, MT, c->wctl, step, stamps ? stamps + 16 : nullptr, cwt);
+    }));
     if (linv_out) {     // T' of the panel from the reconstruction: the owner's next block update needs neither V'V nor k_tinv
         if (sx != st) { CU(cudaEventRecord(c->ev_aux[2], st)); CU(cudaStreamWaitEvent(sx, c->ev_aux[2], 0)); }
-        pre(c, sx);
-        k_trecon<<<4, 256, SMEM_TRECON, sx>>>(vpk, MT, linv_out, c->wctl, step, c->cwt_cur);
-        TRY(post(c, sx, "k_trecon"));
+        TRY(launch(c, sx, "k_trecon", 0.0, [&](CwtSlot cwt) {
+            k_trecon<<<4, 256, SMEM_TRECON, sx>>>(vpk, MT, linv_out, c->wctl, step, cwt);
+        }));
         if (sx != st) CU(cudaEventRecord(c->ev_aux[3], sx));
     }
-    pre(c, st);
-    k_trimm_z<<<10, 256, SMEM_TRIMM, st>>>(Rr, R2, Z23, c->wctl, step, c->cwt_cur);
-    TRY(post(c, st, "k_trimm_z"));
+    TRY(launch(c, st, "k_trimm_z", 0.0, [&](CwtSlot cwt) { k_trimm_z<<<10, 256, SMEM_TRIMM, st>>>(Rr, R2, Z23, c->wctl, step, cwt); }));
     TRY(rmul(2, nq - 2, Z23, P, false));
     if (linv_out && sx != st) CU(cudaStreamWaitEvent(st, c->ev_aux[3], 0));   // T' is part of the panel's result
     c->wide_panels++;
@@ -793,9 +793,7 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
 static int factor_outer_panel(dhqr_context* c, cudaStream_t st, double* vpk, dhqr_context::WSet& w, const Panel& p, int64_t m,
                               int64_t col0, double* A, int64_t lda, double* alpha, int step, bool wide, double* linv_out = nullptr) {
     if (c->wctl) {   // clear the guards of the previous panel and the verdict that travels with this V buffer
-        cwt_open(c, st);
-        k_wide_begin<<<1, 32, 0, st>>>(c->wctl, vpk + KC1, c->cwt_cur);
-        TRY(post(c, st, "k_wide_begin"));
+        TRY(launch(c, st, "k_wide_begin", 0.0, [&](CwtSlot cwt) { k_wide_begin<<<1, 32, 0, st>>>(c->wctl, vpk + KC1, cwt); }));
     }
     if (wide) return factor_outer_panel_wide(c, st, vpk, w, p, m, col0, A, lda, alpha, step, linv_out);
     return factor_outer_panel_narrow(c, st, vpk, w, p, m, col0, A, lda, alpha, step);
@@ -886,8 +884,7 @@ static int qr_blocked_serial(dhqr_context* c, cudaStream_t st, int64_t m, int64_
             // C2 (S:141-143): the owner's reflectors go to every rank, once per panel instead of once per column
             NC(g_nccl.Broadcast(vpk, vpk, (size_t)(g.vrows / KC1) * VPK_CHUNK, ncclFloat64, p.owner, c->comm, st));
             NC(g_nccl.Broadcast(alpha + p.c, alpha + p.c, (size_t)p.kb, ncclFloat64, p.owner, c->comm, st));
-            k_wide_note<<<1, 32, 0, st>>>(c->wctl, vpk + KC1, k);
-            TRY(post(c, st, "k_wide_note"));
+            TRY(launch(c, st, "k_wide_note", 0.0, [&](CwtSlot) { k_wide_note<<<1, 32, 0, st>>>(c->wctl, vpk + KC1, k); }));
         }
         // trailing update of the local columns right of the panel (S:198-213 for nb columns at once)
         const int64_t t0 = std::max(p.c + p.kb, col0);
@@ -896,6 +893,95 @@ static int qr_blocked_serial(dhqr_context* c, cudaStream_t st, int64_t m, int64_
                                       haveT, nullptr, k + 1));
     }
     return 0;
+}
+
+// The events of one run of the look-ahead schedule: per unit (hp: created by the unit's publish, with several ranks only), per
+// upload chunk that joined (caught: its catch-up is done), and the fork from the caller's stream.  They are destroyed with their
+// owner: once recorded and waited on, the work they order is already enqueued.  Unless dismissed, the owner first makes the
+// caller's stream wait for every internal stream of the schedule, so that on an error return it neither runs ahead of nor
+// returns before work already queued there.
+struct LookaheadEvents {
+    dhqr_context* c;
+    cudaStream_t st;
+    std::vector<cudaEvent_t> panel, next, bulk, a2, hp, caught;
+    cudaEvent_t fork = nullptr;
+    bool join = true;
+    LookaheadEvents(dhqr_context* c_, cudaStream_t st_, int K) : c(c_), st(st_), panel(K), next(K), bulk(K), a2(K), hp(K) {}
+    void dismiss() { join = false; }
+    ~LookaheadEvents() {
+        cudaEvent_t done;
+        if (join && cudaEventCreateWithFlags(&done, cudaEventDisableTiming) == cudaSuccess) {
+            for (cudaStream_t s : {c->hp_stream, c->comm_stream, c->hp2_stream, c->cu_stream[0], c->cu_stream[1], c->cu_stream[2]}) {
+                cudaEventRecord(done, s);
+                cudaStreamWaitEvent(st, done, 0);
+            }
+            cudaEventDestroy(done);
+        }
+        for (const auto* v : {&panel, &next, &bulk, &a2, &hp, &caught})
+            for (cudaEvent_t e : *v)
+                if (e) cudaEventDestroy(e);
+        if (fork) cudaEventDestroy(fork);
+    }
+};
+
+// chain_wait_trace, before a look-ahead factorisation: forget the launches of the previous one and reset the stamps in stream
+// order, starts to ~0 (atomicMin), ends to 0 (atomicMax)
+static int cwt_reset(dhqr_context* c, cudaStream_t st) {
+    if (!c->chain_wait_trace || !c->cwt_stamps) return 0;
+    for (auto& r : c->cwt_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
+    c->cwt_recs.clear();
+    c->cwt_rows.clear();
+    c->cwt_unit = 0;
+    if (cudaMemset2DAsync(c->cwt_stamps, 16, 0xFF, 8, CWT_MAX, st) != cudaSuccess ||
+        cudaMemset2DAsync(c->cwt_stamps + 1, 16, 0, 8, CWT_MAX, st) != cudaSuccess) return set_err(1002, "chain_wait_trace reset failed");
+    return 0;
+}
+
+// chain_wait_trace, after it: one row per traced launch (unit, stream, class, event span, stamp span, wait; ms)
+static int cwt_collect(dhqr_context* c, cudaStream_t st) {
+    if (!c->chain_wait_trace || !c->cwt_stamps) return 0;
+    for (cudaStream_t s : {st, c->hp_stream, c->hp2_stream, c->aux_stream}) cudaStreamSynchronize(s);
+    std::vector<unsigned long long> t(2 * c->cwt_recs.size());
+    if (!t.empty() && cudaMemcpy(t.data(), c->cwt_stamps, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return set_err(1002, "chain_wait_trace read-back failed");
+    for (size_t i = 0; i < c->cwt_recs.size(); ++i) {
+        const auto& r = c->cwt_recs[i];
+        float span = 0.f;
+        cudaEventElapsedTime(&span, r.e0, r.e1);
+        const bool stamped = t[2 * i] != ~0ull && t[2 * i + 1] >= t[2 * i];   // kernels without a CwtScope: -1
+        const double run = stamped ? (double)(t[2 * i + 1] - t[2 * i]) * 1e-6 : -1.0;
+        const double row[6] = {(double)r.unit, (double)r.stream, (double)r.cls, (double)span, run, stamped ? span - run : -1.0};
+        c->cwt_rows.insert(c->cwt_rows.end(), row, row + 6);
+    }
+    return 0;
+}
+
+// la_trace, after a look-ahead factorisation: la_times, and under host_trace the stage timeline of the pipelined host entry on
+// stderr (ms since the first chunk was on the device).  joinedAt: the step at which each upload chunk joined.
+static void la_collect(dhqr_context* c, cudaStream_t st, const LookaheadEvents& ev, const std::vector<Panel>& panels, const Plan& pl,
+                       const std::vector<Unit>& units, const std::vector<int>& joinedAt) {
+    if (!c->la_trace) return;
+    cudaStreamSynchronize(st);
+    cudaStreamSynchronize(c->hp_stream);
+    c->la_times.assign(panels.size() * 3, 0.f);
+    for (size_t k = 0; k < units.size(); ++k)
+        for (int q = units[k].a; q < units[k].a + units[k].np; ++q) {
+            cudaEventElapsedTime(&c->la_times[3 * q + 0], ev.fork, ev.panel[k]);
+            cudaEventElapsedTime(&c->la_times[3 * q + 1], ev.fork, ev.next[k]);
+            cudaEventElapsedTime(&c->la_times[3 * q + 2], ev.fork, ev.bulk[k]);
+        }
+    if (!c->host_trace) return;
+    for (size_t j = 0; j < ev.caught.size(); ++j) {
+        float tu = -1.f, tc = -1.f;
+        cudaEventSynchronize(ev.caught[j]);
+        cudaEventElapsedTime(&tu, ev.fork, c->up_chunks[j].ev);
+        cudaEventElapsedTime(&tc, ev.fork, ev.caught[j]);
+        fprintf(stderr, "[dhqr host] chunk at column %5lld: uploaded %7.2f ms, joins at step %2d (planned %2d), caught up %7.2f ms\n",
+                (long long)c->up_chunks[j].c0, tu, joinedAt[j], c->up_chunks[j].join, tc);
+    }
+    for (int k = pl.kstart; k < (int)panels.size(); ++k)
+        fprintf(stderr, "[dhqr host] step %2d: panel %7.2f  T' %7.2f  bulk %7.2f ms\n", k, c->la_times[3 * k], c->la_times[3 * k + 1],
+                c->la_times[3 * k + 2]);
 }
 
 // look-ahead: the panel chain (latency bound) runs on a high-priority stream ahead of the bulk trailing update, which stays on
@@ -917,7 +1003,8 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     auto P = [&](int k) -> const Panel& { return panels[units[k].a]; };                              // first panel of unit k
     auto uend = [&](int k) { const Panel& q = panels[units[k].a + units[k].np - 1]; return q.c + q.kb; };
     cudaStream_t hp = c->hp_stream;
-    std::vector<cudaEvent_t> evPanel(K), evNext(K), evBulk(K), evA2(K);
+    LookaheadEvents ev(c, st, K);
+    auto& evPanel = ev.panel, &evNext = ev.next, &evBulk = ev.bulk, &evA2 = ev.a2, &evHp = ev.hp, &evCatch = ev.caught;
     std::vector<char> haveA2(K, 0);
     const unsigned evflags = c->la_trace ? cudaEventDefault : cudaEventDisableTiming;
     for (int k = K0; k < K; ++k) {
@@ -933,7 +1020,6 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     // evPanel[k].  The comm stream first waits for everything queued on hp so far: on the owner that is the factorisation of
     // panel k, on every rank the last reads of the ring slot's previous occupant V_{k-3}.
     cudaStream_t cs = c->comm_stream;
-    std::vector<cudaEvent_t> evHp(K, nullptr);
     auto publish = [&](int k) -> int {
         if (c->nranks > 1) {
             const PanelGeom g = panel_geom(P(k), m);
@@ -943,8 +1029,8 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             CU(cudaStreamWaitEvent(cs, evHp[k], 0));
             NC(g_nccl.Broadcast(v, v, (size_t)(g.vrows / KC1) * VPK_CHUNK, ncclFloat64, P(k).owner, c->comm, cs));
             NC(g_nccl.Broadcast(alpha + P(k).c, alpha + P(k).c, (size_t)P(k).kb, ncclFloat64, P(k).owner, c->comm, cs));
-            k_wide_note<<<1, 32, 0, cs>>>(c->wctl, v + KC1, units[k].a);   // the owner's verdict on the panel arrived with the buffer
-            TRY(post(c, cs, "k_wide_note"));
+            // the owner's verdict on the panel arrived with the buffer
+            TRY(launch(c, cs, "k_wide_note", 0.0, [&](CwtSlot) { k_wide_note<<<1, 32, 0, cs>>>(c->wctl, v + KC1, units[k].a); }));
             CU(cudaEventRecord(evPanel[k], cs));
         } else {
             CU(cudaEventRecord(evPanel[k], hp));
@@ -978,210 +1064,134 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             const PanelGeom gq = panel_geom(pq, m);
             cudaStreamWaitEvent(cu, evPanel[q], 0);                   // V_q is final in A ...
             cudaStreamWaitEvent(cu, evNext[q], 0);                    // ... and T'_q sits in its slot
-            dim3 grid((unsigned)std::min<int64_t>((gq.vrows / 4 + 255) / 256, 4 * c->sms), gq.nbp <= IB ? IB : NBMAX);
-            k_pack<<<grid, 256, 0, cu>>>(A + (pq.c - col0) * lda + pq.c, lda, m - pq.c, pq.kb, 1, vpk_cu, 0, pq.c - gq.r0, gq.vrows);
-            TRY(post(c, cu, "k_pack"));
+            TRY(pack_v(c, cu, A + (pq.c - col0) * lda + pq.c, lda, m - pq.c, pq.kb, 1, vpk_cu, pq.c - gq.r0, gq.vrows,
+                       gq.nbp <= IB ? IB : NBMAX));
             TRY(apply_block_reflector(c, cu, vpk_cu, ws_cu, 0, gq.nbp, gq.rows, pq.c - gq.r0, A + (u.c0 - col0) * lda + gq.r0, lda,
                                       (int)(u.c1 - u.c0), haveTslot[q] != 0, c->tslot(units[q].a), units[q].a + 1));
         }
         cudaEventRecord(done, cu);
         return 0;
     };
-    std::vector<cudaEvent_t> evCatch;
-    std::vector<int> joinedAt;
-    int rc = 0;
-    cudaEvent_t fork = nullptr, hpdone = nullptr;
-    do {
-        if (c->chain_wait_trace && c->cwt_stamps) {   // starts to ~0 (atomicMin), ends to 0 (atomicMax), in stream order
-            for (auto& r : c->cwt_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
-            c->cwt_recs.clear();
-            c->cwt_rows.clear();
-            c->cwt_unit = 0;
-            if (cudaMemset2DAsync(c->cwt_stamps, 16, 0xFF, 8, CWT_MAX, st) != cudaSuccess ||
-                cudaMemset2DAsync(c->cwt_stamps + 1, 16, 0, 8, CWT_MAX, st) != cudaSuccess) { rc = set_err(1002, "chain_wait_trace reset failed"); break; }
-        }
-        if (cudaEventCreateWithFlags(&fork, evflags) != cudaSuccess) { rc = set_err(1001, "event create failed"); break; }
-        cudaEventRecord(fork, st);
-        cudaStreamWaitEvent(hp, fork, 0);                          // hp starts after everything already queued on st
-        std::vector<char> ownT(K, 0);       // T'_k already sits in the ring slot on this rank (wide panel factored here, k_trecon)
-        if (c->rank == P(K0).owner) {
-            bool wide = false;
-            if ((rc = factor_unit(c, hp, units[K0], c->vpk2[K0 % 3], c->vpkb[K0 % 3], c->ws[1], panels, pl, m, col0, A, lda, alpha,
-                                  c->tslot(units[K0].a), &wide))) break;
-            if (wide) { ownT[K0] = 1; cudaEventRecord(evNext[K0], hp); }
-        }
-        if ((rc = publish(K0))) break;
-        for (int k = K0; k < K && !rc; ++k) {
-            const Panel& p = P(k);
-            const PanelGeom g = panel_geom(p, m);
-            const double* vk = c->vpk2[k % 3];
-            c->cwt_unit = k + 1;   // chain launches of this step end with unit k + 1 factored (unit 0: before the loop)
-            const int pk = units[k].a;                                                   // first panel of the unit
-            const int64_t t0 = uend(k);                                                  // first trailing column
-            const int64_t t1 = k + 1 < K ? uend(k + 1) : t0;                             // end of unit k+1
-            const int64_t t2 = k + 2 < K ? uend(k + 2) : t1;                             // end of unit k+2
-            // V_k (one panel, or both panels of a pair: K = 256, T' and G from their slots) -> local columns [lo, hi) on stream s
-            auto apply_k = [&](cudaStream_t s, dhqr_context::WSet& w, int64_t lo, int64_t hi, bool haveT, double* linv_io) -> int {
-                double* C = A + (lo - col0) * lda + g.r0;
-                if (units[k].np == 2)
-                    return apply_pair(c, s, vk, c->vpkb[k % 3], w, g.rows, C, lda, (int)(hi - lo), c->tslot(pk), c->tslot(pk + 1),
-                                      c->gslot(pk), pk + 2);
-                return apply_block_reflector(c, s, vk, w, 0, g.nbp, g.rows, p.c - g.r0, C, lda, (int)(hi - lo), haveT, linv_io, pk + 1);
-            };
-            int64_t lo, hi;
-            // chunks that join the window at this step: planned, or forced because step k+1 would reach into them
-            const int64_t wold = wend;
-            const size_t up0 = upnext;
-            if (windowed) {
-                const int64_t t3 = k + 3 < K ? uend(k + 3) : lend;                         // end of unit k+3
-                while (upnext < c->up_chunks.size() && (c->up_chunks[upnext].join <= k || c->up_chunks[upnext].c0 < t3)) {
-                    const auto& u = c->up_chunks[upnext];
-                    if (u.c0 < t2 || u.c0 != wend) { rc = set_err(4005, "internal: upload chunk %d joins too late (step %d)", (int)upnext, k); break; }
-                    cudaEvent_t done;
-                    if (cudaEventCreateWithFlags(&done, evflags) != cudaSuccess) { rc = set_err(1001, "event create failed"); break; }
-                    evCatch.push_back(done);
-                    joinedAt.push_back(k);
-                    if ((rc = catch_up(u, (int)(upnext % (size_t)c->host_cu_streams), k, done))) break;
-                    wend = u.c1;
-                    ++upnext;
-                }
-                if (rc) break;
-                if (wend < t2) { rc = set_err(4005, "internal: window ends at %lld before panel %d", (long long)wend, k + 2); break; }
-            }
-            double* lk = c->tslot(pk);
-            bool haveT = ownT[k];                                        // T'_k in lk (this rank)
-            bool hp2_gate = false;                                       // evA2[k] already marks where hp2 may start on hp
-            if (k + 1 < K) {
-                // vpk[(k+1)%3] was last read by the bulk update k-2 (and, on the owner of panel k-2, by its broadcast)
-                if (k - 2 >= K0) {
-                    cudaStreamWaitEvent(hp, evBulk[k - 2], 0);
-                    if (haveA2[k - 2]) cudaStreamWaitEvent(hp, evA2[k - 2], 0);
-                    if (c->nranks > 1) cudaStreamWaitEvent(hp, evPanel[k - 2], 0);
-                }
-                if (c->rank == P(k + 1).owner) {
-                    wait_panel(hp, k);
-                    if (k - 1 >= K0 && haveA2[k - 1]) cudaStreamWaitEvent(hp, evA2[k - 1], 0);   // V_{k-1} reached these columns
-                    if (clip(t0, t1, lo, hi)) {
-                        const bool hadT = haveT;
-                        if ((rc = apply_k(hp, c->ws[1], lo, hi, haveT, lk))) break;
-                        haveT = true;
-                        if (!hadT) cudaEventRecord(evNext[k], hp);       // T'_k is in the ring: the bulk update may start
-                    }
-                    // hp2 needs nothing of the factorisation of unit k+1 below: it neither touches nor gates on its columns
-                    cudaEventRecord(evA2[k], hp);
-                    hp2_gate = true;
-                    bool widen = false;
-                    if ((rc = factor_unit(c, hp, units[k + 1], c->vpk2[(k + 1) % 3], c->vpkb[(k + 1) % 3], c->ws[1], panels, pl, m, col0, A,
-                                          lda, alpha, c->tslot(units[k + 1].a), &widen))) break;
-                    if (widen) { ownT[k + 1] = 1; cudaEventRecord(evNext[k + 1], hp); }
-                }
-                if ((rc = publish(k + 1))) break;
-            }
-            // columns of panel k+2: their V_0..V_{k-1} come from the bulk updates up to k-1.  This apply is off the chain's
-            // stream and overlaps the factorisation of panel k+1; the chain picks it up through evA2[k] before it applies
-            // V_{k+1} to the same columns.
-            if (clip(t1, t2, lo, hi)) {
-                cudaStream_t s2 = c->hp2_stream;
-                if (!hp2_gate) cudaEventRecord(evA2[k], hp);             // (used as a scratch event first: order s2 behind hp's
-                cudaStreamWaitEvent(s2, evA2[k], 0);                     //  work up to T'_k, not behind the factorisation of k+1)
-                if (k - 1 >= K0) cudaStreamWaitEvent(s2, evBulk[k - 1], 0);
-                wait_panel(s2, k);
-                const bool hadT = haveT;
-                if ((rc = apply_k(s2, c->ws[2], lo, hi, haveT, lk))) break;
-                haveT = true;
-                if (!hadT) cudaEventRecord(evNext[k], s2);               // T'_k came from this apply
-                cudaEventRecord(evA2[k], s2);
-                haveA2[k] = true;
-            }
-            if (!haveT) cudaEventRecord(evNext[k], hp);                  // keep the event defined (timeline tracing)
-            wait_panel(st, k);
-            if (clip(t2, std::min(lend, wold), lo, hi)) {
-                if (haveT) cudaStreamWaitEvent(st, evNext[k], 0);
-                if ((rc = apply_k(st, c->ws[0], lo, hi, haveT, haveT ? lk : nullptr))) break;
-            }
-            for (size_t j = up0; j < upnext && !rc; ++j) {             // the chunks that joined at this step, each behind its catch-up
-                const auto& u = c->up_chunks[j];
-                cudaStreamWaitEvent(st, evCatch[j], 0);
-                if (haveT) cudaStreamWaitEvent(st, evNext[k], 0);
-                rc = apply_k(st, c->ws[0], u.c0, u.c1, haveT, haveT ? lk : nullptr);
-            }
-            if (rc) break;
-            haveTslot[k] = haveT;
-            cudaEventRecord(evBulk[k], st);
-        }
-        if (rc) break;
-        cudaStreamWaitEvent(st, evPanel[K - 1], 0);                // join: alpha and the last panel come from hp / the comm stream
-        if (c->nranks > 1) {
-            cudaEventRecord(evHp[K - 1], hp);                      // (re-recorded: everything queued on hp)
-            cudaStreamWaitEvent(st, evHp[K - 1], 0);
-        }
-        if (c->chain_wait_trace && c->cwt_stamps) {
-            for (cudaStream_t s : {st, hp, c->hp2_stream, c->aux_stream}) cudaStreamSynchronize(s);
-            std::vector<unsigned long long> t(2 * c->cwt_recs.size());
-            if (!t.empty() && cudaMemcpy(t.data(), c->cwt_stamps, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) {
-                rc = set_err(1002, "chain_wait_trace read-back failed");
-                break;
-            }
-            for (size_t i = 0; i < c->cwt_recs.size(); ++i) {
-                const auto& r = c->cwt_recs[i];
-                float span = 0.f;
-                cudaEventElapsedTime(&span, r.e0, r.e1);
-                const bool stamped = t[2 * i] != ~0ull && t[2 * i + 1] >= t[2 * i];   // kernels without a CwtScope: -1
-                const double run = stamped ? (double)(t[2 * i + 1] - t[2 * i]) * 1e-6 : -1.0;
-                const double row[6] = {(double)r.unit, (double)r.stream, (double)r.cls, (double)span, run, stamped ? span - run : -1.0};
-                c->cwt_rows.insert(c->cwt_rows.end(), row, row + 6);
-            }
-        }
-        if (c->la_trace) {
-            cudaStreamSynchronize(st);
-            cudaStreamSynchronize(hp);
-            c->la_times.assign(panels.size() * 3, 0.f);
-            for (int k = K0; k < K; ++k)
-                for (int q = units[k].a; q < units[k].a + units[k].np; ++q) {
-                    cudaEventElapsedTime(&c->la_times[3 * q + 0], fork, evPanel[k]);
-                    cudaEventElapsedTime(&c->la_times[3 * q + 1], fork, evNext[k]);
-                    cudaEventElapsedTime(&c->la_times[3 * q + 2], fork, evBulk[k]);
-                }
-            if (c->host_trace) {   // stage timeline of the pipelined host entry (ms since the first chunk was on the device)
-                for (size_t j = 0; j < evCatch.size(); ++j) {
-                    float tu = -1.f, tc = -1.f;
-                    cudaEventSynchronize(evCatch[j]);
-                    cudaEventElapsedTime(&tu, fork, c->up_chunks[j].ev);
-                    cudaEventElapsedTime(&tc, fork, evCatch[j]);
-                    fprintf(stderr, "[dhqr host] chunk at column %5lld: uploaded %7.2f ms, joins at step %2d (planned %2d), caught up %7.2f ms\n",
-                            (long long)c->up_chunks[j].c0, tu, joinedAt[j], c->up_chunks[j].join, tc);
-                }
-                for (int k = pl.kstart; k < (int)panels.size(); ++k)
-                    fprintf(stderr, "[dhqr host] step %2d: panel %7.2f  T' %7.2f  bulk %7.2f ms\n", k, c->la_times[3 * k], c->la_times[3 * k + 1],
-                            c->la_times[3 * k + 2]);
-            }
-        }
-    } while (0);
-    // error path: the caller's stream must not run ahead of (or return before) work already queued on the internal stream
-    if (rc && cudaEventCreateWithFlags(&hpdone, cudaEventDisableTiming) == cudaSuccess) {
-        cudaEventRecord(hpdone, hp);
-        cudaStreamWaitEvent(st, hpdone, 0);
-        cudaEventRecord(hpdone, cs);
-        cudaStreamWaitEvent(st, hpdone, 0);
-        cudaEventRecord(hpdone, c->hp2_stream);
-        cudaStreamWaitEvent(st, hpdone, 0);
-        for (int i = 0; i < 3; ++i) {
-            cudaEventRecord(hpdone, c->cu_stream[i]);
-            cudaStreamWaitEvent(st, hpdone, 0);
-        }
-        cudaEventDestroy(hpdone);
+    std::vector<int> joinedAt;                                    // step at which each upload chunk joined (host_trace)
+    TRY(cwt_reset(c, st));
+    if (cudaEventCreateWithFlags(&ev.fork, evflags) != cudaSuccess) return set_err(1001, "event create failed");
+    cudaEventRecord(ev.fork, st);
+    cudaStreamWaitEvent(hp, ev.fork, 0);                          // hp starts after everything already queued on st
+    std::vector<char> ownT(K, 0);       // T'_k already sits in the ring slot on this rank (wide panel factored here, k_trecon)
+    if (c->rank == P(K0).owner) {
+        bool wide = false;
+        TRY(factor_unit(c, hp, units[K0], c->vpk2[K0 % 3], c->vpkb[K0 % 3], c->ws[1], panels, pl, m, col0, A, lda, alpha,
+                        c->tslot(units[K0].a), &wide));
+        if (wide) { ownT[K0] = 1; cudaEventRecord(evNext[K0], hp); }
     }
-    for (cudaEvent_t e : evHp)
-        if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : evCatch) cudaEventDestroy(e);
-    // events may be destroyed once recorded/waited on: the work they order is already enqueued
-    if (fork) cudaEventDestroy(fork);
-    for (int k = K0; k < K; ++k) { cudaEventDestroy(evPanel[k]); cudaEventDestroy(evNext[k]); cudaEventDestroy(evBulk[k]); cudaEventDestroy(evA2[k]); }
-    if (!rc) {
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) rc = set_err(1000 + (int)e, "look-ahead enqueue failed: %s", cudaGetErrorString(e));
+    TRY(publish(K0));
+    for (int k = K0; k < K; ++k) {
+        const Panel& p = P(k);
+        const PanelGeom g = panel_geom(p, m);
+        const double* vk = c->vpk2[k % 3];
+        c->cwt_unit = k + 1;   // chain launches of this step end with unit k + 1 factored (unit 0: before the loop)
+        const int pk = units[k].a;                                                   // first panel of the unit
+        const int64_t t0 = uend(k);                                                  // first trailing column
+        const int64_t t1 = k + 1 < K ? uend(k + 1) : t0;                             // end of unit k+1
+        const int64_t t2 = k + 2 < K ? uend(k + 2) : t1;                             // end of unit k+2
+        // V_k (one panel, or both panels of a pair: K = 256, T' and G from their slots) -> local columns [lo, hi) on stream s
+        auto apply_k = [&](cudaStream_t s, dhqr_context::WSet& w, int64_t lo, int64_t hi, bool haveT, double* linv_io) -> int {
+            double* C = A + (lo - col0) * lda + g.r0;
+            if (units[k].np == 2)
+                return apply_pair(c, s, vk, c->vpkb[k % 3], w, g.rows, C, lda, (int)(hi - lo), c->tslot(pk), c->tslot(pk + 1),
+                                  c->gslot(pk), pk + 2);
+            return apply_block_reflector(c, s, vk, w, 0, g.nbp, g.rows, p.c - g.r0, C, lda, (int)(hi - lo), haveT, linv_io, pk + 1);
+        };
+        int64_t lo, hi;
+        // chunks that join the window at this step: planned, or forced because step k+1 would reach into them
+        const int64_t wold = wend;
+        const size_t up0 = upnext;
+        if (windowed) {
+            const int64_t t3 = k + 3 < K ? uend(k + 3) : lend;                         // end of unit k+3
+            while (upnext < c->up_chunks.size() && (c->up_chunks[upnext].join <= k || c->up_chunks[upnext].c0 < t3)) {
+                const auto& u = c->up_chunks[upnext];
+                if (u.c0 < t2 || u.c0 != wend) return set_err(4005, "internal: upload chunk %d joins too late (step %d)", (int)upnext, k);
+                cudaEvent_t done;
+                if (cudaEventCreateWithFlags(&done, evflags) != cudaSuccess) return set_err(1001, "event create failed");
+                evCatch.push_back(done);
+                joinedAt.push_back(k);
+                TRY(catch_up(u, (int)(upnext % (size_t)c->host_cu_streams), k, done));
+                wend = u.c1;
+                ++upnext;
+            }
+            if (wend < t2) return set_err(4005, "internal: window ends at %lld before panel %d", (long long)wend, k + 2);
+        }
+        double* lk = c->tslot(pk);
+        bool haveT = ownT[k];                                        // T'_k in lk (this rank)
+        bool hp2_gate = false;                                       // evA2[k] already marks where hp2 may start on hp
+        if (k + 1 < K) {
+            // vpk[(k+1)%3] was last read by the bulk update k-2 (and, on the owner of panel k-2, by its broadcast)
+            if (k - 2 >= K0) {
+                cudaStreamWaitEvent(hp, evBulk[k - 2], 0);
+                if (haveA2[k - 2]) cudaStreamWaitEvent(hp, evA2[k - 2], 0);
+                if (c->nranks > 1) cudaStreamWaitEvent(hp, evPanel[k - 2], 0);
+            }
+            if (c->rank == P(k + 1).owner) {
+                wait_panel(hp, k);
+                if (k - 1 >= K0 && haveA2[k - 1]) cudaStreamWaitEvent(hp, evA2[k - 1], 0);   // V_{k-1} reached these columns
+                if (clip(t0, t1, lo, hi)) {
+                    const bool hadT = haveT;
+                    TRY(apply_k(hp, c->ws[1], lo, hi, haveT, lk));
+                    haveT = true;
+                    if (!hadT) cudaEventRecord(evNext[k], hp);       // T'_k is in the ring: the bulk update may start
+                }
+                // hp2 needs nothing of the factorisation of unit k+1 below: it neither touches nor gates on its columns
+                cudaEventRecord(evA2[k], hp);
+                hp2_gate = true;
+                bool widen = false;
+                TRY(factor_unit(c, hp, units[k + 1], c->vpk2[(k + 1) % 3], c->vpkb[(k + 1) % 3], c->ws[1], panels, pl, m, col0, A, lda,
+                                alpha, c->tslot(units[k + 1].a), &widen));
+                if (widen) { ownT[k + 1] = 1; cudaEventRecord(evNext[k + 1], hp); }
+            }
+            TRY(publish(k + 1));
+        }
+        // columns of panel k+2: their V_0..V_{k-1} come from the bulk updates up to k-1.  This apply is off the chain's
+        // stream and overlaps the factorisation of panel k+1; the chain picks it up through evA2[k] before it applies
+        // V_{k+1} to the same columns.
+        if (clip(t1, t2, lo, hi)) {
+            cudaStream_t s2 = c->hp2_stream;
+            if (!hp2_gate) cudaEventRecord(evA2[k], hp);             // (used as a scratch event first: order s2 behind hp's
+            cudaStreamWaitEvent(s2, evA2[k], 0);                     //  work up to T'_k, not behind the factorisation of k+1)
+            if (k - 1 >= K0) cudaStreamWaitEvent(s2, evBulk[k - 1], 0);
+            wait_panel(s2, k);
+            const bool hadT = haveT;
+            TRY(apply_k(s2, c->ws[2], lo, hi, haveT, lk));
+            haveT = true;
+            if (!hadT) cudaEventRecord(evNext[k], s2);               // T'_k came from this apply
+            cudaEventRecord(evA2[k], s2);
+            haveA2[k] = true;
+        }
+        if (!haveT) cudaEventRecord(evNext[k], hp);                  // keep the event defined (timeline tracing)
+        wait_panel(st, k);
+        if (clip(t2, std::min(lend, wold), lo, hi)) {
+            if (haveT) cudaStreamWaitEvent(st, evNext[k], 0);
+            TRY(apply_k(st, c->ws[0], lo, hi, haveT, haveT ? lk : nullptr));
+        }
+        for (size_t j = up0; j < upnext; ++j) {                      // the chunks that joined at this step, each behind its catch-up
+            const auto& u = c->up_chunks[j];
+            cudaStreamWaitEvent(st, evCatch[j], 0);
+            if (haveT) cudaStreamWaitEvent(st, evNext[k], 0);
+            TRY(apply_k(st, c->ws[0], u.c0, u.c1, haveT, haveT ? lk : nullptr));
+        }
+        haveTslot[k] = haveT;
+        cudaEventRecord(evBulk[k], st);
     }
-    return rc;
+    cudaStreamWaitEvent(st, evPanel[K - 1], 0);                    // join: alpha and the last panel come from hp / the comm stream
+    if (c->nranks > 1) {
+        cudaEventRecord(evHp[K - 1], hp);                          // (re-recorded: everything queued on hp)
+        cudaStreamWaitEvent(st, evHp[K - 1], 0);
+    }
+    TRY(cwt_collect(c, st));
+    la_collect(c, st, ev, panels, pl, units, joinedAt);
+    ev.dismiss();
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_err(1000 + (int)e, "look-ahead enqueue failed: %s", cudaGetErrorString(e));
+    return 0;
 }
 
 // largest row count the resident 32-column panel kernel can take on this device (slab of rows in shared memory)
@@ -1213,8 +1223,7 @@ static int qr_blocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, in
     for (;;) {
         bool any_wide = false;
         for (int k = pl.kstart; k < (int)panels.size(); ++k) any_wide |= plan_wide(c, pl, panels, k, m);
-        k_wide_reset<<<1, 32, 0, st>>>(c->wctl);
-        TRY(post(c, st, "k_wide_reset"));
+        TRY(launch(c, st, "k_wide_reset", 0.0, [&](CwtSlot) { k_wide_reset<<<1, 32, 0, st>>>(c->wctl); }));
         const bool use_la = la && (int)panels.size() - pl.kstart > 1;
         if (!use_la && !c->up_chunks.empty()) {   // the serial schedule knows nothing about columns still in flight: wait for them
             for (const auto& u : c->up_chunks) CU(cudaStreamWaitEvent(st, u.ev, 0));
@@ -1243,9 +1252,7 @@ static int qr_blocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, in
                 const PanelGeom ga = panel_geom(pa, m);
                 const int64_t t0 = panels[fail].c + panels[fail].kb;
                 if (t0 >= col0 + nl) break;
-                dim3 grid((unsigned)std::min<int64_t>((ga.vrows / 4 + 255) / 256, 4 * c->sms), NBMAX);
-                k_pack<<<grid, 256, 0, st>>>(A + (pa.c - col0) * lda + pa.c, lda, m - pa.c, pa.kb, 1, c->vpk2[0], 0, 0, ga.vrows);
-                TRY(post(c, st, "k_pack"));
+                TRY(pack_v(c, st, A + (pa.c - col0) * lda + pa.c, lda, m - pa.c, pa.kb, 1, c->vpk2[0], 0, ga.vrows, NBMAX));
                 TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, WP, ga.rows, 0, A + (t0 - col0) * lda + ga.r0, lda,
                                           (int)(col0 + nl - t0), true, c->tslot(u.a), 0));
             }
@@ -1277,25 +1284,22 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
         int nn = (int)n;
         void* args[] = {&A, &lda, &m, &nn, &alpha, &c->uw_flags, (void*)&tag};
         const int G = (int)std::min<int64_t>(c->sms, n);
-        pre(c, st);
-        cudaError_t e = cudaLaunchCooperativeKernel((void*)k_unblocked_wave, dim3(G), dim3(UW_THREADS), args, 0, st);
-        if (e != cudaSuccess) return set_err(1000 + (int)e, "cooperative launch of k_unblocked_wave failed: %s", cudaGetErrorString(e));
-        return post(c, st, "k_unblocked_wave", 16.0 * (double)m * n * n / 2);
+        return launch(c, st, "k_unblocked_wave", 16.0 * (double)m * n * n / 2, [&](CwtSlot) {
+            return cudaLaunchCooperativeKernel((void*)k_unblocked_wave, dim3(G), dim3(UW_THREADS), args, 0, st);
+        });
     }
     if (c->nranks == 1 && n > 0 && (size_t)((m + 2) & ~(int64_t)1) * 8 * (A1_CW + 1) <= 200 * 1024 && c->fuse_house) {
         // single GPU, the column tile fits in shared memory: one launch per column step (the next reflector is formed by the
         // CTA that has just updated its column, k_apply1_tma), two v buffers alternating between steps
         const int64_t voff = rup(m + 4, 2);
-        k_house1<<<1, 1024, 0, st>>>(A, m, alpha, c->v1);
-        TRY(post(c, st, "k_house1"));
+        TRY(launch(c, st, "k_house1", 0.0, [&](CwtSlot) { k_house1<<<1, 1024, 0, st>>>(A, m, alpha, c->v1); }));
         for (int64_t j = 0; j + 1 < n; ++j) {
             const int lead = (int)(j & 1);
             const int64_t lenw = m - j + lead, lenp = (lenw + 1) & ~(int64_t)1;
             const int nc = (int)(n - j - 1);
             double* C = A + (j + 1) * lda + (j - lead);
-            const int aligned = (((uintptr_t)C & 15) == 0 && (lda & 1) == 0) ? 1 : 0;
+            const int aligned = bulk_ok(C, lda);
             double* vcur = c->v1 + (j & 1) * voff, *vnext = c->v1 + ((j + 1) & 1) * voff;
-            pre(c, st);
             cudaLaunchConfig_t cfg = {};
             cfg.gridDim = dim3((nc + A1_CW - 1) / A1_CW);
             cfg.blockDim = dim3(A1_THREADS);
@@ -1308,8 +1312,9 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
             cfg.numAttrs = 1;
             const double* vc = vcur;
             const int64_t ldc = lda;
-            CU(cudaLaunchKernelEx(&cfg, k_apply1_tma, vc, lenw, C, ldc, nc, aligned, vnext, alpha + j + 1, lead));
-            TRY(post(c, st, "k_apply1_tma", 16.0 * (double)(m - j) * nc));
+            TRY(launch(c, st, "k_apply1_tma", 16.0 * (double)(m - j) * nc, [&](CwtSlot) {
+                return cudaLaunchKernelEx(&cfg, k_apply1_tma, vc, lenw, C, ldc, nc, aligned, vnext, alpha + j + 1, lead);
+            }));
         }
         return 0;
     }
@@ -1319,8 +1324,9 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
             const int64_t len = m - j;
             if (c->rank == owner) {
                 if (lead) CU(cudaMemsetAsync(c->v1, 0, sizeof(double), st));
-                k_house1<<<1, 1024, 0, st>>>(A + (j - col0) * lda + j, len, alpha + j, c->v1 + lead);
-                TRY(post(c, st, "k_house1"));
+                TRY(launch(c, st, "k_house1", 0.0, [&](CwtSlot) {
+                    k_house1<<<1, 1024, 0, st>>>(A + (j - col0) * lda + j, len, alpha + j, c->v1 + lead);
+                }));
             }
             if (c->nranks > 1) {
                 NC(g_nccl.Broadcast(c->v1, c->v1, (size_t)(len + lead + 1), ncclFloat64, owner, c->comm, st));
@@ -1334,12 +1340,14 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
             const int64_t lenp = (lenw + 1) & ~(int64_t)1;
             const size_t smem = (size_t)lenp * 8 * (A1_CW + 1);
             if (smem <= 200 * 1024) {
-                const int aligned = (((uintptr_t)C & 15) == 0 && (lda & 1) == 0) ? 1 : 0;
-                k_apply1_tma<<<(nc + A1_CW - 1) / A1_CW, A1_THREADS, smem, st>>>(c->v1, lenw, C, lda, nc, aligned, nullptr, nullptr, lead);
-                TRY(post(c, st, "k_apply1_tma"));
+                const int aligned = bulk_ok(C, lda);
+                TRY(launch(c, st, "k_apply1_tma", 0.0, [&](CwtSlot) {
+                    k_apply1_tma<<<(nc + A1_CW - 1) / A1_CW, A1_THREADS, smem, st>>>(c->v1, lenw, C, lda, nc, aligned, nullptr, nullptr, lead);
+                }));
             } else {
-                k_apply1_direct<<<std::min(nc, 8 * c->sms), A1_THREADS, 0, st>>>(c->v1, lenw, C, lda, nc);
-                TRY(post(c, st, "k_apply1_direct"));
+                TRY(launch(c, st, "k_apply1_direct", 0.0, [&](CwtSlot) {
+                    k_apply1_direct<<<std::min(nc, 8 * c->sms), A1_THREADS, 0, st>>>(c->v1, lenw, C, lda, nc);
+                }));
             }
         }
     }
@@ -1362,9 +1370,7 @@ static int apply_qt_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t c
         const int64_t r0 = cs & ~(int64_t)31;
         const int64_t rows = m - r0, vrows = rup(rows, 128);
         const int nbp = kb <= IB ? IB : NBMAX;
-        dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), nbp);
-        k_pack<<<grid, 256, 0, st>>>(A + o * lda + cs, lda, m - cs, kb, 1, c->vpk2[0], 0, cs - r0, vrows);
-        TRY(post(c, st, "k_pack"));
+        TRY(pack_v(c, st, A + o * lda + cs, lda, m - cs, kb, 1, c->vpk2[0], cs - r0, vrows, nbp));
         TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, nbp, rows, cs - r0, b + r0, ldb, nrhs, false, nullptr, 0, notrans));
     }
     return 0;
@@ -1388,21 +1394,17 @@ static int qt_prepare(dhqr_context* c, cudaStream_t st, int64_t m, int64_t col0,
         const int64_t o = (int64_t)p * NBMAX, cs = col0 + o, r0 = cs & ~(int64_t)31;
         const int kb = (int)std::min<int64_t>(NBMAX, nl - o);
         const int64_t rows = m - r0, vrows = rup(rows, 128);
-        dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), NBMAX);
-        pre(c, st);
-        k_pack<<<grid, 256, 0, st>>>(A + o * lda + cs, lda, m - cs, kb, 1, c->vpk2[0], 0, cs - r0, vrows);
-        TRY(post(c, st, "k_pack"));
+        TRY(pack_v(c, st, A + o * lda + cs, lda, m - cs, kb, 1, c->vpk2[0], cs - r0, vrows, NBMAX));
         int nsplit = 0;
         int64_t pstride = 0;
         TRY(launch_panel_gram(c, st, c->vpk2[0], w, rows, &nsplit, &pstride));
-        pre(c, st);
-        k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum + (size_t)p * WP * WP);
-        TRY(post(c, st, "k_wreduce4"));
+        TRY(launch(c, st, "k_wreduce4", 0.0, [&](CwtSlot) {
+            k_wreduce4<<<(WP * WP * 4) / 256, 256, 0, st>>>(w.wpart, pstride, nsplit, (int64_t)WP * WP, w.wsum + (size_t)p * WP * WP);
+        }));
     }
-    pre(c, st);
-    k_tinv<128><<<npl, 512, smem_tinv(128), st>>>(w.wsum, c->qt_T, (int64_t)WP * WP);
-    TRY(post(c, st, "k_tinv128"));
-    return 0;
+    return launch(c, st, "k_tinv128", 0.0, [&](CwtSlot) {
+        k_tinv<128><<<npl, 512, smem_tinv(128), st>>>(w.wsum, c->qt_T, (int64_t)WP * WP);
+    });
 }
 
 static int apply_qt_local_vec(dhqr_context* c, cudaStream_t st, int64_t m, int64_t col0, int64_t nl, const double* A, int64_t lda,
@@ -1420,12 +1422,10 @@ static int apply_qt_local_vec(dhqr_context* c, cudaStream_t st, int64_t m, int64
         const int64_t G = (a.mp + rpc - 1) / rpc;
         if (G > QT_MAXG) return set_err(4007, "internal: too many k_qt_dot CTAs");                  // callers check m first
         a.rows_per_cta = (int)rpc;
-        pre(c, st);
-        k_qt_dot<<<(unsigned)G, QT_THREADS, 0, st>>>(a);
-        TRY(post(c, st, "k_qt_dot", 8.0 * (double)a.mp * a.kb));
-        pre(c, st);
-        k_qt_axpy<<<(unsigned)((a.mp + QT_AROWS - 1) / QT_AROWS), QT_ATHREADS, 0, st>>>(a);
-        TRY(post(c, st, "k_qt_axpy", 8.0 * (double)a.mp * a.kb));
+        TRY(launch(c, st, "k_qt_dot", 8.0 * (double)a.mp * a.kb, [&](CwtSlot) { k_qt_dot<<<(unsigned)G, QT_THREADS, 0, st>>>(a); }));
+        TRY(launch(c, st, "k_qt_axpy", 8.0 * (double)a.mp * a.kb, [&](CwtSlot) {
+            k_qt_axpy<<<(unsigned)((a.mp + QT_AROWS - 1) / QT_AROWS), QT_ATHREADS, 0, st>>>(a);
+        }));
     }
     return 0;
 }
@@ -1471,9 +1471,10 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
         for (int rhs = 0; rhs < nrhs; ++rhs) {
             uint32_t tag;
             TRY(wave_tag(c, st, &tag));
-            k_backsolve_wave<<<(unsigned)(nbk + nlow), BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx, col0, nl,
-                                                                          (int)nlow, c->bs_cells, tag);
-            TRY(post(c, st, "k_backsolve_wave"));
+            TRY(launch(c, st, "k_backsolve_wave", 0.0, [&](CwtSlot) {
+                k_backsolve_wave<<<(unsigned)(nbk + nlow), BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx,
+                                                                              col0, nl, (int)nlow, c->bs_cells, tag);
+            }));
         }
         return 0;
     }
@@ -1482,8 +1483,9 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
         const int bs = (int)std::min<int64_t>(BS_BLK, nl - o);
         const int64_t c0 = col0 + o;
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((c0 + 255) / 256, 2 * c->sms));
-        k_backsolve_step<<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs);
-        TRY(post(c, st, "k_backsolve_step"));
+        TRY(launch(c, st, "k_backsolve_step", 0.0, [&](CwtSlot) {
+            k_backsolve_step<<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs);
+        }));
     }
     return 0;
 }
@@ -1502,18 +1504,18 @@ static int forwardsolve_local(dhqr_context* c, cudaStream_t st, int64_t n, const
         for (int rhs = 0; rhs < nrhs; ++rhs) {
             uint32_t tag;
             TRY(wave_tag(c, st, &tag));
-            pre(c, st);
-            k_forwardsolve_wave<<<(unsigned)nbk, BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx, n,
-                                                                     c->bs_cells, tag);
-            TRY(post(c, st, "k_forwardsolve_wave"));
+            TRY(launch(c, st, "k_forwardsolve_wave", 0.0, [&](CwtSlot) {
+                k_forwardsolve_wave<<<(unsigned)nbk, BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx, n,
+                                                                         c->bs_cells, tag);
+            }));
         }
     } else {
         for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
             const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
             const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
-            pre(c, st);
-            k_forwardsolve_step<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs, n);
-            TRY(post(c, st, "k_forwardsolve_step"));
+            TRY(launch(c, st, "k_forwardsolve_step", 0.0, [&](CwtSlot) {
+                k_forwardsolve_step<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs, n);
+            }));
         }
     }
     CU(cudaMemcpy2DAsync(y, (size_t)ldy * 8, x, (size_t)ldx * 8, (size_t)n * 8, nrhs, cudaMemcpyDeviceToDevice, st));
@@ -1945,8 +1947,7 @@ static int check_c64_args(dhqr_context* c, int64_t m, int64_t n_global, int64_t 
 
 static int pack_complex_panel(dhqr_context* c, cudaStream_t st, const double2* P, int64_t lda, int64_t mpc, int kb, int64_t vrows) {
     dim3 grid((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), NBMAX);
-    k_pack_c<<<grid, 256, 0, st>>>(P, lda, mpc, kb, c->vpk2[0], 0, vrows);
-    return post(c, st, "k_pack_c");
+    return launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) { k_pack_c<<<grid, 256, 0, st>>>(P, lda, mpc, kb, c->vpk2[0], 0, vrows); });
 }
 
 int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, void* dA, int64_t lda, void* d_alpha,
@@ -1968,11 +1969,11 @@ int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
         const int64_t mpc = m - c0;
         for (int j = 0; j < kb; ++j) {                       // S:127-144 restricted to the panel
             double2* col = P + (int64_t)j * lda + j;
-            k_house1_c<<<1, 1024, 0, st>>>(col, mpc - j, alpha + c0 + j);
-            TRY(post(c, st, "k_house1_c"));
+            TRY(launch(c, st, "k_house1_c", 0.0, [&](CwtSlot) { k_house1_c<<<1, 1024, 0, st>>>(col, mpc - j, alpha + c0 + j); }));
             if (j + 1 < kb) {
-                k_apply1_c<<<kb - j - 1, 256, 0, st>>>(col, mpc - j, col + lda, lda, kb - j - 1);
-                TRY(post(c, st, "k_apply1_c"));
+                TRY(launch(c, st, "k_apply1_c", 0.0, [&](CwtSlot) {
+                    k_apply1_c<<<kb - j - 1, 256, 0, st>>>(col, mpc - j, col + lda, lda, kb - j - 1);
+                }));
             }
         }
         const int64_t t0 = c0 + kb;
@@ -2021,8 +2022,9 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     for (int64_t o = ((n - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {     // S:260: i = n:-1:1, by blocks
         const int bs = (int)std::min<int64_t>(BS_BLK, n - o);
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((o + 255) / 256, 2 * c->sms));
-        k_backsolve_step_c<<<grid, 256, 0, st>>>(A + o * lda, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs, x, n, o, bs);
-        TRY(post(c, st, "k_backsolve_step_c"));
+        TRY(launch(c, st, "k_backsolve_step_c", 0.0, [&](CwtSlot) {
+            k_backsolve_step_c<<<grid, 256, 0, st>>>(A + o * lda, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs, x, n, o, bs);
+        }));
     }
     CU(cudaMemcpy2DAsync(d_b, (size_t)ldb * 16, x, (size_t)n * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -2047,8 +2049,9 @@ int dhqr_partialdot_c64(dhqr_handle c, const void* d_a, const void* d_b, int64_t
     TRY(check_c64_ptr(d_out, -6, "out"));
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    k_partialdot_c<<<1, 1024, 0, st>>>((const double2*)d_a, (const double2*)d_b, i0, i1, (double2*)d_out);
-    return post(c, st, "k_partialdot_c");
+    return launch(c, st, "k_partialdot_c", 0.0, [&](CwtSlot) {
+        k_partialdot_c<<<1, 1024, 0, st>>>((const double2*)d_a, (const double2*)d_b, i0, i1, (double2*)d_out);
+    });
 }
 
 // ---- explicit thin Q (LAPACK orgqr / ungqr) ---------------------------------------------------------------------------------
@@ -2077,10 +2080,10 @@ static int check_form_q(dhqr_context* c, int64_t m, int64_t n, const void* A, in
 
 static int eye_cols(dhqr_context* c, cudaStream_t st, void* Q, bool cplx, int64_t ldq, int64_t m, int64_t c0, int kb) {
     const dim3 grid((unsigned)std::min<int64_t>((m + 255) / 256, 64), kb);
-    pre(c, st);
-    if (cplx) k_eye_cols<double2><<<grid, 256, 0, st>>>((double2*)Q, ldq, m, c0);
-    else k_eye_cols<double><<<grid, 256, 0, st>>>((double*)Q, ldq, m, c0);
-    return post(c, st, cplx ? "k_eye_cols_c" : "k_eye_cols");
+    return launch(c, st, cplx ? "k_eye_cols_c" : "k_eye_cols", 0.0, [&](CwtSlot) {
+        if (cplx) k_eye_cols<double2><<<grid, 256, 0, st>>>((double2*)Q, ldq, m, c0);
+        else k_eye_cols<double><<<grid, 256, 0, st>>>((double*)Q, ldq, m, c0);
+    });
 }
 
 int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, double* dQ, int64_t ldq, void* stream) {
@@ -2093,10 +2096,7 @@ int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64
     for (int64_t p = (n - 1) / NBMAX; p >= 0; --p) {
         const int64_t cs = p * NBMAX, rows = m - cs, vrows = rup(rows, 128);   // cs is 128-aligned: the window starts at row cs
         const int kb = (int)std::min<int64_t>(NBMAX, n - cs);
-        dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), NBMAX);
-        pre(c, st);
-        k_pack<<<grid, 256, 0, st>>>(dA + cs * lda + cs, lda, rows, kb, 1, c->vpk2[0], 0, 0, vrows);
-        TRY(post(c, st, "k_pack"));
+        TRY(pack_v(c, st, dA + cs * lda + cs, lda, rows, kb, 1, c->vpk2[0], 0, vrows, NBMAX));
         TRY(eye_cols(c, st, dQ, false, ldq, m, cs, kb));
         TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, dQ + cs * ldq + cs, ldq, (int)(n - cs), true,
                                   c->qt_T + (size_t)p * NBMAX * NBMAX, 0, 1));
@@ -2156,9 +2156,9 @@ static int forwardsolve_c64_local(dhqr_context* c, cudaStream_t st, int64_t n, c
     for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
         const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
-        pre(c, st);
-        k_forwardsolve_step_c<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, n, c0, bs, n);
-        TRY(post(c, st, "k_forwardsolve_step_c"));
+        TRY(launch(c, st, "k_forwardsolve_step_c", 0.0, [&](CwtSlot) {
+            k_forwardsolve_step_c<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, n, c0, bs, n);
+        }));
     }
     CU(cudaMemcpy2DAsync(y, (size_t)ldy * 16, x, (size_t)n * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -2251,47 +2251,44 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, do
     a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
     a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = a.vn2 + n; a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
     a.part1 = a.x + m; a.part2 = a.part1 + p1; a.ldp = n;
-    pre(c, st);
-    k_qrcp_init<<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
-    TRY(post(c, st, "k_qrcp_init", 8.0 * (double)m * n));
+    TRY(launch(c, st, "k_qrcp_init", 8.0 * (double)m * n, [&](CwtSlot) {
+        k_qrcp_init<<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
+    }));
     for (int64_t k0 = 0; k0 < n; k0 += QP_NB) {
         const int kb = (int)std::min<int64_t>(QP_NB, n - k0);
         const int tiles = (int)((n - k0 + QP_GCOLS - 1) / QP_GCOLS);
         for (int jj = 0; jj < kb; ++jj) {
             const int64_t j = k0 + jj, rows = m - j;
             a.j = j; a.k0 = k0; a.jj = jj;
-            pre(c, st);
-            k_qrcp_pivot<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
-            TRY(post(c, st, "k_qrcp_pivot", 8.0 * ((double)m * 4 + (double)rows * (jj + 1) + (double)(n - j))));
+            TRY(launch(c, st, "k_qrcp_pivot", 8.0 * ((double)m * 4 + (double)rows * (jj + 1) + (double)(n - j)), [&](CwtSlot) {
+                k_qrcp_pivot<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
+            }));
             // row splits: about eight CTAs per SM in all, at least QP_THREADS rows each
             const int64_t s = std::max<int64_t>(1, std::min<int64_t>((rows + QP_THREADS - 1) / QP_THREADS,
                                                                      (8 * (int64_t)c->sms + tiles - 1) / tiles));
             a.split_rows = rup((rows + s - 1) / s, QP_THREADS);
             a.nsplit = (int)((rows + a.split_rows - 1) / a.split_rows);
-            pre(c, st);
-            k_qrcp_gemv<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
-            TRY(post(c, st, "k_qrcp_gemv", 8.0 * (double)rows * (double)(n - k0)));
+            TRY(launch(c, st, "k_qrcp_gemv", 8.0 * (double)rows * (double)(n - k0), [&](CwtSlot) {
+                k_qrcp_gemv<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
+            }));
             if (j + 1 >= n) continue;
-            pre(c, st);
-            k_qrcp_finish<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
-            TRY(post(c, st, "k_qrcp_finish"));
-            pre(c, st);
-            k_qrcp_renorm<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
-            TRY(post(c, st, "k_qrcp_renorm"));
+            TRY(launch(c, st, "k_qrcp_finish", 0.0, [&](CwtSlot) {
+                k_qrcp_finish<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
+            }));
+            TRY(launch(c, st, "k_qrcp_renorm", 0.0, [&](CwtSlot) {
+                k_qrcp_renorm<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
+            }));
         }
         const int64_t c1 = k0 + kb;
         if (c1 >= n) break;
         // A[c1:, c1:] -= V F'  on the window starting at row k0 (a multiple of 32), rows >= c1 only
         const int64_t wrows = m - k0, vrows = rup(wrows, 128);
         const int ncols = (int)(n - c1);
-        pre(c, st);
-        dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), QP_NB);
-        k_pack<<<grid, 256, 0, st>>>(A + k0 * lda + k0, lda, wrows, kb, 1, c->vpk2[0], 0, 0, vrows);
-        TRY(post(c, st, "k_pack"));
+        TRY(pack_v(c, st, A + k0 * lda + k0, lda, wrows, kb, 1, c->vpk2[0], 0, vrows, QP_NB));
         const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * YT * LDK;
-        pre(c, st);
-        k_qrcp_ypack<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(a.F, a.ldf, c1, ncols, kb, c->ws[0].ypk);
-        TRY(post(c, st, "k_qrcp_ypack"));
+        TRY(launch(c, st, "k_qrcp_ypack", 0.0, [&](CwtSlot) {
+            k_qrcp_ypack<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(a.F, a.ldf, c1, ncols, kb, c->ws[0].ypk);
+        }));
         TRY(launch_cvy(c, st, c->vpk2[0], 0, QP_NB, c->ws[0].ypk, wrows, kb, A + c1 * lda + k0, lda, ncols, 0));
     }
     return 0;
@@ -2350,10 +2347,10 @@ int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const
     }
     for (int r0 = 0; r0 < nrhs; r0 += 65535) {
         const int nr = std::min(nrhs - r0, 65535);
-        pre(c, st);
-        k_qrcp_scatter<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(c->xbuf + (size_t)r0 * rank, rank, d_jpvt, n, rank,
-                                                                                     d_b + (size_t)r0 * ldb, ldb);
-        TRY(post(c, st, "k_qrcp_scatter"));
+        TRY(launch(c, st, "k_qrcp_scatter", 0.0, [&](CwtSlot) {
+            k_qrcp_scatter<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(c->xbuf + (size_t)r0 * rank, rank, d_jpvt, n,
+                                                                                         rank, d_b + (size_t)r0 * ldb, ldb);
+        }));
     }
     return 0;
 }
@@ -2543,8 +2540,7 @@ int dhqr_partialdot_f64(dhqr_handle c, const double* d_a, const double* d_b, int
     if (!d_out) return set_err(-6, "null out");
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    k_partialdot<<<1, 1024, 0, st>>>(d_a, d_b, i0, i1, d_out);
-    return post(c, st, "k_partialdot");
+    return launch(c, st, "k_partialdot", 0.0, [&](CwtSlot) { k_partialdot<<<1, 1024, 0, st>>>(d_a, d_b, i0, i1, d_out); });
 }
 
 int dhqr_fill_uniform_f64(dhqr_handle c, uint64_t seed, int64_t i0, int64_t j0, int64_t m, int64_t n, double* dA,
@@ -2558,8 +2554,7 @@ int dhqr_fill_uniform_f64(dhqr_handle c, uint64_t seed, int64_t i0, int64_t j0, 
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid((unsigned)std::min<int64_t>((m + 255) / 256, 1024), (unsigned)std::min<int64_t>(n, 4096));
-    k_fill_uniform<<<grid, 256, 0, st>>>(seed, i0, j0, m, n, dA, lda);
-    return post(c, st, "k_fill_uniform");
+    return launch(c, st, "k_fill_uniform", 0.0, [&](CwtSlot) { k_fill_uniform<<<grid, 256, 0, st>>>(seed, i0, j0, m, n, dA, lda); });
 }
 
 // ---- kernel-level hooks ---------------------------------------------------------------------------
@@ -2576,9 +2571,7 @@ int dhqr_k_block_reflector_f64(dhqr_handle c, int64_t rows, int nbp, const doubl
     TRY(ensure_workspace(c, st, rows, ncols));
     const int nbk = nbp <= IB ? IB : NBMAX;
     const int64_t vrows = rup(rows, 128);
-    dim3 grid((unsigned)std::min<int64_t>((vrows / 4 + 255) / 256, 4 * c->sms), nbk);
-    k_pack<<<grid, 256, 0, st>>>(dV, ldv, rows, nbp, 0, c->vpk2[0], 0, 0, vrows);
-    TRY(post(c, st, "k_pack"));
+    TRY(pack_v(c, st, dV, ldv, rows, nbp, 0, c->vpk2[0], 0, vrows, nbk));
     TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, nbk, rows, row_lo, dC, ldc, ncols));
     if (d_linv_out) CU(cudaMemcpyAsync(d_linv_out, c->ws[0].linv, sizeof(double) * (size_t)nbk * nbk, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -2640,8 +2633,7 @@ int dhqr_k_wide_panel_f64(dhqr_handle c, int64_t rows, double* dP, int64_t ldp, 
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     TRY(ensure_workspace(c, st, rows, WP));
-    k_wide_reset<<<1, 32, 0, st>>>(c->wctl);
-    TRY(post(c, st, "k_wide_reset"));
+    TRY(launch(c, st, "k_wide_reset", 0.0, [&](CwtSlot) { k_wide_reset<<<1, 32, 0, st>>>(c->wctl); }));
     const Panel p = {0, 0, WP};
     TRY(factor_outer_panel(c, st, c->vpk2[0], c->ws[0], p, rows, 0, dP, ldp, d_alpha, 0, true, c->ws[0].linv));
     WideCtl host;

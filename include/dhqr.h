@@ -89,7 +89,8 @@ int dhqr_destroy(dhqr_handle h);
  *                 host link, the device and a step of the schedule on a narrow window; "host_cu_streams" (3): catch-up streams; "host_first" (0 = three panels): columns of the first, exposed upload;
  *                 "host_trace" 1: stage timeline on stderr.  A wrong assumption costs idle time, never correctness
  *   "sync"        1: cudaStreamSynchronize + error check after every kernel launch (debugging; implies serial)
- *   "profile"     1: CUDA-event bracket per launch (implies serial), read with dhqr_profile_get
+ *   "profile"     1: CUDA-event bracket around every kernel launch (implies serial), read with dhqr_profile_get: the
+ *                 classes together count every launch that dhqr_launch_count counts while it is on
  *   "bs_wave", "unblocked_wave", "fuse_house"  1 (default): back-substitution (and the Float64 forward substitution of
  *                 dhqr_forwardsolve_f64 / dhqr_solve_adj_f64) as one wavefront launch per right-hand side where all its CTAs fit
  *                 on the device, nb = 1 as one persistent launch (m <= 8192), nb = 1 with the next reflector formed inside the
