@@ -12,7 +12,9 @@
 #include <time.h>
 
 #include <algorithm>
+#include <memory>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "dhqr_kernels.cuh"
@@ -109,6 +111,64 @@ static int load_nccl() {
 // ------------------------------------------------------------------------------------------------
 static inline int64_t rup(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 
+// Owns one device allocation of n elements of T and frees it with its owner.  Converts to the raw pointer (null when empty),
+// which is what kernels and the CUDA API take.
+template <typename T>
+struct DevBuf {
+    T* p = nullptr;
+    size_t n = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(n, o.n); return *this; }
+    ~DevBuf() { release(); }
+    operator T*() const { return p; }
+    cudaError_t release() {
+        T* q = p;
+        p = nullptr;
+        n = 0;
+        return q ? cudaFree(q) : cudaSuccess;
+    }
+    // `need` elements, contents undefined
+    int alloc(size_t need) {
+        CU(release());
+        CU(cudaMalloc((void**)&p, need * sizeof(T)));
+        n = need;
+        return 0;
+    }
+    // Grows to at least `need` elements.  The zero fill goes on `st`, the stream of the call that needs the buffer: a synchronous
+    // cudaMemset would run on the legacy default stream, which a non-blocking caller stream is not ordered after.
+    int ensure(size_t need, cudaStream_t st) {
+        if (n >= need && p) return 0;
+        CU(release());
+        CU(cudaMalloc((void**)&p, need * sizeof(T)));
+        CU(cudaMemsetAsync(p, 0, need * sizeof(T), st));
+        n = need;
+        return 0;
+    }
+};
+
+// Owns one CUDA stream or event and destroys it with its owner.  Converts to the raw handle (null when empty).
+template <typename H, cudaError_t (*Destroy)(H)>
+struct Owned {
+    H h = nullptr;
+    Owned() = default;
+    Owned(Owned&& o) noexcept : h(o.h) { o.h = nullptr; }
+    Owned& operator=(Owned&& o) noexcept { std::swap(h, o.h); return *this; }
+    ~Owned() { reset(); }
+    operator H() const { return h; }
+    void reset() {
+        if (h) Destroy(h);
+        h = nullptr;
+    }
+};
+struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
+    cudaError_t create() { reset(); return cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking); }
+    cudaError_t create(int priority) { reset(); return cudaStreamCreateWithPriority(&h, cudaStreamNonBlocking, priority); }
+};
+struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
+    cudaError_t create(unsigned flags) { reset(); return cudaEventCreateWithFlags(&h, flags); }
+};
+
 struct dhqr_context {
     int device = 0, sms = 0;
     int rank = 0, nranks = 1;
@@ -118,24 +178,24 @@ struct dhqr_context {
     // workspace
     // three V buffers (panels k, k+1 and the one being broadcast live at the same time under look-ahead) and two
     // workspace sets (set 0: trailing update on the caller's stream; set 1: panel chain on the high-priority stream)
-    double* vpk2[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}; size_t vpk_elems[6] = {0, 0, 0, 0, 0, 0}; int64_t vrows_cap = 0;   // packed V [chunk][128][68]; [3..5]: catch-up of late column chunks (host entry)
+    DevBuf<double> vpk2[6];                                             // packed V [chunk][128][68]; [3..5]: catch-up of late column chunks (host entry)
     struct WSet {
-        double* wpart = nullptr; size_t wpart_elems = 0;                // gemm_vta partials
-        double* wsum = nullptr;  size_t wsum_elems = 0;                 // reduced Wext
-        double* ypk = nullptr;   size_t ypk_elems = 0;                  // packed Y = -T'W
-        double* linv = nullptr;  size_t linv_elems = 0;                 // [128*128]
+        DevBuf<double> wpart;                                           // gemm_vta partials
+        DevBuf<double> wsum;                                            // reduced Wext
+        DevBuf<double> ypk;                                             // packed Y = -T'W
+        DevBuf<double> linv;                                            // [128*128]
     } ws[6];                                                            // [2]: the chain's second apply (columns of panel k+2) on its own stream; [3..5]: catch-up (host entry)
-    double* linv_all = nullptr; size_t linv_all_elems = 0;              // T' of every outer panel of the factorisation in flight (look-ahead): slot k = panel k
-    double* tslot(int k) const { return linv_all + (size_t)k * 128 * 128; }
-    double* gram_all = nullptr; size_t gram_all_elems = 0;              // G = V_b' V_a of each panel pair (slot = first panel of the pair)
-    double* gslot(int k) const { return gram_all + (size_t)k * 128 * 128; }
-    double* vpkb[3] = {nullptr, nullptr, nullptr}; size_t vpkb_elems[3] = {0, 0, 0};   // V of the second panel of a pair, ring as vpk2[0..2]
+    DevBuf<double> linv_all;                                            // T' of every outer panel of the factorisation in flight (look-ahead): slot k = panel k
+    double* tslot(int k) const { return linv_all.p + (size_t)k * 128 * 128; }
+    DevBuf<double> gram_all;                                            // G = V_b' V_a of each panel pair (slot = first panel of the pair)
+    double* gslot(int k) const { return gram_all.p + (size_t)k * 128 * 128; }
+    DevBuf<double> vpkb[3];                                             // V of the second panel of a pair, ring as vpk2[0..2]
     int64_t pair_units = 0;                                             // statistics: panel pairs applied as one 256-wide block
-    cudaStream_t hp_stream = nullptr;                                   // stream of the panel chain (high priority)
-    cudaStream_t comm_stream = nullptr;                                 // collectives of the look-ahead schedule (high priority)
-    cudaStream_t aux_stream = nullptr;                                  // small side kernels of the wide chain (Rt = R2 R1, k_trecon), high priority
-    cudaEvent_t ev_aux[4] = {nullptr, nullptr, nullptr, nullptr};
-    cudaStream_t hp2_stream = nullptr;                                  // the chain's second apply (V_k -> columns of panel k+2), high priority
+    Stream hp_stream;                                                   // stream of the panel chain (high priority)
+    Stream comm_stream;                                                 // collectives of the look-ahead schedule (high priority)
+    Stream aux_stream;                                                  // small side kernels of the wide chain (Rt = R2 R1, k_trecon), high priority
+    Event ev_aux[4];
+    Stream hp2_stream;                                                  // the chain's second apply (V_k -> columns of panel k+2), high priority
     int host_trace = 0;                                                 // option: print a stage timeline of dhqr_qr_host_f64 to stderr
     int lookahead = 1;
     int la_trace = 0;                                                   // keep timing events of the look-ahead schedule
@@ -143,54 +203,56 @@ struct dhqr_context {
     // option chain_wait_trace (look-ahead schedule): CUDA events right before and after every launch on hp, hp2 and aux, and
     // the CwtScope stamps of the same launch, so that the time a launch was ready but had no SM can be told from its run time
     int chain_wait_trace = 0;
-    unsigned long long* cwt_stamps = nullptr;                           // [CWT_MAX][2]: first CTA start, last warp end (%globaltimer ns)
+    DevBuf<unsigned long long> cwt_stamps;                              // [CWT_MAX][2]: first CTA start, last warp end (%globaltimer ns)
     int cwt_unit = 0;                                                   // unit of the look-ahead step being enqueued
-    struct CwtRec { int unit, stream, cls; cudaEvent_t e0, e1; };
+    struct CwtRec { int unit, stream, cls; Event e0, e1; };
     std::vector<CwtRec> cwt_recs;
     std::vector<double> cwt_rows;                                       // [launch][6]: unit, stream, class, event span, stamp span, wait (ms)
-    unsigned long long* cells = nullptr;                                // panel exchange cells [IB+1][MAXG+1][IB][2]
+    DevBuf<unsigned long long> cells;                                   // panel exchange cells [IB+1][MAXG+1][IB][2]
     uint32_t ll_epoch = 0;
-    unsigned long long* cells2 = nullptr;                               // exchange cells of the panel kernel's fast path
-    int* fast_stats = nullptr;                                          // [2] fast / fallback panel counters
+    DevBuf<unsigned long long> cells2;                                  // exchange cells of the panel kernel's fast path
+    DevBuf<int> fast_stats;                                             // [2] fast / fallback panel counters
     int panel_fast = 1;
     int bs_wave = 1;                                                    // back-substitution as one wavefront launch per right-hand side
     int bs_wave_max_ctas = 0;                                           // co-residency limit of k_backsolve_wave on this device
     int fs_wave_max_ctas = 0;                                           // ... and of k_forwardsolve_wave
-    unsigned long long* bs_cells = nullptr; size_t bs_cells_blocks = 0; // x cells of the wavefronts ([block][32][2 words])
+    DevBuf<unsigned long long> bs_cells;                                // x cells of the wavefronts ([block][32][2 words])
+    size_t bs_blocks() const { return bs_cells.n / 64; }
     uint32_t bs_epoch = 0;
     int unblocked_wave = 1;                                             // nb = 1, m <= 8192: the column loop as one persistent launch
-    unsigned int* uw_flags = nullptr; size_t uw_flags_n = 0; unsigned int uw_epoch = 0;
+    DevBuf<unsigned int> uw_flags; unsigned int uw_epoch = 0;
     int fuse_house = 1;                                                 // nb = 1: next reflector formed inside the apply kernel (one launch per column)
     int cvy_persist = 4;                                                // 128-wide gemm_cvy: consecutive tiles per CTA (0: one tile per CTA); 4 is fastest on an H100 at one CTA per SM
-    long long* panel_trace = nullptr;                                   // optional k_panel clock stamps (option "panel_trace")
+    DevBuf<long long> panel_trace;                                      // optional k_panel clock stamps (option "panel_trace")
     // 128-column panel chain (dhqr_wide.cuh)
     int wide_panel = 1;                                                 // option: factor full aligned outer panels with CholeskyQR2 + reconstruction
-    WideCtl* wctl = nullptr;                                            // device control words (first refused panel, guards of the panel in flight)
-    double* wbuf = nullptr;                                             // R1, R2, X2, Rt, Y3 (plain 128x128) + XL, XL3 (rmul operand layout)
+    DevBuf<WideCtl> wctl;                                               // device control words (first refused panel, guards of the panel in flight)
+    DevBuf<double> wbuf;                                                // R1, R2, X2, Rt, Y3 (plain 128x128) + XL, XL3 (rmul operand layout)
     int64_t wide_panels = 0, wide_redone = 0;                           // statistics: panels factored by the wide chain / factorisations restarted
     double wide_kappa = 1000.0;                                         // guard on ||D R1^{-1}||_F of the first Cholesky factor (option "wide_kappa")
-    long long* wstamps = nullptr;                                       // clock64 stamps of the single-CTA kernels (option "wide_trace")
+    DevBuf<long long> wstamps;                                          // clock64 stamps of the single-CTA kernels (option "wide_trace")
     int wide_trace = 0;
     // Q'b / Qb with one right-hand side: T' of every local panel (computed before the sweep), per-CTA partials of V'b, y, ticket
-    double* qt_T = nullptr;  size_t qt_T_elems = 0;
-    double* qt_part = nullptr; unsigned int* qt_ticket = nullptr;
+    DevBuf<double> qt_T;
+    DevBuf<double> qt_part;
+    DevBuf<unsigned int> qt_ticket;
     int qt_vec = 1;                                                     // option: use it (0: the GEMM-shaped block update also for one right-hand side)
-    double* v1 = nullptr;    size_t v1_elems = 0;                       // unblocked path: v
-    double* xbuf = nullptr;  size_t xbuf_elems = 0;                     // back-substitution output
-    double* xfer = nullptr;  size_t xfer_elems = 0;                     // a right-hand-side block packed for the rank-to-rank hand-over
+    DevBuf<double> v1;                                                  // unblocked path: v
+    DevBuf<double> xbuf;                                                // back-substitution output
+    DevBuf<double> xfer;                                                // a right-hand-side block packed for the rank-to-rank hand-over
     // pivoted factorisation (dhqr_qrcp.cuh): vn1, vn2, F, the column in flight and the partials of both reductions; renorm
     // flags; scalars of the reflector in flight, the pivot ticket and the renorm counter
-    double* qp_buf = nullptr; size_t qp_buf_elems = 0;
-    int* qp_flag = nullptr;  size_t qp_flag_elems = 0;
-    QrcpCtl* qp_ctl = nullptr;
-    double* hostA = nullptr; size_t hostA_elems = 0;                    // device staging for _host_ entry points
-    double* hostB = nullptr; size_t hostB_elems = 0;
-    int64_t* d_i64 = nullptr;                                           // small int64 scratch (partition exchange)
+    DevBuf<double> qp_buf;
+    DevBuf<int> qp_flag;
+    DevBuf<QrcpCtl> qp_ctl;
+    DevBuf<double> hostA;                                               // device staging for _host_ entry points
+    DevBuf<double> hostB;
+    DevBuf<int64_t> d_i64;                                              // small int64 scratch (partition exchange)
     int64_t launches = 0;
-    cudaStream_t copy_stream = nullptr;      // compute stream of the _host_ entry points
-    cudaStream_t d2h_stream = nullptr;       // drains finished panels to the host while the factorisation continues
-    cudaStream_t h2d_stream = nullptr;       // uploads the later column chunks while the first ones are being factored
-    cudaStream_t cu_stream[3] = {nullptr, nullptr, nullptr};   // catch-up: reflectors of finished panels applied to a column chunk that arrived late (chunks alternate)
+    Stream copy_stream;                      // compute stream of the _host_ entry points
+    Stream d2h_stream;                       // drains finished panels to the host while the factorisation continues
+    Stream h2d_stream;                       // uploads the later column chunks while the first ones are being factored
+    Stream cu_stream[3];                     // catch-up: reflectors of finished panels applied to a column chunk that arrived late (chunks alternate)
     // dhqr_qr_host_f64 -> look-ahead driver: column chunks still on their way to the device.  Chunk j = global columns [c0, c1),
     // usable once `ev` has fired, joins the trailing matrix at step `join` (after a catch-up with the reflectors of panels < join)
     struct UpChunk { int64_t c0, c1; cudaEvent_t ev; int join; };
@@ -200,7 +262,7 @@ struct dhqr_context {
     int host_h2d_gbs = 50, host_tflops = 27; // option: what the join-step planner assumes about the link and the device
     int host_chain_us = 300;                 // option: ... and about the duration of a step of the schedule while the window is narrow
     int host_cu_streams = 3;                 // option: catch-up streams in use (1..3)
-    std::vector<cudaEvent_t> panel_events;
+    std::vector<Event> panel_events;
     // set by dhqr_qr_host_f64: finished columns are copied back as soon as their panel is final
     double* mirror_host = nullptr;
     int64_t mirror_lda = 0;
@@ -208,7 +270,7 @@ struct dhqr_context {
     bool attrs_set = false;
     // per-kernel-class CUDA-event profiling (option "profile")
     int profile = 0;
-    struct ProfRec { int slot; cudaEvent_t e0, e1; };
+    struct ProfRec { int slot; Event e0, e1; };
     struct ProfSlot { const char* name; double ms = 0.0; int64_t count = 0; double work = 0.0; };
     std::vector<ProfRec> prof_pending;
     std::vector<ProfSlot> prof_slots;
@@ -279,31 +341,27 @@ using CwtSlot = unsigned long long*;
 // leaves no bracket behind.
 template <typename Enqueue>
 static int launch(dhqr_context* c, cudaStream_t st, const char* what, double work, Enqueue&& enqueue) {
-    cudaEvent_t cw0 = nullptr, cw1 = nullptr, pf0 = nullptr, pf1 = nullptr;
+    Event cw0, cw1, pf0, pf1;
     CwtSlot cwt = nullptr;
     const int cws = st == c->hp_stream ? 0 : st == c->hp2_stream ? 1 : st == c->aux_stream ? 2 : -1;
-    if (c->chain_wait_trace && c->cwt_stamps && c->cwt_recs.size() < (size_t)CWT_MAX && cws >= 0 && cudaEventCreate(&cw0) == cudaSuccess) {
+    if (c->chain_wait_trace && c->cwt_stamps && c->cwt_recs.size() < (size_t)CWT_MAX && cws >= 0 && cw0.create(cudaEventDefault) == cudaSuccess) {
         cudaEventRecord(cw0, st);
         cwt = c->cwt_stamps + 2 * c->cwt_recs.size();
     }
-    if (c->profile && cudaEventCreate(&pf0) == cudaSuccess) cudaEventRecord(pf0, st);
+    if (c->profile && pf0.create(cudaEventDefault) == cudaSuccess) cudaEventRecord(pf0, st);
     cudaError_t e = cudaSuccess;
     if constexpr (std::is_void_v<decltype(enqueue(cwt))>) enqueue(cwt);
     else e = enqueue(cwt);
     c->launches++;
-    if (cw0) { cudaEventCreate(&cw1); cudaEventRecord(cw1, st); }
-    if (pf0) { cudaEventCreate(&pf1); cudaEventRecord(pf1, st); }
+    if (cw0) { cw1.create(cudaEventDefault); cudaEventRecord(cw1, st); }
+    if (pf0) { pf1.create(cudaEventDefault); cudaEventRecord(pf1, st); }
     const cudaError_t e2 = cudaGetLastError();
     if (e == cudaSuccess) e = e2;
-    if (e != cudaSuccess) {
-        for (cudaEvent_t ev : {cw0, cw1, pf0, pf1})
-            if (ev) cudaEventDestroy(ev);
-        return set_err(1000 + (int)e, "launch of %s failed: %s", what, cudaGetErrorString(e));
-    }
-    if (cw0) c->cwt_recs.push_back({c->cwt_unit, cws, prof_slot(c, what), cw0, cw1});
+    if (e != cudaSuccess) return set_err(1000 + (int)e, "launch of %s failed: %s", what, cudaGetErrorString(e));
+    if (cw0) c->cwt_recs.push_back({c->cwt_unit, cws, prof_slot(c, what), std::move(cw0), std::move(cw1)});
     if (pf0) {
         const int s = prof_slot(c, what);
-        c->prof_pending.push_back({s, pf0, pf1});
+        c->prof_pending.push_back({s, std::move(pf0), std::move(pf1)});
         c->prof_slots[s].work += work;
     }
     if (c->sync) {
@@ -316,68 +374,45 @@ static int launch(dhqr_context* c, cudaStream_t st, const char* what, double wor
 // Every column of `p` starts 16 B aligned (bulk copies legal): `p` itself is, and the leading dimension is even.
 static bool bulk_ok(const void* p, int64_t ld) { return ((uintptr_t)p & 15) == 0 && (ld & 1) == 0; }
 
-// Grows a workspace buffer.  The zero fill goes on `st`, the stream of the call that needs the buffer: a synchronous
-// cudaMemset would run on the legacy default stream, which a non-blocking caller stream is not ordered after.
-template <typename T>
-static int ensure(T** p, size_t* have, size_t need, cudaStream_t st) {
-    if (*have >= need && *p) return 0;
-    if (*p) CU(cudaFree(*p));
-    *p = nullptr;
-    *have = 0;
-    CU(cudaMalloc((void**)p, need * sizeof(T)));
-    CU(cudaMemsetAsync(*p, 0, need * sizeof(T), st));
-    *have = need;
-    return 0;
-}
-
 static constexpr int64_t WPART_TILES = 2304;   // capacity of the partial buffer in 128 x 64 tiles (151 MB per set)
 
 // npanels: outer panels of the factorisation about to run (T' slots of the look-ahead schedule); catchup: also size the fourth
 // V buffer / workspace set (dhqr_qr_host_f64 only)
 static int ensure_workspace(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n_local_max, int64_t npanels = 0, bool catchup = false) {
     TRY(set_attrs(c));
-    const int64_t vrows = rup(m, 128) + 128;
-    if (c->vrows_cap < vrows || !c->vpk2[0]) {
-        for (int b = 0; b < 3; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
-        for (int b = 0; b < 3; ++b) TRY(ensure(&c->vpkb[b], &c->vpkb_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
-        c->vrows_cap = vrows;
-    }
-    if (catchup) for (int b = 3; b < 3 + c->host_cu_streams; ++b) TRY(ensure(&c->vpk2[b], &c->vpk_elems[b], (size_t)(vrows / KC1) * VPK_CHUNK, st));
-    TRY(ensure(&c->linv_all, &c->linv_all_elems, (size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
-    TRY(ensure(&c->gram_all, &c->gram_all_elems, (size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
+    const size_t vpk_elems = (size_t)((rup(m, 128) + 128) / KC1) * VPK_CHUNK;
+    for (int b = 0; b < 3; ++b) TRY(c->vpk2[b].ensure(vpk_elems, st));
+    for (int b = 0; b < 3; ++b) TRY(c->vpkb[b].ensure(vpk_elems, st));
+    if (catchup) for (int b = 3; b < 3 + c->host_cu_streams; ++b) TRY(c->vpk2[b].ensure(vpk_elems, st));
+    TRY(c->linv_all.ensure((size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
+    TRY(c->gram_all.ensure((size_t)std::max<int64_t>(npanels, 4) * NBMAX * NBMAX, st));
     const int64_t tiles_max = (n_local_max + NBMAX + G1_BN - 1) / G1_BN + 1;
     for (int b = 0; b < (catchup ? 3 + c->host_cu_streams : 3); ++b) {
         auto& w = c->ws[b];
         // set 2 only ever updates the <= 128 columns of one panel: a quarter of the split-K partial buffer is plenty
-        TRY(ensure(&w.wpart, &w.wpart_elems, (size_t)(b != 2 ? std::max(WPART_TILES, tiles_max) : WPART_TILES / 4) * NBMAX * G1_BN, st));
+        TRY(w.wpart.ensure((size_t)(b != 2 ? std::max(WPART_TILES, tiles_max) : WPART_TILES / 4) * NBMAX * G1_BN, st));
         // sets 0-2 also hold W and Y of a panel pair: W_a and W_b side by side, 8 k-chunks of Y per column tile
         const size_t pairx = b < 3 ? 2 : 1;
-        TRY(ensure(&w.wsum, &w.wsum_elems, pairx * NBMAX * (rup(n_local_max + NBMAX, 128) + 128), st));
-        TRY(ensure(&w.ypk, &w.ypk_elems, pairx * (NBMAX / KC) * YT * LDK * ((n_local_max + YT - 1) / YT + 2), st));
-        TRY(ensure(&w.linv, &w.linv_elems, (size_t)NBMAX * NBMAX, st));
+        TRY(w.wsum.ensure(pairx * NBMAX * (rup(n_local_max + NBMAX, 128) + 128), st));
+        TRY(w.ypk.ensure(pairx * (NBMAX / KC) * YT * LDK * ((n_local_max + YT - 1) / YT + 2), st));
+        TRY(w.linv.ensure((size_t)NBMAX * NBMAX, st));
     }
-    size_t one = 0;
     if (!c->cells2) {
         const size_t words = (2 * (size_t)(PANEL_MAXG + 1) * (IB * (IB + 1) / 2) + IB * IB + 2 * IB) * 2;
-        CU(cudaMalloc((void**)&c->cells2, words * sizeof(unsigned long long)));
-        CU(cudaMemsetAsync(c->cells2, 0, words * sizeof(unsigned long long), st));
-        CU(cudaMalloc((void**)&c->fast_stats, 2 * sizeof(int)));
-        CU(cudaMemsetAsync(c->fast_stats, 0, 2 * sizeof(int), st));
+        TRY(c->cells2.ensure(words, st));
+        TRY(c->fast_stats.ensure(2, st));
         c->ll_epoch = 0;
     }
-    if (!c->cells) { one = 0; TRY(ensure(&c->cells, &one, (size_t)IB * (PANEL_MAXG + 2) * IB * 2, st)); c->ll_epoch = 0; }
+    if (!c->cells) { TRY(c->cells.ensure((size_t)IB * (PANEL_MAXG + 2) * IB * 2, st)); c->ll_epoch = 0; }
     if (!c->wctl) {
-        CU(cudaMalloc((void**)&c->wctl, sizeof(WideCtl)));
-        CU(cudaMemsetAsync(c->wctl, 0, sizeof(WideCtl), st));
+        TRY(c->wctl.ensure(1, st));
         // initial state {W_NOFAIL, 0}, in the caller's stream order
         TRY(launch(c, st, "k_wide_reset", 0.0, [&](CwtSlot) { k_wide_reset<<<1, 32, 0, st>>>(c->wctl); }));
-        size_t o3 = 0;
-        TRY(ensure(&c->wbuf, &o3, (size_t)5 * WP * WP + 3 * XL_ELEMS, st));
-        CU(cudaMalloc((void**)&c->wstamps, 32 * sizeof(long long)));
-        CU(cudaMemsetAsync(c->wstamps, 0, 32 * sizeof(long long), st));
+        TRY(c->wbuf.ensure((size_t)5 * WP * WP + 3 * XL_ELEMS, st));
+        TRY(c->wstamps.ensure(32, st));
     }
-    TRY(ensure(&c->v1, &c->v1_elems, (size_t)2 * rup(m + 4, 2), st));
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)1, st));
+    TRY(c->v1.ensure((size_t)2 * rup(m + 4, 2), st));
+    TRY(c->xbuf.ensure(1, st));
     return 0;
 }
 
@@ -419,9 +454,9 @@ static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* v
     const int bn = small ? G1S_BN : G1_BN;
     const int tiles = (nv + ncols + bn - 1) / bn;
     const int nchunks = (int)((rows + KC1 - 1) / KC1);
-    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart_elems / ((size_t)bn * NBPK)));
+    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart.n / ((size_t)bn * NBPK)));
     const int64_t pstride = (int64_t)tiles * bn * NBPK;
-    if ((size_t)(pstride * nsplit) > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
+    if ((size_t)(pstride * nsplit) > w.wpart.n) return set_err(4001, "internal: W partial workspace too small");
     GemmVtaArgs g1;
     g1.vpk = vpk; g1.voff = voff; g1.nv = nv;
     g1.A = B; g1.lda = ldb; g1.rows = rows; g1.na = ncols; g1.nchunks = nchunks;
@@ -455,7 +490,7 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     const int NBPK = small ? 32 : 128;          // kernel instantiation
     const int nv = reuse_T ? 0 : NBPK;
     const int next = nv + ncols;
-    if ((size_t)next * NBPK > w.wsum_elems) return set_err(4003, "internal: W workspace too small");
+    if ((size_t)next * NBPK > w.wsum.n) return set_err(4003, "internal: W workspace too small");
     int nsplit = 0;
     int64_t pstride = 0;
     TRY(launch_vta_partials(c, st, vpk, w, voff, nbp, nv, C, ldc, rows, ncols, small ? "k_gemm_vta32" : "k_gemm_vta128", &nsplit,
@@ -553,7 +588,7 @@ static int form_pair_gram(dhqr_context* c, cudaStream_t st, const double* vpk_b,
 static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const double* vpb, dhqr_context::WSet& w, int64_t rows,
                       double* C, int64_t ldc, int ncols, const double* Ta, const double* Tb, const double* G, int gate) {
     if (ncols <= 0) return 0;
-    if ((size_t)2 * ncols * NBMAX > w.wsum_elems) return set_err(4003, "internal: W workspace too small");
+    if ((size_t)2 * ncols * NBMAX > w.wsum.n) return set_err(4003, "internal: W workspace too small");
     double* Wa = w.wsum, *Wb = w.wsum + (size_t)ncols * NBMAX;
     TRY(block_w(c, st, vpa, w, C, ldc, rows, ncols, Wa));
     TRY(block_w(c, st, vpb, w, C + WP, ldc, rows - WP, ncols, Wb));
@@ -697,7 +732,7 @@ static int panel_gram_split(dhqr_context* c, const dhqr_context::WSet& w, int64_
     const int nchunks = (int)((rows + KC1 - 1) / KC1);
     const int cps = std::max(1, (nchunks + c->sms - 1) / c->sms);                           // chunks per CTA: whole waves of equal CTAs
     const int nsplit = (nchunks + cps - 1) / cps;
-    if ((size_t)nsplit * WP * WP > w.wpart_elems) return set_err(4001, "internal: W partial workspace too small");
+    if ((size_t)nsplit * WP * WP > w.wpart.n) return set_err(4001, "internal: W partial workspace too small");
     *nchunks_out = nchunks;
     *nsplit_out = nsplit;
     return 0;
@@ -730,7 +765,7 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     double* Z1 = MT + WP * WP, *Z2 = Z1 + XL_ELEMS, *Z23 = Z2 + XL_ELEMS;
     double* vflag = vpk + KC1;                  // padding row 64 of packed column 0: travels with the V buffer
     const int nq = (int)(g.vrows / KC1);
-    long long* stamps = c->wide_trace ? c->wstamps : nullptr;
+    long long* stamps = c->wide_trace ? c->wstamps.p : nullptr;
     // Gram matrices of the panel: partials over the window rows, split over CTAs as launch_panel_gram splits them
     int nchunks = 0, nsplit = 0;
     const int64_t pstride = (int64_t)WP * WP;
@@ -740,7 +775,7 @@ static int factor_outer_panel_wide(dhqr_context* c, cudaStream_t st, double* vpk
     r.Wp = nullptr; r.nchunks = nchunks; r.pstride = pstride;
     auto rmul = [&](int q0, int n, const double* Z, double* Pout, bool with_gram) -> int {
         if (n <= 0) return 0;
-        r.q0 = q0; r.nq = n; r.ZL = Z; r.P = Pout; r.Wp = with_gram ? w.wpart : nullptr;
+        r.q0 = q0; r.nq = n; r.ZL = Z; r.P = Pout; r.Wp = with_gram ? w.wpart.p : nullptr;
         const double work = 2.0 * 64.0 * n * WP * 80.0 + (with_gram ? 2.0 * (double)g.rows * WP * WP : 0.0);
         return launch(c, st, with_gram ? "k_rmul_gram" : "k_vpk_rmul", work, [&](CwtSlot cwt) {
             r.cwt = cwt;
@@ -802,11 +837,11 @@ static int factor_outer_panel(dhqr_context* c, cudaStream_t st, double* vpk, dhq
 static int mirror_panel_to_host(dhqr_context* c, cudaStream_t st, const Panel& p, int64_t m, int64_t col0, const double* A,
                                 int64_t lda) {
     if (!c->mirror_host) return 0;   // host entry point only: this panel's columns are final -> start their D2H now
-    cudaEvent_t ev;
-    CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    c->panel_events.push_back(ev);
+    Event ev;
+    CU(ev.create(cudaEventDisableTiming));
     CU(cudaEventRecord(ev, st));
     CU(cudaStreamWaitEvent(c->d2h_stream, ev, 0));
+    c->panel_events.push_back(std::move(ev));
     CU(cudaMemcpy2DAsync(c->mirror_host + p.c * c->mirror_lda, (size_t)c->mirror_lda * 8, A + (p.c - col0) * lda, (size_t)lda * 8,
                          (size_t)m * 8, (size_t)p.kb, cudaMemcpyDeviceToHost, c->d2h_stream));
     return 0;
@@ -903,24 +938,19 @@ static int qr_blocked_serial(dhqr_context* c, cudaStream_t st, int64_t m, int64_
 struct LookaheadEvents {
     dhqr_context* c;
     cudaStream_t st;
-    std::vector<cudaEvent_t> panel, next, bulk, a2, hp, caught;
-    cudaEvent_t fork = nullptr;
+    std::vector<Event> panel, next, bulk, a2, hp, caught;
+    Event fork;
     bool join = true;
     LookaheadEvents(dhqr_context* c_, cudaStream_t st_, int K) : c(c_), st(st_), panel(K), next(K), bulk(K), a2(K), hp(K) {}
     void dismiss() { join = false; }
     ~LookaheadEvents() {
-        cudaEvent_t done;
-        if (join && cudaEventCreateWithFlags(&done, cudaEventDisableTiming) == cudaSuccess) {
-            for (cudaStream_t s : {c->hp_stream, c->comm_stream, c->hp2_stream, c->cu_stream[0], c->cu_stream[1], c->cu_stream[2]}) {
+        Event done;
+        if (join && done.create(cudaEventDisableTiming) == cudaSuccess) {
+            for (cudaStream_t s : {c->hp_stream.h, c->comm_stream.h, c->hp2_stream.h, c->cu_stream[0].h, c->cu_stream[1].h, c->cu_stream[2].h}) {
                 cudaEventRecord(done, s);
                 cudaStreamWaitEvent(st, done, 0);
             }
-            cudaEventDestroy(done);
         }
-        for (const auto* v : {&panel, &next, &bulk, &a2, &hp, &caught})
-            for (cudaEvent_t e : *v)
-                if (e) cudaEventDestroy(e);
-        if (fork) cudaEventDestroy(fork);
     }
 };
 
@@ -928,7 +958,6 @@ struct LookaheadEvents {
 // order, starts to ~0 (atomicMin), ends to 0 (atomicMax)
 static int cwt_reset(dhqr_context* c, cudaStream_t st) {
     if (!c->chain_wait_trace || !c->cwt_stamps) return 0;
-    for (auto& r : c->cwt_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
     c->cwt_recs.clear();
     c->cwt_rows.clear();
     c->cwt_unit = 0;
@@ -940,7 +969,7 @@ static int cwt_reset(dhqr_context* c, cudaStream_t st) {
 // chain_wait_trace, after it: one row per traced launch (unit, stream, class, event span, stamp span, wait; ms)
 static int cwt_collect(dhqr_context* c, cudaStream_t st) {
     if (!c->chain_wait_trace || !c->cwt_stamps) return 0;
-    for (cudaStream_t s : {st, c->hp_stream, c->hp2_stream, c->aux_stream}) cudaStreamSynchronize(s);
+    for (cudaStream_t s : {st, c->hp_stream.h, c->hp2_stream.h, c->aux_stream.h}) cudaStreamSynchronize(s);
     std::vector<unsigned long long> t(2 * c->cwt_recs.size());
     if (!t.empty() && cudaMemcpy(t.data(), c->cwt_stamps, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess)
         return set_err(1002, "chain_wait_trace read-back failed");
@@ -1008,10 +1037,10 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     std::vector<char> haveA2(K, 0);
     const unsigned evflags = c->la_trace ? cudaEventDefault : cudaEventDisableTiming;
     for (int k = K0; k < K; ++k) {
-        CU(cudaEventCreateWithFlags(&evA2[k], cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&evPanel[k], evflags));
-        CU(cudaEventCreateWithFlags(&evNext[k], evflags));
-        CU(cudaEventCreateWithFlags(&evBulk[k], evflags));
+        CU(evA2[k].create(cudaEventDisableTiming));
+        CU(evPanel[k].create(evflags));
+        CU(evNext[k].create(evflags));
+        CU(evBulk[k].create(evflags));
     }
     // local intersection of the global column range [a, b) -> pointer + count
     auto clip = [&](int64_t a, int64_t b, int64_t& lo, int64_t& hi) { lo = std::max(a, col0); hi = std::min(b, lend); return hi > lo; };
@@ -1024,7 +1053,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
         if (c->nranks > 1) {
             const PanelGeom g = panel_geom(P(k), m);
             double* v = c->vpk2[k % 3];
-            CU(cudaEventCreateWithFlags(&evHp[k], cudaEventDisableTiming));
+            CU(evHp[k].create(cudaEventDisableTiming));
             CU(cudaEventRecord(evHp[k], hp));
             CU(cudaStreamWaitEvent(cs, evHp[k], 0));
             NC(g_nccl.Broadcast(v, v, (size_t)(g.vrows / KC1) * VPK_CHUNK, ncclFloat64, P(k).owner, c->comm, cs));
@@ -1074,7 +1103,7 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
     };
     std::vector<int> joinedAt;                                    // step at which each upload chunk joined (host_trace)
     TRY(cwt_reset(c, st));
-    if (cudaEventCreateWithFlags(&ev.fork, evflags) != cudaSuccess) return set_err(1001, "event create failed");
+    if (ev.fork.create(evflags) != cudaSuccess) return set_err(1001, "event create failed");
     cudaEventRecord(ev.fork, st);
     cudaStreamWaitEvent(hp, ev.fork, 0);                          // hp starts after everything already queued on st
     std::vector<char> ownT(K, 0);       // T'_k already sits in the ring slot on this rank (wide panel factored here, k_trecon)
@@ -1111,11 +1140,11 @@ static int qr_blocked_lookahead(dhqr_context* c, cudaStream_t st, int64_t m, int
             while (upnext < c->up_chunks.size() && (c->up_chunks[upnext].join <= k || c->up_chunks[upnext].c0 < t3)) {
                 const auto& u = c->up_chunks[upnext];
                 if (u.c0 < t2 || u.c0 != wend) return set_err(4005, "internal: upload chunk %d joins too late (step %d)", (int)upnext, k);
-                cudaEvent_t done;
-                if (cudaEventCreateWithFlags(&done, evflags) != cudaSuccess) return set_err(1001, "event create failed");
-                evCatch.push_back(done);
+                Event done;
+                if (done.create(evflags) != cudaSuccess) return set_err(1001, "event create failed");
+                evCatch.push_back(std::move(done));
                 joinedAt.push_back(k);
-                TRY(catch_up(u, (int)(upnext % (size_t)c->host_cu_streams), k, done));
+                TRY(catch_up(u, (int)(upnext % (size_t)c->host_cu_streams), k, evCatch.back()));
                 wend = u.c1;
                 ++upnext;
             }
@@ -1239,7 +1268,7 @@ static int qr_blocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, in
         // learn whether a panel was refused; if so, everything from that panel on was skipped on the device and is redone
         // here, that panel with the 32-column chain (same result on every rank: the verdict travels with the V buffer).
         int fail = W_NOFAIL;
-        CU(cudaMemcpyAsync(&fail, &c->wctl->fail_step, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(&fail, &c->wctl.p->fail_step, sizeof(int), cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         if (fail == W_NOFAIL) return 0;
         if (fail < pl.kstart || fail >= (int)panels.size()) return set_err(4004, "internal: bad restart index %d", fail);
@@ -1271,18 +1300,15 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
     const int64_t lend = col0 + nl;
     if (c->nranks == 1 && n > 0 && m <= (int64_t)UW_MAXI * UW_THREADS && c->unblocked_wave && !c->profile && !c->sync) {
         // single GPU, short columns: the whole column loop as one persistent cooperative launch (k_unblocked_wave)
-        if (c->uw_flags_n < (size_t)n) {
-            if (c->uw_flags) CU(cudaFree(c->uw_flags));
-            c->uw_flags = nullptr;
-            CU(cudaMalloc((void**)&c->uw_flags, sizeof(unsigned int) * (size_t)(n + 64)));
-            CU(cudaMemsetAsync(c->uw_flags, 0, sizeof(unsigned int) * (size_t)(n + 64), st));
-            c->uw_flags_n = (size_t)n + 64;
+        if (c->uw_flags.n < (size_t)n) {
+            TRY(c->uw_flags.ensure((size_t)n + 64, st));
             c->uw_epoch = 0;
         }
-        if (c->uw_epoch > 0xFFFFFFF0u) { CU(cudaMemsetAsync(c->uw_flags, 0, sizeof(unsigned int) * c->uw_flags_n, st)); c->uw_epoch = 0; }
+        if (c->uw_epoch > 0xFFFFFFF0u) { CU(cudaMemsetAsync(c->uw_flags, 0, sizeof(unsigned int) * c->uw_flags.n, st)); c->uw_epoch = 0; }
         const unsigned int tag = ++c->uw_epoch;
         int nn = (int)n;
-        void* args[] = {&A, &lda, &m, &nn, &alpha, &c->uw_flags, (void*)&tag};
+        unsigned int* flags = c->uw_flags;
+        void* args[] = {&A, &lda, &m, &nn, &alpha, &flags, (void*)&tag};
         const int G = (int)std::min<int64_t>(c->sms, n);
         return launch(c, st, "k_unblocked_wave", 16.0 * (double)m * n * n / 2, [&](CwtSlot) {
             return cudaLaunchCooperativeKernel((void*)k_unblocked_wave, dim3(G), dim3(UW_THREADS), args, 0, st);
@@ -1382,14 +1408,13 @@ static constexpr int QT_MAXG = 1024;
 static int qt_prepare(dhqr_context* c, cudaStream_t st, int64_t m, int64_t col0, int64_t nl, const double* A, int64_t lda) {
     const int npl = (int)((nl + NBMAX - 1) / NBMAX);
     if (npl <= 0) return 0;
-    TRY(ensure(&c->qt_T, &c->qt_T_elems, (size_t)npl * NBMAX * NBMAX, st));
+    TRY(c->qt_T.ensure((size_t)npl * NBMAX * NBMAX, st));
     if (!c->qt_part) {
-        CU(cudaMalloc((void**)&c->qt_part, sizeof(double) * (size_t)(QT_MAXG + 1) * WP));     // last row: y
-        CU(cudaMalloc((void**)&c->qt_ticket, sizeof(unsigned int)));
-        CU(cudaMemsetAsync(c->qt_ticket, 0, sizeof(unsigned int), st));
+        TRY(c->qt_part.alloc((size_t)(QT_MAXG + 1) * WP));     // last row: y
+        TRY(c->qt_ticket.ensure(1, st));
     }
     auto& w = c->ws[0];
-    if ((size_t)npl * NBMAX * NBMAX > w.wsum_elems) return set_err(4006, "internal: Gram workspace too small");
+    if ((size_t)npl * NBMAX * NBMAX > w.wsum.n) return set_err(4006, "internal: Gram workspace too small");
     for (int p = 0; p < npl; ++p) {
         const int64_t o = (int64_t)p * NBMAX, cs = col0 + o, r0 = cs & ~(int64_t)31;
         const int kb = (int)std::min<int64_t>(NBMAX, nl - o);
@@ -1434,12 +1459,8 @@ static bool qt_vec_ok(const dhqr_context* c, int64_t m, int nrhs) { return c->qt
 // Set-up shared by both wavefront substitutions: the x cells for nl local unknowns (zeroed in stream order when they grow)
 // and the co-residency limit of each wave kernel on this device.
 static int wave_prepare(dhqr_context* c, cudaStream_t st, int64_t nl) {
-    if (c->bs_cells_blocks < (size_t)(nl + 31) / 32 + 1) {
-        if (c->bs_cells) CU(cudaFree(c->bs_cells));
-        c->bs_cells = nullptr;
-        c->bs_cells_blocks = (size_t)(nl + 31) / 32 + 64;
-        CU(cudaMalloc((void**)&c->bs_cells, c->bs_cells_blocks * 32 * 16));
-        CU(cudaMemsetAsync(c->bs_cells, 0, c->bs_cells_blocks * 32 * 16, st));
+    if (c->bs_blocks() < (size_t)(nl + 31) / 32 + 1) {
+        TRY(c->bs_cells.ensure(((size_t)(nl + 31) / 32 + 64) * 64, st));
         c->bs_epoch = 0;
     }
     if (!c->bs_wave_max_ctas) {
@@ -1455,7 +1476,7 @@ static int wave_prepare(dhqr_context* c, cudaStream_t st, int64_t nl) {
 // Tag of the next wave launch; the cells are cleared before the 32-bit tag could come round to a value they still hold.
 static int wave_tag(dhqr_context* c, cudaStream_t st, uint32_t* tag) {
     if (c->bs_epoch > 0xFFFFFFF0u) {
-        CU(cudaMemsetAsync(c->bs_cells, 0, (size_t)c->bs_cells_blocks * 32 * 16, st));
+        CU(cudaMemsetAsync(c->bs_cells, 0, c->bs_cells.n * sizeof(unsigned long long), st));
         c->bs_epoch = 0;
     }
     *tag = ++c->bs_epoch;
@@ -1467,7 +1488,7 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
     if (nl <= 0) return 0;
     // one launch per right-hand side: a wavefront over 32-row strips (k_backsolve_wave); needs every CTA resident at once
     const int64_t nbk = (nl + 31) / 32, nlow = (col0 + 31) / 32;
-    if (c->bs_wave && nbk + nlow <= c->bs_wave_max_ctas && nbk <= (int64_t)c->bs_cells_blocks) {
+    if (c->bs_wave && nbk + nlow <= c->bs_wave_max_ctas && nbk <= (int64_t)c->bs_blocks()) {
         for (int rhs = 0; rhs < nrhs; ++rhs) {
             uint32_t tag;
             TRY(wave_tag(c, st, &tag));
@@ -1496,11 +1517,11 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
 static int forwardsolve_local(dhqr_context* c, cudaStream_t st, int64_t n, const double* A, int64_t lda, const double* alpha,
                               double* y, int64_t ldy, int nrhs) {
     if (n <= 0 || nrhs <= 0) return 0;
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n * nrhs, st));
+    TRY(c->xbuf.ensure((size_t)n * nrhs, st));
     TRY(wave_prepare(c, st, n));
     double* x = c->xbuf;
     const int64_t ldx = n, nbk = (n + 31) / 32;
-    if (c->bs_wave && nbk <= c->fs_wave_max_ctas && nbk <= (int64_t)c->bs_cells_blocks) {
+    if (c->bs_wave && nbk <= c->fs_wave_max_ctas && nbk <= (int64_t)c->bs_blocks()) {
         for (int rhs = 0; rhs < nrhs; ++rhs) {
             uint32_t tag;
             TRY(wave_tag(c, st, &tag));
@@ -1530,8 +1551,8 @@ extern "C" {
 int dhqr_version(void) { return DHQR_VERSION; }
 const char* dhqr_last_error(void) { return g_err; }
 
-static int create_common(dhqr_handle* h, int device) {
-    if (!h) return set_err(-1, "null handle pointer");
+// A new context on `device` in *out; on failure *out stays empty and nothing is left behind.
+static int create_context(std::unique_ptr<dhqr_context>& out, int device) {
     int ndev = 0;
     CU(cudaGetDeviceCount(&ndev));
     if (device < 0 || device >= ndev) return set_err(-2, "device %d out of range (%d devices)", device, ndev);
@@ -1540,28 +1561,34 @@ static int create_common(dhqr_handle* h, int device) {
     CU(cudaGetDeviceProperties(&prop, device));
     // sm_90a code runs on compute capability 9.0 only (architecture-specific features do not carry forward)
     if (prop.major != 9 || prop.minor != 0) return set_err(5001, "libdhqr is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
-    dhqr_context* c = new dhqr_context();
+    auto c = std::make_unique<dhqr_context>();
     c->device = device;
     c->sms = prop.multiProcessorCount;
-    CU(cudaMalloc((void**)&c->d_i64, sizeof(int64_t) * 2 * 1025));
-    CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&c->d2h_stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&c->h2d_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 3; ++i) CU(cudaStreamCreateWithFlags(&c->cu_stream[i], cudaStreamNonBlocking));
+    TRY(c->d_i64.alloc((size_t)2 * 1025));
+    CU(c->copy_stream.create());
+    CU(c->d2h_stream.create());
+    CU(c->h2d_stream.create());
+    for (int i = 0; i < 3; ++i) CU(c->cu_stream[i].create());
     {
         int lo = 0, hi = 0;
         CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        CU(cudaStreamCreateWithPriority(&c->hp_stream, cudaStreamNonBlocking, hi));
-        CU(cudaStreamCreateWithPriority(&c->comm_stream, cudaStreamNonBlocking, hi));
-        CU(cudaStreamCreateWithPriority(&c->hp2_stream, cudaStreamNonBlocking, hi));
-        CU(cudaStreamCreateWithPriority(&c->aux_stream, cudaStreamNonBlocking, hi));
-        for (int i = 0; i < 4; ++i) CU(cudaEventCreateWithFlags(&c->ev_aux[i], cudaEventDisableTiming));
+        CU(c->hp_stream.create(hi));
+        CU(c->comm_stream.create(hi));
+        CU(c->hp2_stream.create(hi));
+        CU(c->aux_stream.create(hi));
+        for (int i = 0; i < 4; ++i) CU(c->ev_aux[i].create(cudaEventDisableTiming));
     }
-    *h = c;
+    out = std::move(c);
     return 0;
 }
 
-int dhqr_create(dhqr_handle* h, int device) { return create_common(h, device); }
+int dhqr_create(dhqr_handle* h, int device) {
+    if (!h) return set_err(-1, "null handle pointer");
+    std::unique_ptr<dhqr_context> c;
+    TRY(create_context(c, device));
+    *h = c.release();
+    return 0;
+}
 
 int dhqr_nccl_unique_id(void* out) {
     if (!out) return set_err(-1, "null output");
@@ -1576,16 +1603,18 @@ int dhqr_create_dist(dhqr_handle* h, int device, const void* unique_id, int rank
     if (nranks < 1 || nranks > 1024) return set_err(-5, "nranks out of range");
     if (rank < 0 || rank >= nranks) return set_err(-4, "rank out of range");
     if (nranks > 1 && !unique_id) return set_err(-3, "null unique id");
-    TRY(create_common(h, device));
-    dhqr_context* c = *h;
+    if (!h) return set_err(-1, "null handle pointer");
+    if (nranks > 1) TRY(load_nccl());
+    std::unique_ptr<dhqr_context> c;
+    TRY(create_context(c, device));
     c->rank = rank;
     c->nranks = nranks;
     if (nranks > 1) {
-        TRY(load_nccl());
         ncclUniqueId id;
         memcpy(&id, unique_id, sizeof(id));
         NC(g_nccl.CommInitRank(&c->comm, nranks, id, rank));
     }
+    *h = c.release();
     return 0;
 }
 
@@ -1593,28 +1622,7 @@ int dhqr_destroy(dhqr_handle c) {
     if (!c) return 0;
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
-    if (c->comm) g_nccl.CommDestroy(c->comm);
-    cudaFree(c->linv_all);
-    for (int b = 0; b < 6; ++b) {
-        cudaFree(c->vpk2[b]);
-        cudaFree(c->ws[b].wpart); cudaFree(c->ws[b].wsum); cudaFree(c->ws[b].ypk); cudaFree(c->ws[b].linv);
-    }
-    cudaFree(c->uw_flags);
-    cudaFree(c->qt_T); cudaFree(c->qt_part); cudaFree(c->qt_ticket);
-    cudaFree(c->wctl); cudaFree(c->wbuf); cudaFree(c->wstamps); cudaFree(c->bs_cells);
-    cudaFree(c->cells); cudaFree(c->cells2); cudaFree(c->fast_stats); cudaFree(c->panel_trace); cudaFree(c->cwt_stamps);
-    if (c->hp_stream) cudaStreamDestroy(c->hp_stream);
-    if (c->comm_stream) cudaStreamDestroy(c->comm_stream);
-    if (c->hp2_stream) cudaStreamDestroy(c->hp2_stream);
-    if (c->aux_stream) cudaStreamDestroy(c->aux_stream);
-    for (int i = 0; i < 4; ++i)
-        if (c->ev_aux[i]) cudaEventDestroy(c->ev_aux[i]);
-    cudaFree(c->qp_buf); cudaFree(c->qp_flag); cudaFree(c->qp_ctl);
-    cudaFree(c->v1); cudaFree(c->xbuf); cudaFree(c->xfer); cudaFree(c->hostA); cudaFree(c->hostB); cudaFree(c->d_i64);
-    if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-    if (c->d2h_stream) cudaStreamDestroy(c->d2h_stream);
-    if (c->h2d_stream) cudaStreamDestroy(c->h2d_stream);
-    for (int i = 0; i < 3; ++i) if (c->cu_stream[i]) cudaStreamDestroy(c->cu_stream[i]);
+    if (c->comm) g_nccl.CommDestroy(c->comm);   // before the buffers it may still reference are freed
     delete c;
     return 0;
 }
@@ -1668,7 +1676,7 @@ int dhqr_set_option(dhqr_handle c, const char* key, int64_t value) {
     } else if (!strcmp(key, "la_trace")) {
         c->la_trace = value ? 1 : 0;
     } else if (!strcmp(key, "chain_wait_trace")) {
-        if (value && !c->cwt_stamps) CU(cudaMalloc((void**)&c->cwt_stamps, sizeof(unsigned long long) * 2 * CWT_MAX));
+        if (value && !c->cwt_stamps) TRY(c->cwt_stamps.alloc((size_t)2 * CWT_MAX));
         c->chain_wait_trace = value ? 1 : 0;
     } else if (!strcmp(key, "panel_fast")) {
         c->panel_fast = value ? 1 : 0;
@@ -1681,13 +1689,11 @@ int dhqr_set_option(dhqr_handle c, const char* key, int64_t value) {
         c->wide_trace = value ? 1 : 0;
     } else if (!strcmp(key, "panel_trace")) {
         if (value && !c->panel_trace) {
-            CU(cudaMalloc((void**)&c->panel_trace, sizeof(long long) * (size_t)PANEL_MAXG * IB * 8));
             // no stream here: the fill is complete before the call returns, so every later call sees it
-            CU(cudaMemsetAsync(c->panel_trace, 0, sizeof(long long) * (size_t)PANEL_MAXG * IB * 8, cudaStreamLegacy));
+            TRY(c->panel_trace.ensure((size_t)PANEL_MAXG * IB * 8, cudaStreamLegacy));
             CU(cudaStreamSynchronize(cudaStreamLegacy));
         } else if (!value && c->panel_trace) {
-            CU(cudaFree(c->panel_trace));
-            c->panel_trace = nullptr;
+            CU(c->panel_trace.release());
         }
     } else {
         return set_err(-2, "unknown option '%s'", key);
@@ -1717,7 +1723,7 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
     else if (!strcmp(key, "pair_units")) *value = c->pair_units;
     else if (!strcmp(key, "qrcp_renorms")) {
         unsigned long long r = 0;
-        if (c->qp_ctl) CU(cudaMemcpy(&r, &c->qp_ctl->renorms, sizeof(r), cudaMemcpyDeviceToHost));
+        if (c->qp_ctl) CU(cudaMemcpy(&r, &c->qp_ctl.p->renorms, sizeof(r), cudaMemcpyDeviceToHost));
         *value = (int64_t)r;
     }
     else if (!strcmp(key, "panels_fast") || !strcmp(key, "panels_fallback")) {
@@ -1746,8 +1752,6 @@ static int prof_drain(dhqr_context* c) {
         CU(cudaEventElapsedTime(&ms, r.e0, r.e1));
         c->prof_slots[r.slot].ms += ms;
         c->prof_slots[r.slot].count += 1;
-        cudaEventDestroy(r.e0);
-        cudaEventDestroy(r.e1);
     }
     c->prof_pending.clear();
     return 0;
@@ -1791,7 +1795,7 @@ int dhqr_qr_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
 static int rhs_message(dhqr_context* c, cudaStream_t st, double* b, int64_t ldb, int64_t rows, int nrhs, double** msg) {
     *msg = b;
     if (ldb == rows || nrhs == 1) return 0;
-    TRY(ensure(&c->xfer, &c->xfer_elems, (size_t)rows * nrhs, st));
+    TRY(c->xfer.ensure((size_t)rows * nrhs, st));
     *msg = c->xfer;
     return 0;
 }
@@ -1882,7 +1886,7 @@ int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     std::vector<int64_t> col0s, nls;
     TRY(gather_partition(c, st, col0, n_local, col0s, nls));
     TRY(check_partition(col0s, nls, n_global));
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n_global * nrhs, st));
+    TRY(c->xbuf.ensure((size_t)n_global * nrhs, st));
     TRY(wave_prepare(c, st, n_local));
     // C4 (S:260-267), column oriented: the last owner solves its block of unknowns and removes their
     // contribution from the rows above; the partially reduced right-hand side then moves one rank down.
@@ -2016,9 +2020,9 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t n = n_global;
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)2 * n * nrhs, st));
+    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
     const double2* A = (const double2*)dA;
-    double2* x = (double2*)c->xbuf;
+    double2* x = (double2*)c->xbuf.p;
     for (int64_t o = ((n - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {     // S:260: i = n:-1:1, by blocks
         const int bs = (int)std::min<int64_t>(BS_BLK, n - o);
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((o + 255) / 256, 2 * c->sms));
@@ -2151,8 +2155,8 @@ static int check_adj(dhqr_context* c, int64_t m, int64_t n, const void* A, int64
 // complex y[0:n] <- R^{-H} y[0:n], blocks of BS_BLK columns first to last, through c->xbuf
 static int forwardsolve_c64_local(dhqr_context* c, cudaStream_t st, int64_t n, const double2* A, int64_t lda, const double2* alpha,
                                   double2* y, int64_t ldy, int nrhs) {
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)2 * n * nrhs, st));
-    double2* x = (double2*)c->xbuf;
+    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
+    double2* x = (double2*)c->xbuf.p;
     for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
         const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
         const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
@@ -2241,12 +2245,9 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, do
     const int64_t p1 = (m + QP_PROWS - 1) / QP_PROWS;                                    // k_qrcp_pivot CTAs
     const int64_t smax = std::max<int64_t>(1, std::min<int64_t>((m + QP_THREADS - 1) / QP_THREADS, 8 * c->sms));
     const size_t need = (size_t)2 * n + (size_t)QP_NB * n + (size_t)m + (size_t)p1 + (size_t)smax * n;
-    TRY(ensure(&c->qp_buf, &c->qp_buf_elems, need, st));
-    TRY(ensure(&c->qp_flag, &c->qp_flag_elems, (size_t)n, st));
-    if (!c->qp_ctl) {
-        CU(cudaMalloc((void**)&c->qp_ctl, sizeof(QrcpCtl)));
-        CU(cudaMemsetAsync(c->qp_ctl, 0, sizeof(QrcpCtl), st));
-    }
+    TRY(c->qp_buf.ensure(need, st));
+    TRY(c->qp_flag.ensure((size_t)n, st));
+    TRY(c->qp_ctl.ensure(1, st));
     QrcpArgs a;
     a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
     a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = a.vn2 + n; a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
@@ -2333,7 +2334,7 @@ int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
-    TRY(ensure(&c->xbuf, &c->xbuf_elems, (size_t)n * nrhs, st));
+    TRY(c->xbuf.ensure((size_t)n * nrhs, st));
     if (rank > 0) {
         // (Q'b)[0:rank] needs only the first `rank` reflectors
         if (qt_vec_ok(c, m, nrhs)) {
@@ -2432,13 +2433,12 @@ int dhqr_qr_host_f64(dhqr_handle c, int64_t m, int64_t n, double* hA, int64_t ld
     else { B = {0, n}; join = {0}; }
     const int nch = (int)B.size() - 1;
     cudaStream_t st = c->copy_stream;
-    TRY(ensure(&c->hostA, &c->hostA_elems, (size_t)ldd * n + (size_t)n, st));
+    TRY(c->hostA.ensure((size_t)ldd * n + (size_t)n, st));
     // everything sized once, before the pipeline starts: growing a buffer later would synchronise the device
     TRY(ensure_workspace(c, st, m, n, blocked ? (n + nbe - 1) / nbe + 1 : 0, nch > 1));
     double* dA = c->hostA;
     double* dal = c->hostA + (size_t)ldd * n;
-    int rc = 0;
-    std::vector<cudaEvent_t> evUp;
+    std::vector<Event> evUp;
     struct timespec ts0;
     clock_gettime(CLOCK_MONOTONIC, &ts0);
     auto stamp = [&](const char* what, bool sync_all) {
@@ -2454,49 +2454,49 @@ int dhqr_qr_host_f64(dhqr_handle c, int64_t m, int64_t n, double* hA, int64_t ld
         fprintf(stderr, "\n");
     }
     c->up_chunks.clear();
-    do {
-        if (cudaMemcpy2DAsync(dA, (size_t)ldd * 8, hA, (size_t)lda * 8, (size_t)m * 8, (size_t)B[1], cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = set_err(1001, "H2D failed"); break; }
+    // The pipeline returns at its first failure, possibly with work still queued; the tail below runs after it either way.
+    const int rc = [&]() -> int {
+        if (cudaMemcpy2DAsync(dA, (size_t)ldd * 8, hA, (size_t)lda * 8, (size_t)m * 8, (size_t)B[1], cudaMemcpyHostToDevice, st) != cudaSuccess)
+            return set_err(1001, "H2D failed");
         if (nch > 1) {
             // the later chunks go up one after the other BEHIND the first (concurrent uploads would share the link and delay the
             // start of the factorisation), on their own stream
-            cudaEvent_t e0;
-            if (cudaEventCreateWithFlags(&e0, cudaEventDisableTiming) != cudaSuccess) { rc = set_err(1001, "event create failed"); break; }
-            evUp.push_back(e0);
-            cudaEventRecord(e0, st);
-            cudaStreamWaitEvent(c->h2d_stream, e0, 0);
-            for (int j = 1; j < nch && !rc; ++j) {
-                cudaEvent_t e;
-                if (cudaEventCreateWithFlags(&e, c->host_trace ? cudaEventDefault : cudaEventDisableTiming) != cudaSuccess) { rc = set_err(1001, "event create failed"); break; }
-                evUp.push_back(e);
+            evUp.emplace_back();
+            if (evUp.back().create(cudaEventDisableTiming) != cudaSuccess) return set_err(1001, "event create failed");
+            cudaEventRecord(evUp.back(), st);
+            cudaStreamWaitEvent(c->h2d_stream, evUp.back(), 0);
+            for (int j = 1; j < nch; ++j) {
+                evUp.emplace_back();
+                if (evUp.back().create(c->host_trace ? cudaEventDefault : cudaEventDisableTiming) != cudaSuccess)
+                    return set_err(1001, "event create failed");
                 if (cudaMemcpy2DAsync(dA + B[j] * ldd, (size_t)ldd * 8, hA + B[j] * lda, (size_t)lda * 8, (size_t)m * 8, (size_t)(B[j + 1] - B[j]),
-                                      cudaMemcpyHostToDevice, c->h2d_stream) != cudaSuccess) { rc = set_err(1001, "H2D failed"); break; }
-                cudaEventRecord(e, c->h2d_stream);
-                c->up_chunks.push_back({B[j], B[j + 1], e, join[j]});
+                                      cudaMemcpyHostToDevice, c->h2d_stream) != cudaSuccess)
+                    return set_err(1001, "H2D failed");
+                cudaEventRecord(evUp.back(), c->h2d_stream);
+                c->up_chunks.push_back({B[j], B[j + 1], evUp.back(), join[j]});
             }
-            if (rc) break;
         }
         stamp("first chunk uploaded", true);
         if (blocked) { c->mirror_host = hA; c->mirror_lda = lda; }   // finished panels stream back while later panels are factored
         const int la_trace_keep = c->la_trace;
         if (c->host_trace) c->la_trace = 1;
-        rc = dhqr_qr_f64(c, m, n, 0, n, dA, ldd, dal, nb, st);
+        const int rq = dhqr_qr_f64(c, m, n, 0, n, dA, ldd, dal, nb, st);
         c->la_trace = la_trace_keep;
         c->mirror_host = nullptr;
-        if (rc) break;
+        TRY(rq);
         stamp("factored", true);
-        if (!blocked)
-            if (cudaMemcpy2DAsync(hA, (size_t)lda * 8, dA, (size_t)ldd * 8, (size_t)m * 8, (size_t)n, cudaMemcpyDeviceToHost, st) != cudaSuccess) { rc = set_err(1001, "D2H failed"); break; }
-        if (cudaMemcpyAsync(h_alpha, dal, (size_t)n * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) { rc = set_err(1001, "D2H failed"); break; }
-    } while (0);
+        if (!blocked && cudaMemcpy2DAsync(hA, (size_t)lda * 8, dA, (size_t)ldd * 8, (size_t)m * 8, (size_t)n, cudaMemcpyDeviceToHost, st) != cudaSuccess)
+            return set_err(1001, "D2H failed");
+        if (cudaMemcpyAsync(h_alpha, dal, (size_t)n * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) return set_err(1001, "D2H failed");
+        return 0;
+    }();
     c->mirror_host = nullptr;
     c->up_chunks.clear();
-    cudaError_t e0 = cudaStreamSynchronize(c->h2d_stream), e1 = cudaStreamSynchronize(st), e2 = cudaStreamSynchronize(c->d2h_stream);
+    const cudaError_t e0 = cudaStreamSynchronize(c->h2d_stream), e1 = cudaStreamSynchronize(st), e2 = cudaStreamSynchronize(c->d2h_stream);
     cudaError_t e3 = cudaSuccess;
     for (int i = 0; i < 3; ++i) { const cudaError_t e4 = cudaStreamSynchronize(c->cu_stream[i]); if (e3 == cudaSuccess) e3 = e4; }
     stamp("everything back on the host", false);
-    for (cudaEvent_t ev : c->panel_events) cudaEventDestroy(ev);
     c->panel_events.clear();
-    for (cudaEvent_t ev : evUp) cudaEventDestroy(ev);
     if (rc) return rc;
     if (e0 != cudaSuccess) return set_err(1000 + (int)e0, "qr_host H2D: %s", cudaGetErrorString(e0));
     if (e1 != cudaSuccess) return set_err(1000 + (int)e1, "qr_host: %s", cudaGetErrorString(e1));
@@ -2516,8 +2516,8 @@ int dhqr_ldiv_host_f64(dhqr_handle c, int64_t m, int64_t n, const double* hA, in
     CU(cudaSetDevice(c->device));
     const int64_t ldd = rup(m, 32);
     cudaStream_t st = c->copy_stream;
-    TRY(ensure(&c->hostA, &c->hostA_elems, (size_t)ldd * n + (size_t)n, st));
-    TRY(ensure(&c->hostB, &c->hostB_elems, (size_t)ldd, st));
+    TRY(c->hostA.ensure((size_t)ldd * n + (size_t)n, st));
+    TRY(c->hostB.ensure((size_t)ldd, st));
     double* dA = c->hostA;
     double* dal = c->hostA + (size_t)ldd * n;
     CU(cudaMemcpy2DAsync(dA, (size_t)ldd * 8, hA, (size_t)lda * 8, (size_t)m * 8, (size_t)n, cudaMemcpyHostToDevice, st));
@@ -2596,14 +2596,14 @@ int dhqr_debug_copy_f64(dhqr_handle c, const char* which, double* d_dst, int64_t
     }
     const double* src = nullptr;
     size_t have = 0;
-    if (!strcmp(which, "wpart")) { src = c->ws[0].wpart; have = c->ws[0].wpart_elems; }
-    else if (!strcmp(which, "wsum")) { src = c->ws[0].wsum; have = c->ws[0].wsum_elems; }
-    else if (!strcmp(which, "ypk")) { src = c->ws[0].ypk; have = c->ws[0].ypk_elems; }
+    if (!strcmp(which, "wpart")) { src = c->ws[0].wpart; have = c->ws[0].wpart.n; }
+    else if (!strcmp(which, "wsum")) { src = c->ws[0].wsum; have = c->ws[0].wsum.n; }
+    else if (!strcmp(which, "ypk")) { src = c->ws[0].ypk; have = c->ws[0].ypk.n; }
     else if (!strcmp(which, "linv")) { src = c->ws[0].linv; have = (size_t)NBMAX * NBMAX; }
-    else if (!strcmp(which, "vpk")) { src = c->vpk2[0]; have = c->vpk_elems[0]; }
-    else if (!strcmp(which, "wstamps")) { src = (const double*)c->wstamps; have = c->wstamps ? 32 : 0; }
-    else if (!strcmp(which, "wide")) { src = c->wbuf; have = c->wbuf ? (size_t)5 * WP * WP + 3 * XL_ELEMS : 0; }
-    else if (!strcmp(which, "panel_trace")) { src = (const double*)c->panel_trace; have = c->panel_trace ? (size_t)PANEL_MAXG * IB * 8 : 0; }
+    else if (!strcmp(which, "vpk")) { src = c->vpk2[0]; have = c->vpk2[0].n; }
+    else if (!strcmp(which, "wstamps")) { src = (const double*)c->wstamps.p; have = c->wstamps.n; }
+    else if (!strcmp(which, "wide")) { src = c->wbuf; have = c->wbuf.n; }
+    else if (!strcmp(which, "panel_trace")) { src = (const double*)c->panel_trace.p; have = c->panel_trace.n; }
     else return set_err(-2, "unknown buffer '%s'", which);
     if (nelems < 0 || (size_t)nelems > have) return set_err(-4, "nelems out of range (have %zu)", have);
     CU(cudaMemcpyAsync(d_dst, src, sizeof(double) * (size_t)nelems, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));

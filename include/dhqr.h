@@ -68,7 +68,8 @@ int dhqr_create(dhqr_handle *h, int device);
  * Distributed/SharedArrays (S:116-118, S:141-143, S:227-229, S:260-267, S:302, S:318).
  * NCCL is loaded on first use (here or in dhqr_nccl_unique_id): from the path in the environment variable
  * DHQR_NCCL_LIBRARY if it is set (opened RTLD_LOCAL, so it never displaces a libnccl the process already has), otherwise
- * libnccl.so.2 by soname. */
+ * libnccl.so.2 by soname.
+ * Both create calls write *h only on success; a failed call leaves *h as it was and holds nothing on the device. */
 int dhqr_create_dist(dhqr_handle *h, int device, const void *unique_id, int rank, int nranks);
 int dhqr_nccl_unique_id(void *out_unique_id);
 int dhqr_destroy(dhqr_handle h);
