@@ -552,6 +552,43 @@ class PivotedHouseholderQRStruct:
 
     solve = ldiv
 
+    def cod(self, rcond: Optional[float] = None) -> "CompleteOrthogonalStruct":
+        """The complete orthogonal decomposition A P ~ Q1 [U' 0] Z' at rank ``self.rank(rcond)`` (DESIGN §2.8), whose ``.ldiv``
+        gives the minimum-norm least-squares solution, as numpy.linalg.lstsq and LAPACK dgelsy do.  The factorisation is read,
+        never modified."""
+        r = self.rank(rcond)
+        F, gamma = cod_(self.A, self.α, r, self.handle)
+        return CompleteOrthogonalStruct(self, F, gamma, r)
+
+
+class CompleteOrthogonalStruct:
+    """A P ~ Q1 [U' 0] Z' from ``PivotedHouseholderQRStruct.cod``: ``.qrcp`` is the pivoted factorisation (Q1, P), ``.F`` and ``.γ``
+    (``.gamma``) the factorisation R_r' = Z [U; 0] of the leading ``.rank`` rows of R, in the library's storage format (so
+    form_q(F) is Z[:, :rank], and forwardsolve_ / apply_q_ take (F, γ) as any other factorisation)."""
+
+    def __init__(self, qrcp, F, gamma, rank: int):
+        self.qrcp = qrcp
+        self.F = F
+        self.γ = gamma
+        self.rank = rank
+
+    @property
+    def gamma(self):
+        return self.γ
+
+    def ldiv(self, b):
+        """The minimum-norm solution x of min ||A x - b|| at rank ``self.rank``; neither the factorisations nor b is modified.
+        ``b``: length m, or (m, k).  Returns a new length-n vector or (n, k) tensor."""
+        A = self.qrcp.A
+        if b.dim() == 1:
+            s = b.to(device=A.device, dtype=A.dtype).clone()
+        else:
+            s = to_colmajor(b, device=A.device)
+        solve_cod_(s, A, self.qrcp.p, self.F, self.γ, self.rank, self.qrcp.handle)
+        return s[:A.shape[1]].clone()
+
+    solve = ldiv
+
 
 def qrcp_(A: torch.Tensor, handle: Optional[Handle] = None) -> PivotedHouseholderQRStruct:
     """A P = Q R with column pivoting (LAPACK dgeqp3; scipy.linalg.qr(pivoting=True)), in place, on a column-major float64 CUDA
@@ -583,6 +620,47 @@ def solve_qrcp_(b: torch.Tensor, A: torch.Tensor, alpha: torch.Tensor, p: torch.
     with torch.cuda.device(A.device):
         _lib.call("dhqr_solve_qrcp_f64", h.raw, m, n, int(rank), C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
                   C.c_void_p(p.data_ptr()), C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(A.device))
+    return b[:n]
+
+
+def cod_(A: torch.Tensor, alpha: torch.Tensor, rank: int, handle: Optional[Handle] = None):
+    """The second factorisation of the complete orthogonal decomposition at the given rank, from a factorisation made by
+    ``qrcp_``: R_r' = Z [U; 0] with R_r = rows [0, rank) of R = triu(A, 1) + diag(alpha).  Returns (F, γ): F a fresh (n, rank)
+    column-major tensor in the library's storage format, γ = diag(U).  A and alpha are read, never written.  Synchronises the
+    stream once when a 128-column panel of R_r' went through the wide chain, as qr_ does."""
+    if not isinstance(A, torch.Tensor) or not A.is_cuda or A.dtype != torch.float64:
+        raise TypeError("cod_ works on a column-major float64 CUDA tensor")
+    if alpha.dtype != torch.float64:
+        raise TypeError("alpha must be float64")
+    h = handle or default_handle(A.device.index)
+    m, n = A.shape
+    rank = int(rank)
+    F = colmajor_empty(n, max(rank, 0), A.device)
+    gamma = torch.zeros(max(rank, 0), dtype=torch.float64, device=A.device)
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_cod_f64", h.raw, m, n, rank, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+                  C.c_void_p(F.data_ptr() if rank > 0 else None), max(n, 1), C.c_void_p(gamma.data_ptr() if rank > 0 else None),
+                  _stream_ptr(A.device))
+    return F, gamma
+
+
+def solve_cod_(b: torch.Tensor, A: torch.Tensor, p: torch.Tensor, F: torch.Tensor, gamma: torch.Tensor, rank: int,
+               handle: Optional[Handle] = None) -> torch.Tensor:
+    """x = P Z [U^{-T} (Q'b)[0:rank]; 0], the minimum-norm solution at the given rank, from ``qrcp_``'s (A, p) and ``cod_``'s
+    (F, γ) at that rank.  ``b``: length m, or (m, k) column-major; on return b[0:n] = x (returned as a view) and rows n..m-1
+    hold rows n..m-1 of H_rank ... H_1 b, as in solve_qrcp_."""
+    h = handle or default_handle(A.device.index)
+    m, n = A.shape
+    if p.dtype != torch.int64 or F.dtype != torch.float64 or gamma.dtype != torch.float64:
+        raise TypeError("p must be int64, F and gamma float64")
+    rank = int(rank)
+    if rank > 0 and (tuple(F.shape) != (n, rank) or tuple(gamma.shape) != (rank,)):
+        raise ValueError(f"F must be ({n}, {rank}) and gamma ({rank},)")
+    ldb, nrhs = _rhs_args(b, m, A.dtype)
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_solve_cod_f64", h.raw, m, n, rank, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(p.data_ptr()),
+                  C.c_void_p(F.data_ptr() if rank > 0 else None), _lda(F) if rank > 0 else max(n, 1),
+                  C.c_void_p(gamma.data_ptr() if rank > 0 else None), C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(A.device))
     return b[:n]
 
 

@@ -2197,12 +2197,9 @@ int dhqr_forwardsolve_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, i
     return forwardsolve_c64_local(c, (cudaStream_t)stream, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs);
 }
 
-int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
-                       int64_t ldb, int nrhs, void* stream) {
-    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, false));
-    if (m == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
+// y = Q [R^{-T} c; 0] in place on b[0:m] (c = b[0:n]): the body of dhqr_solve_adj_f64, also the second stage of dhqr_solve_cod_f64
+static int solve_adj_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha,
+                           double* d_b, int64_t ldb, int nrhs) {
     TRY(forwardsolve_local(c, st, n, dA, lda, d_alpha, d_b, ldb, nrhs));
     if (m > n) CU(cudaMemset2DAsync(d_b + n, (size_t)ldb * 8, 0, (size_t)(m - n) * 8, nrhs, st));    // n = 0: y = 0, as in ?gels
     if (n == 0) return 0;
@@ -2214,6 +2211,14 @@ int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, in
         TRY(apply_qt_local(c, st, m, 0, n, dA, lda, d_b, ldb, nrhs, 1));
     }
     return 0;
+}
+
+int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
+                       int64_t ldb, int nrhs, void* stream) {
+    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, false));
+    if (m == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return solve_adj_local(c, (cudaStream_t)stream, m, n, dA, lda, d_alpha, d_b, ldb, nrhs);
 }
 
 int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
@@ -2312,6 +2317,29 @@ int dhqr_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, double* dA, int64_t lda, 
     return qrcp_local(c, (cudaStream_t)stream, m, n, dA, lda, d_alpha, d_jpvt);
 }
 
+// (Q'b)[0:rank]: the first `rank` reflectors of a pivoted factorisation on b, the first stage of both pivoted solves
+static int qrcp_qtb(dhqr_context* c, cudaStream_t st, int64_t m, int64_t rank, const double* dA, int64_t lda, double* d_b, int64_t ldb,
+                    int nrhs) {
+    if (qt_vec_ok(c, m, nrhs)) {
+        TRY(qt_prepare(c, st, m, 0, rank, dA, lda));
+        return apply_qt_local_vec(c, st, m, 0, rank, dA, lda, d_b, 0);
+    }
+    return apply_qt_local(c, st, m, 0, rank, dA, lda, d_b, ldb, nrhs);
+}
+
+// b[jpvt[i]] = z[i] for i < rank, 0 for rank <= i < n, on every right-hand side; jpvt entries outside [0, n) are skipped
+static int qrcp_scatter(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double* z, int64_t ldz, const int64_t* d_jpvt,
+                        double* d_b, int64_t ldb, int nrhs) {
+    for (int r0 = 0; r0 < nrhs; r0 += 65535) {
+        const int nr = std::min(nrhs - r0, 65535);
+        TRY(launch(c, st, "k_qrcp_scatter", 0.0, [&](CwtSlot) {
+            k_qrcp_scatter<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(z + (size_t)r0 * ldz, ldz, d_jpvt, n, rank,
+                                                                                         d_b + (size_t)r0 * ldb, ldb);
+        }));
+    }
+    return 0;
+}
+
 int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha,
                         const int64_t* d_jpvt, double* d_b, int64_t ldb, int nrhs, void* stream) {
     if (!c) return set_err(-1, "null handle");
@@ -2336,24 +2364,88 @@ int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const
     TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
     TRY(c->xbuf.ensure((size_t)n * nrhs, st));
     if (rank > 0) {
-        // (Q'b)[0:rank] needs only the first `rank` reflectors
-        if (qt_vec_ok(c, m, nrhs)) {
-            TRY(qt_prepare(c, st, m, 0, rank, dA, lda));
-            TRY(apply_qt_local_vec(c, st, m, 0, rank, dA, lda, d_b, 0));
-        } else {
-            TRY(apply_qt_local(c, st, m, 0, rank, dA, lda, d_b, ldb, nrhs));
-        }
+        TRY(qrcp_qtb(c, st, m, rank, dA, lda, d_b, ldb, nrhs));
         TRY(wave_prepare(c, st, rank));
         TRY(backsolve_local(c, st, 0, rank, dA, lda, d_alpha, d_b, ldb, nrhs, c->xbuf, rank));
     }
-    for (int r0 = 0; r0 < nrhs; r0 += 65535) {
-        const int nr = std::min(nrhs - r0, 65535);
-        TRY(launch(c, st, "k_qrcp_scatter", 0.0, [&](CwtSlot) {
-            k_qrcp_scatter<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(c->xbuf + (size_t)r0 * rank, rank, d_jpvt, n,
-                                                                                         rank, d_b + (size_t)r0 * ldb, ldb);
-        }));
+    return qrcp_scatter(c, st, n, rank, c->xbuf, rank, d_jpvt, d_b, ldb, nrhs);
+}
+
+// ---- complete orthogonal decomposition on the pivoted QR (DESIGN §2.8) -------------------------------------------------------
+// A P = Q R at rank r: R_r = R[0:r, 0:n] (r x n, upper trapezoidal), and its transpose factored by the unpivoted QR, R_r' = Z [U; 0],
+// gives A P ~ Q1 [U' 0] Z'.  The minimum-norm solution of the rank-r problem is x = P Z [U^{-T} (Q'b)[0:r]; 0], and the step after
+// Q'b is exactly the minimum-norm solution of R_r y = c that dhqr_solve_adj_f64 computes from the factorisation (F, gamma) of R_r'.
+static bool spans_overlap(const void* p, size_t pbytes, const void* q, size_t qbytes) {
+    const uintptr_t p0 = (uintptr_t)p, q0 = (uintptr_t)q;
+    return pbytes > 0 && qbytes > 0 && p0 < q0 + qbytes && q0 < p0 + pbytes;
+}
+
+// Arguments 1-10, which both entry points share but for the 7th: alpha (dhqr_cod_f64, factor = true) or jpvt (dhqr_solve_cod_f64)
+static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const void* seventh,
+                     const double* dF, int64_t ldf, const double* d_gamma, bool factor) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the complete orthogonal decomposition is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (factor && n > narrow_panel_max_rows(c))                        // R_r' has n rows and goes through the unpivoted path
+        return set_err(-3, "n = %lld exceeds the row limit of the unpivoted factorisation (%lld)", (long long)n,
+                       (long long)narrow_panel_max_rows(c));
+    if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
+    if (n > 0 && !dA) return set_err(-5, "null A");
+    TRY(check_qrcp_ptr(dA, -5, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
+    const char* name7 = factor ? "alpha" : "jpvt";
+    if (n > 0 && !seventh) return set_err(-7, "null %s", name7);
+    TRY(check_qrcp_ptr(seventh, -7, name7));
+    if (rank > 0 && !dF) return set_err(-8, "null F");
+    TRY(check_qrcp_ptr(dF, -8, "F"));
+    if (ldf < std::max<int64_t>(1, n)) return set_err(-9, "ldf < max(1,n)");
+    if (rank > 0 && !d_gamma) return set_err(-10, "null gamma");
+    TRY(check_qrcp_ptr(d_gamma, -10, "gamma"));
+    if (factor && rank > 0) {                                          // F and gamma are written: neither may overlap an input
+        const size_t abytes = ((size_t)(n - 1) * lda + m) * 8, alphabytes = (size_t)n * 8;
+        const size_t fbytes = ((size_t)(rank - 1) * ldf + n) * 8, gbytes = (size_t)rank * 8;
+        if (spans_overlap(dF, fbytes, dA, abytes) || spans_overlap(dF, fbytes, seventh, alphabytes))
+            return set_err(-8, "F overlaps A or alpha");
+        if (spans_overlap(d_gamma, gbytes, dA, abytes) || spans_overlap(d_gamma, gbytes, seventh, alphabytes) ||
+            spans_overlap(d_gamma, gbytes, dF, fbytes))
+            return set_err(-10, "gamma overlaps A, alpha or F");
     }
     return 0;
+}
+
+int dhqr_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha, double* dF,
+                 int64_t ldf, double* d_gamma, void* stream) {
+    TRY(check_cod(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, true));
+    if (n == 0 || rank == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(launch(c, st, "k_cod_pack", 8.0 * (double)n * rank, [&](CwtSlot) {
+        k_cod_pack<<<dim3((unsigned)((n + CP_TILE - 1) / CP_TILE), (unsigned)((rank + CP_TILE - 1) / CP_TILE)), dim3(CP_TILE, CP_ROWS), 0,
+                     st>>>(dA, lda, d_alpha, n, rank, dF, ldf);
+    }));
+    return qr_blocked(c, st, n, rank, 0, rank, dF, ldf, d_gamma, c->nb);   // what dhqr_qr_f64 runs for nb = 0
+}
+
+int dhqr_solve_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const int64_t* d_jpvt,
+                       const double* dF, int64_t ldf, const double* d_gamma, double* d_b, int64_t ldb, int nrhs, void* stream) {
+    TRY(check_cod(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, false));
+    if (nrhs > 0 && !d_b) return set_err(-11, "null b");
+    TRY(check_qrcp_ptr(d_b, -11, "b"));
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-12, "ldb < max(1,m)");
+    if (nrhs < 0) return set_err(-13, "nrhs < 0");
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
+    TRY(c->xbuf.ensure((size_t)n * nrhs, st));
+    if (rank > 0) {
+        TRY(qrcp_qtb(c, st, m, rank, dA, lda, d_b, ldb, nrhs));
+        // b[0:n] <- Z [U^{-T} b[0:rank]; 0], rows n..m-1 untouched; then into xbuf, which the scatter reads while it writes b
+        TRY(solve_adj_local(c, st, n, rank, dF, ldf, d_gamma, d_b, ldb, nrhs));
+        CU(cudaMemcpy2DAsync(c->xbuf, (size_t)n * 8, d_b, (size_t)ldb * 8, (size_t)n * 8, nrhs, cudaMemcpyDeviceToDevice, st));
+    }
+    return qrcp_scatter(c, st, n, rank > 0 ? n : 0, c->xbuf, n, d_jpvt, d_b, ldb, nrhs);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

@@ -314,4 +314,30 @@ __global__ void k_qrcp_scatter(const double* __restrict__ z, int64_t ldz, const 
     b[d + (int64_t)blockIdx.y * ldb] = i < rank ? z[i + (int64_t)blockIdx.y * ldz] : 0.0;
 }
 
+// Complete orthogonal decomposition (dhqr_cod_f64): F (n x rank) <- R_r', R_r = rows [0, rank) of R = triu(A, 1) + diag(alpha), so
+// F[j, i] = A[i, j] for j > i, alpha[i] for j = i and 0 for j < i.  One CTA per 32 x 32 tile of F: the strip of A it needs is
+// read along A's columns (coalesced), transposed through shared memory and written along F's columns.  A tile that lies wholly
+// above F's diagonal is zero and reads nothing; the strict lower triangle of A (the reflectors) is never read.
+constexpr int CP_TILE = 32, CP_ROWS = 8;
+__global__ void __launch_bounds__(CP_TILE * CP_ROWS) k_cod_pack(const double* __restrict__ A, int64_t lda, const double* __restrict__ alpha,
+                                                                int64_t n, int64_t rank, double* __restrict__ F, int64_t ldf) {
+    __shared__ double t[CP_TILE][CP_TILE + 1];                         // t[j - j0][i - i0]
+    const int64_t j0 = (int64_t)blockIdx.x * CP_TILE, i0 = (int64_t)blockIdx.y * CP_TILE;
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const bool lower = j0 + CP_TILE - 1 >= i0;                         // the tile holds some j >= i
+    if (lower) {
+        for (int r = ty; r < CP_TILE; r += CP_ROWS) {
+            const int64_t j = j0 + r, i = i0 + tx;                     // row i of column j of A
+            double v = 0.0;
+            if (j < n && i < rank) v = j > i ? A[i + j * lda] : (j == i ? alpha[i] : 0.0);
+            t[r][tx] = v;
+        }
+        __syncthreads();
+    }
+    for (int r = ty; r < CP_TILE; r += CP_ROWS) {
+        const int64_t i = i0 + r, j = j0 + tx;                         // row j of column i of F
+        if (i < rank && j < n) F[j + i * ldf] = lower ? t[tx][r] : 0.0;
+    }
+}
+
 }  // namespace dhqr

@@ -244,4 +244,36 @@ function LinearAlgebra.ldiv!(x::AbstractVector, H::PivotedHouseholderQRStruct, b
 end
 LinearAlgebra.:(\)(H::PivotedHouseholderQRStruct, b::AbstractVector) = ldiv!(Vector{Float64}(undef, size(H.A, 2)), H, b)
 
+# ---- complete orthogonal decomposition on the pivoted QR (DESIGN §2.8), Float64, single GPU ----
+# A P ~ Q1 [U' 0] Z' at r = rank(H; rtol): (F, γ) is the factorisation R_r' = Z [U; 0] in the storage format above.  Its \ is the
+# minimum-norm solution, the answer the stdlib's qr(A, ColumnNorm()) \ b gives (up to how the rank is picked); \ on the pivoted
+# struct itself stays the basic solution.
+struct CompleteOrthogonalStruct{T1, T2, T3}
+    qrcp::T1
+    F::T2
+    γ::T3
+    rank::Int
+end
+function complete_orthogonal(H::PivotedHouseholderQRStruct; rtol::Real = max(size(H.A)...) * eps(Float64))
+    A = H.A; m, n = size(A)
+    r = rank(H; rtol)
+    F = CUDA.zeros(Float64, n, r); γ = CUDA.zeros(Float64, r)
+    GC.@preserve A F γ check(:dhqr_cod_f64, ccall((:dhqr_cod_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, CuPtr{Float64}, Ptr{Cvoid}),
+        handle().ptr, m, n, r, pointer(A), stride(A, 2), pointer(H.α), pointer(F), max(n, 1), pointer(γ), stream_ptr()))
+    return CompleteOrthogonalStruct(H, F, γ, r)
+end
+function LinearAlgebra.ldiv!(x::AbstractVector, C::CompleteOrthogonalStruct, b::AbstractVector)
+    A = C.qrcp.A; m, n = size(A)
+    s = CuVector{Float64}(b)
+    GC.@preserve A s check(:dhqr_solve_cod_f64, ccall((:dhqr_solve_cod_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Int64}, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64,
+         Cint, Ptr{Cvoid}),
+        handle().ptr, m, n, C.rank, pointer(A), stride(A, 2), pointer(C.qrcp.jpvt), pointer(C.F), max(n, 1), pointer(C.γ), pointer(s), m,
+        1, stream_ptr()))
+    copyto!(x, Array(s[1:n]))
+    return x
+end
+LinearAlgebra.:(\)(C::CompleteOrthogonalStruct, b::AbstractVector) = ldiv!(Vector{Float64}(undef, size(C.qrcp.A, 2)), C, b)
+
 end # module

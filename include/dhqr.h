@@ -22,7 +22,7 @@
  *     until their result is in host memory; (ii) dhqr_qr_f64 with the default blocked path synchronises
  *     the stream ONCE before returning whenever a panel went through the speculative 128-column chain
  *     (option "wide_panel", on by default: its conditioning guards are evaluated on the device and a
- *     refused panel is redone by the 32-column chain); (iii) with nranks > 1 every qr / apply_qt /
+ *     refused panel is redone by the 32-column chain), and so does dhqr_cod_f64, which factors R_r' on that path; (iii) with nranks > 1 every qr / apply_qt /
  *     backsolve call exchanges the column partition first (one small all-gather + stream sync);
  *     (iv) workspace growth (first call, or a larger problem than any before) allocates device memory.
  *     Everything else returns without synchronising.  Any caller stream works, non-blocking and prioritised ones
@@ -234,6 +234,29 @@ int dhqr_qrcp_f64(dhqr_handle h, int64_t m, int64_t n, double *dA, int64_t lda, 
  * misaligned b, -10 ldb < max(1, m), -11 nrhs < 0.  n = 0 or nrhs = 0 is a no-op. */
 int dhqr_solve_qrcp_f64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const double *dA, int64_t lda, const double *d_alpha,
                         const int64_t *d_jpvt, double *d_b, int64_t ldb, int nrhs, void *stream);
+
+/* ---- complete orthogonal decomposition on the pivoted QR (not in the reference; LAPACK dgelsy's minimum-norm solution) --------
+ * From A P = Q R (dhqr_qrcp_f64) at rank r: R_r = rows [0, r) of R = triu(A, 1) + diag(alpha), an r x n upper trapezoid, and the
+ * unpivoted QR of its transpose, R_r' = Z [U; 0], give A P ~ Q1 [U' 0] Z' (DESIGN §2.8).  Float64, single GPU (a handle with
+ * nranks > 1 returns -1), stream-ordered.  Every pointer must be 8 B aligned; every check runs before anything is enqueued.
+ *
+ * dhqr_cod_f64: F (n x rank, ldf >= max(1, n)) <- the factorisation of R_r' = Z [U; 0] in the library's storage format, gamma (rank)
+ * <- diag(U).  A and alpha are read, never written; nothing outside F's n x rank block and gamma is written.  The factorisation is
+ * the one dhqr_qr_f64 runs for nb = 0 on F, with the handle's options, so it synchronises the stream once when a 128-column panel of
+ * R_r' went through the speculative wide chain (point (ii)).  n = 0 or rank = 0 is a no-op.  Errors: -1 null or multi-rank handle,
+ * -2 m < 0, -3 n < 0 or n > m, or n above the row limit of the blocked unpivoted path (R_r' has n rows), -4 rank < 0 or rank > n,
+ * -5 null or misaligned A, -6 lda < max(1, m), -7 null or misaligned alpha, -8 F null (rank > 0), misaligned, or overlapping A's
+ * m x n block or alpha, -9 ldf < max(1, n), -10 gamma null (rank > 0), misaligned, or overlapping A, alpha or F. */
+int dhqr_cod_f64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const double *dA, int64_t lda, const double *d_alpha,
+                 double *dF, int64_t ldf, double *d_gamma, void *stream);
+/* x = P Z [U^{-T} (Q'b)[0:rank]; 0]: the minimum-norm solution of the rank-`rank` problem min ||Q1 R_r P' x - b||, from
+ * dhqr_qrcp_f64's (A, jpvt) and dhqr_cod_f64's (F, gamma) at the same rank.  d_b: m x nrhs, ldb >= max(1, m), in place: on return
+ * b[0:n] = x, and rows n..m-1 hold rows n..m-1 of H_rank ... H_1 b, as in dhqr_solve_qrcp_f64.  rank = 0 gives x = 0.  jpvt
+ * entries outside [0, n) are skipped.  No synchronisation apart from workspace growth (point (iv)).  Errors: -1 to -6 as above,
+ * -7 null or misaligned jpvt, -8 F null (rank > 0) or misaligned, -9 ldf < max(1, n), -10 gamma null (rank > 0) or misaligned,
+ * -11 null or misaligned b, -12 ldb < max(1, m), -13 nrhs < 0.  n = 0 or nrhs = 0 is a no-op. */
+int dhqr_solve_cod_f64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const double *dA, int64_t lda, const int64_t *d_jpvt,
+                       const double *dF, int64_t ldf, const double *d_gamma, double *d_b, int64_t ldb, int nrhs, void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
