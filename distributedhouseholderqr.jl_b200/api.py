@@ -511,6 +511,18 @@ def ldiv(H: DistributedHouseholderQRStruct, b):
 # QR with column pivoting (LAPACK dgeqp3) and the basic least-squares solution (dgelsy without the complete orthogonal
 # decomposition); scipy.linalg.qr(pivoting=True) / Julia's qr(A, ColumnNorm())
 # --------------------------------------------------------------------------------------------
+def _rhs_copy(b, A: torch.Tensor) -> torch.Tensor:
+    """A fresh copy of ``b`` (length m, or (m, k)) on A's device for the pivoted solves: a vector takes A's dtype, a block is made
+    column-major, and a real block is promoted to complex128 for a ComplexF64 factorisation."""
+    if b.dim() == 1:
+        return b.to(device=A.device, dtype=A.dtype).clone()
+    if A.is_complex():
+        out = colmajor_empty(b.shape[0], b.shape[1], A.device, dtype=A.dtype)
+        out.copy_(torch.as_tensor(b))
+        return out
+    return to_colmajor(b, device=A.device)
+
+
 class PivotedHouseholderQRStruct:
     """A P = Q R from ``qrcp_``: ``.A`` (the caller's storage, factored in place) and ``.α`` (``.alpha``) are the factorisation of
     ``A[:, p]`` in the library's storage format, so every other entry point (apply_qt_, apply_q_, backsolve_, form_q,
@@ -543,10 +555,7 @@ class PivotedHouseholderQRStruct:
         b is modified.  ``b``: length m, or (m, k)."""
         r = self.rank(rcond)
         loc = self.A
-        if b.dim() == 1:
-            s = b.to(device=loc.device, dtype=loc.dtype).clone()
-        else:
-            s = to_colmajor(b, device=loc.device)
+        s = _rhs_copy(b, loc)
         solve_qrcp_(s, self.A, self.α, self.p, r, self.handle)
         return s[:loc.shape[1]].clone(), r
 
@@ -580,10 +589,7 @@ class CompleteOrthogonalStruct:
         """The minimum-norm solution x of min ||A x - b|| at rank ``self.rank``; neither the factorisations nor b is modified.
         ``b``: length m, or (m, k).  Returns a new length-n vector or (n, k) tensor."""
         A = self.qrcp.A
-        if b.dim() == 1:
-            s = b.to(device=A.device, dtype=A.dtype).clone()
-        else:
-            s = to_colmajor(b, device=A.device)
+        s = _rhs_copy(b, A)
         solve_cod_(s, A, self.qrcp.p, self.F, self.γ, self.rank, self.qrcp.handle)
         return s[:A.shape[1]].clone()
 
@@ -591,54 +597,57 @@ class CompleteOrthogonalStruct:
 
 
 def qrcp_(A: torch.Tensor, handle: Optional[Handle] = None) -> PivotedHouseholderQRStruct:
-    """A P = Q R with column pivoting (LAPACK dgeqp3; scipy.linalg.qr(pivoting=True)), in place, on a column-major float64 CUDA
-    tensor with n <= m.  Single GPU, stream-ordered, no synchronisation."""
+    """A P = Q R with column pivoting (LAPACK dgeqp3 / zgeqp3; scipy.linalg.qr(pivoting=True)), in place, on a column-major float64
+    or complex128 CUDA tensor with n <= m (alpha has A's dtype).  Single GPU, stream-ordered, no synchronisation."""
     if not isinstance(A, torch.Tensor) or not A.is_cuda:
-        raise TypeError("qrcp_ works on a column-major float64 CUDA tensor")
-    if A.dtype != torch.float64:
-        raise TypeError("qrcp_ is Float64 only")
+        raise TypeError("qrcp_ works on a column-major float64 or complex128 CUDA tensor")
+    if A.dtype not in (torch.float64, torch.complex128):
+        raise TypeError("qrcp_ takes Float64 or ComplexF64 (float64 / complex128) only")
     h = handle or default_handle(A.device.index)
     m, n = A.shape
-    alpha = torch.zeros(n, dtype=torch.float64, device=A.device)
+    alpha = torch.zeros(n, dtype=A.dtype, device=A.device)
     p = torch.zeros(n, dtype=torch.int64, device=A.device)
     with torch.cuda.device(A.device):
-        _lib.call("dhqr_qrcp_f64", h.raw, m, n, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+        _lib.call("dhqr_qrcp_" + _sfx(A), h.raw, m, n, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
                   C.c_void_p(p.data_ptr()), _stream_ptr(A.device))
     return PivotedHouseholderQRStruct(A, alpha, p, h)
 
 
 def solve_qrcp_(b: torch.Tensor, A: torch.Tensor, alpha: torch.Tensor, p: torch.Tensor, rank: int,
                 handle: Optional[Handle] = None) -> torch.Tensor:
-    """x = P [R11^{-1} (Q'b)[0:rank]; 0], the basic solution at the given rank, from a factorisation made by ``qrcp_``.  ``b``:
+    """x = P [R11^{-1} (Q^H b)[0:rank]; 0], the basic solution at the given rank, from a factorisation made by ``qrcp_`` (Float64
+    or ComplexF64).  ``b``:
     length m, or (m, k) column-major; on return b[0:n] = x (returned as a view) and rows n..m-1 hold rows n..m-1 of
     H_rank ... H_1 b."""
     h = handle or default_handle(A.device.index)
     m, n = A.shape
-    if alpha.dtype != torch.float64 or p.dtype != torch.int64:
-        raise TypeError("alpha must be float64 and p int64")
+    sfx = _sfx(A)
+    if alpha.dtype != A.dtype or p.dtype != torch.int64:
+        raise TypeError("alpha must have the element type of A and p must be int64")
     ldb, nrhs = _rhs_args(b, m, A.dtype)
     with torch.cuda.device(A.device):
-        _lib.call("dhqr_solve_qrcp_f64", h.raw, m, n, int(rank), C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+        _lib.call("dhqr_solve_qrcp_" + sfx, h.raw, m, n, int(rank), C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
                   C.c_void_p(p.data_ptr()), C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(A.device))
     return b[:n]
 
 
 def cod_(A: torch.Tensor, alpha: torch.Tensor, rank: int, handle: Optional[Handle] = None):
     """The second factorisation of the complete orthogonal decomposition at the given rank, from a factorisation made by
-    ``qrcp_``: R_r' = Z [U; 0] with R_r = rows [0, rank) of R = triu(A, 1) + diag(alpha).  Returns (F, γ): F a fresh (n, rank)
-    column-major tensor in the library's storage format, γ = diag(U).  A and alpha are read, never written.  Synchronises the
-    stream once when a 128-column panel of R_r' went through the wide chain, as qr_ does."""
-    if not isinstance(A, torch.Tensor) or not A.is_cuda or A.dtype != torch.float64:
-        raise TypeError("cod_ works on a column-major float64 CUDA tensor")
-    if alpha.dtype != torch.float64:
-        raise TypeError("alpha must be float64")
+    ``qrcp_``: R_r^H = Z [U; 0] with R_r = rows [0, rank) of R = triu(A, 1) + diag(alpha).  Returns (F, γ): F a fresh (n, rank)
+    column-major tensor of A's dtype in the library's storage format, γ = diag(U).  A and alpha are read, never written.  Float64:
+    synchronises the stream once when a 128-column panel of R_r' went through the wide chain, as qr_ does; ComplexF64 never
+    synchronises."""
+    if not isinstance(A, torch.Tensor) or not A.is_cuda or A.dtype not in (torch.float64, torch.complex128):
+        raise TypeError("cod_ works on a column-major float64 or complex128 CUDA tensor")
+    if alpha.dtype != A.dtype:
+        raise TypeError("alpha must have the element type of A")
     h = handle or default_handle(A.device.index)
     m, n = A.shape
     rank = int(rank)
-    F = colmajor_empty(n, max(rank, 0), A.device)
-    gamma = torch.zeros(max(rank, 0), dtype=torch.float64, device=A.device)
+    F = colmajor_empty(n, max(rank, 0), A.device, dtype=A.dtype)
+    gamma = torch.zeros(max(rank, 0), dtype=A.dtype, device=A.device)
     with torch.cuda.device(A.device):
-        _lib.call("dhqr_cod_f64", h.raw, m, n, rank, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+        _lib.call("dhqr_cod_" + _sfx(A), h.raw, m, n, rank, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
                   C.c_void_p(F.data_ptr() if rank > 0 else None), max(n, 1), C.c_void_p(gamma.data_ptr() if rank > 0 else None),
                   _stream_ptr(A.device))
     return F, gamma
@@ -646,19 +655,20 @@ def cod_(A: torch.Tensor, alpha: torch.Tensor, rank: int, handle: Optional[Handl
 
 def solve_cod_(b: torch.Tensor, A: torch.Tensor, p: torch.Tensor, F: torch.Tensor, gamma: torch.Tensor, rank: int,
                handle: Optional[Handle] = None) -> torch.Tensor:
-    """x = P Z [U^{-T} (Q'b)[0:rank]; 0], the minimum-norm solution at the given rank, from ``qrcp_``'s (A, p) and ``cod_``'s
-    (F, γ) at that rank.  ``b``: length m, or (m, k) column-major; on return b[0:n] = x (returned as a view) and rows n..m-1
+    """x = P Z [U^{-H} (Q^H b)[0:rank]; 0], the minimum-norm solution at the given rank, from ``qrcp_``'s (A, p) and ``cod_``'s
+    (F, γ) at that rank (Float64 or ComplexF64).  ``b``: length m, or (m, k) column-major; on return b[0:n] = x (returned as a view) and rows n..m-1
     hold rows n..m-1 of H_rank ... H_1 b, as in solve_qrcp_."""
     h = handle or default_handle(A.device.index)
     m, n = A.shape
-    if p.dtype != torch.int64 or F.dtype != torch.float64 or gamma.dtype != torch.float64:
-        raise TypeError("p must be int64, F and gamma float64")
+    sfx = _sfx(A)
+    if p.dtype != torch.int64 or F.dtype != A.dtype or gamma.dtype != A.dtype:
+        raise TypeError("p must be int64, F and gamma of the element type of A")
     rank = int(rank)
     if rank > 0 and (tuple(F.shape) != (n, rank) or tuple(gamma.shape) != (rank,)):
         raise ValueError(f"F must be ({n}, {rank}) and gamma ({rank},)")
     ldb, nrhs = _rhs_args(b, m, A.dtype)
     with torch.cuda.device(A.device):
-        _lib.call("dhqr_solve_cod_f64", h.raw, m, n, rank, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(p.data_ptr()),
+        _lib.call("dhqr_solve_cod_" + sfx, h.raw, m, n, rank, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(p.data_ptr()),
                   C.c_void_p(F.data_ptr() if rank > 0 else None), _lda(F) if rank > 0 else max(n, 1),
                   C.c_void_p(gamma.data_ptr() if rank > 0 else None), C.c_void_p(b.data_ptr()), ldb, nrhs, _stream_ptr(A.device))
     return b[:n]

@@ -21,6 +21,7 @@
 #include "dhqr_wide.cuh"
 #include "dhqr_complex.cuh"
 #include "dhqr_qrcp.cuh"
+#include "dhqr_qrcp_c.cuh"
 
 using namespace dhqr;
 
@@ -1954,6 +1955,8 @@ static int pack_complex_panel(dhqr_context* c, cudaStream_t st, const double2* P
     return launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) { k_pack_c<<<grid, 256, 0, st>>>(P, lda, mpc, kb, c->vpk2[0], 0, vrows); });
 }
 
+static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double2* A, int64_t lda, double2* alpha);
+
 int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, void* dA, int64_t lda, void* d_alpha,
                 void* stream) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
@@ -1962,11 +1965,12 @@ int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
     TRY(check_c64_ptr(d_alpha, -8, "alpha"));
     if (n_global == 0) return 0;
     CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    const int64_t n = n_global;
+    return qr_c64_local(c, (cudaStream_t)stream, m, n_global, (double2*)dA, lda, (double2*)d_alpha);
+}
+
+// the body of dhqr_qr_c64 (n > 0), also the second factorisation of dhqr_cod_c64
+static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double2* A, int64_t lda, double2* alpha) {
     TRY(ensure_workspace(c, st, 2 * m, n));
-    double2* A = (double2*)dA;
-    double2* alpha = (double2*)d_alpha;
     for (int64_t c0 = 0; c0 < n; c0 += CPW) {
         const int kb = (int)std::min<int64_t>(CPW, n - c0);
         double2* P = A + c0 * lda + c0;
@@ -1990,6 +1994,9 @@ int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_
     return 0;
 }
 
+static int apply_qt_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b,
+                              int64_t ldb, int nrhs);
+
 int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                       void* d_b, int64_t ldb, int nrhs, void* stream) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
@@ -2000,15 +2007,31 @@ int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
     if (ldb < std::max<int64_t>(1, m)) return set_err(-9, "ldb < max(1,m)");
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n_global, nrhs)));
-    const double2* A = (const double2*)dA;
-    double2* b = (double2*)d_b;
-    for (int64_t c0 = 0; c0 < n_global; c0 += CPW) {         // S:232-242, panel by panel
-        const int kb = (int)std::min<int64_t>(CPW, n_global - c0);
+    return apply_qt_c64_local(c, (cudaStream_t)stream, m, n_global, (const double2*)dA, lda, (double2*)d_b, ldb, nrhs);
+}
+
+// the body of dhqr_apply_qt_c64 (n > 0, nrhs > 0), also the (Q^H b)[0:rank] stage of the complex pivoted solves
+static int apply_qt_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b,
+                              int64_t ldb, int nrhs) {
+    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
+    for (int64_t c0 = 0; c0 < n; c0 += CPW) {                // S:232-242, panel by panel
+        const int kb = (int)std::min<int64_t>(CPW, n - c0);
         const int64_t mpc = m - c0, rows = 2 * mpc, vrows = rup(rows, 128);
         TRY(pack_complex_panel(c, st, A + c0 * lda + c0, lda, mpc, kb, vrows));
         TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, (double*)(b + c0), 2 * ldb, nrhs));
+    }
+    return 0;
+}
+
+// x (n x nrhs, ldx) <- R^{-1} b[0:n] for complex R = triu(A, 1) + diag(alpha); b[0:n] is overwritten on the way
+static int backsolve_c64_local(dhqr_context* c, cudaStream_t st, int64_t n, const double2* A, int64_t lda, const double2* alpha, double2* b,
+                               int64_t ldb, int nrhs, double2* x, int64_t ldx) {
+    for (int64_t o = ((n - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {     // S:260: i = n:-1:1, by blocks
+        const int bs = (int)std::min<int64_t>(BS_BLK, n - o);
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((o + 255) / 256, 2 * c->sms));
+        TRY(launch(c, st, "k_backsolve_step_c", 0.0, [&](CwtSlot) {
+            k_backsolve_step_c<<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, b, ldb, nrhs, x, ldx, o, bs);
+        }));
     }
     return 0;
 }
@@ -2021,15 +2044,8 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t n = n_global;
     TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
-    const double2* A = (const double2*)dA;
     double2* x = (double2*)c->xbuf.p;
-    for (int64_t o = ((n - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {     // S:260: i = n:-1:1, by blocks
-        const int bs = (int)std::min<int64_t>(BS_BLK, n - o);
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((o + 255) / 256, 2 * c->sms));
-        TRY(launch(c, st, "k_backsolve_step_c", 0.0, [&](CwtSlot) {
-            k_backsolve_step_c<<<grid, 256, 0, st>>>(A + o * lda, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs, x, n, o, bs);
-        }));
-    }
+    TRY(backsolve_c64_local(c, st, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs, x, n));
     CU(cudaMemcpy2DAsync(d_b, (size_t)ldb * 16, x, (size_t)n * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
     return 0;
 }
@@ -2221,18 +2237,21 @@ int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, in
     return solve_adj_local(c, (cudaStream_t)stream, m, n, dA, lda, d_alpha, d_b, ldb, nrhs);
 }
 
+// y = Q [R^{-H} c; 0] in place on complex b[0:m]: the body of dhqr_solve_adj_c64, also the second stage of dhqr_solve_cod_c64
+static int solve_adj_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, const double2* alpha,
+                               double2* b, int64_t ldb, int nrhs) {
+    if (n > 0) TRY(forwardsolve_c64_local(c, st, n, A, lda, alpha, b, ldb, nrhs));
+    if (m > n) CU(cudaMemset2DAsync(b + n, (size_t)ldb * 16, 0, (size_t)(m - n) * 16, nrhs, st));
+    if (n == 0) return 0;
+    return apply_q_c64_local(c, st, m, n, A, lda, b, ldb, nrhs);
+}
+
 int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
                        int nrhs, void* stream) {
     TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, true));
     if (m == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    const double2* A = (const double2*)dA;
-    double2* b = (double2*)d_b;
-    if (n > 0) TRY(forwardsolve_c64_local(c, st, n, A, lda, (const double2*)d_alpha, b, ldb, nrhs));
-    if (m > n) CU(cudaMemset2DAsync(b + n, (size_t)ldb * 16, 0, (size_t)(m - n) * 16, nrhs, st));
-    if (n == 0) return 0;
-    return apply_q_c64_local(c, st, m, n, A, lda, b, ldb, nrhs);
+    return solve_adj_c64_local(c, (cudaStream_t)stream, m, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs);
 }
 
 // ---- QR with column pivoting (LAPACK dgeqp3 / dlaqps, dhqr_qrcp.cuh) -------------------------------------------------------
@@ -2380,31 +2399,34 @@ static bool spans_overlap(const void* p, size_t pbytes, const void* q, size_t qb
     return pbytes > 0 && qbytes > 0 && p0 < q0 + qbytes && q0 < p0 + pbytes;
 }
 
-// Arguments 1-10, which both entry points share but for the 7th: alpha (dhqr_cod_f64, factor = true) or jpvt (dhqr_solve_cod_f64)
-static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const void* seventh,
-                     const double* dF, int64_t ldf, const double* d_gamma, bool factor) {
+// Arguments 1-10, which both entry points share but for the 7th: alpha (dhqr_cod_*, factor = true) or jpvt (dhqr_solve_cod_*).
+// cplx: the _c64 twins, whose A, alpha, F and gamma are ComplexF64 (16 B aligned, 16 B elements) and have no row limit.
+static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* seventh,
+                     const void* dF, int64_t ldf, const void* d_gamma, bool factor, bool cplx = false) {
+    auto check_ptr = [cplx](const void* p, int arg, const char* name) { return cplx ? check_c64_ptr(p, arg, name) : check_qrcp_ptr(p, arg, name); };
+    const size_t esz = cplx ? 16 : 8;
     if (!c) return set_err(-1, "null handle");
     if (c->nranks != 1) return set_err(-1, "the complete orthogonal decomposition is single-GPU (the handle has %d ranks)", c->nranks);
     if (m < 0) return set_err(-2, "m < 0");
     if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (factor && n > narrow_panel_max_rows(c))                        // R_r' has n rows and goes through the unpivoted path
+    if (factor && !cplx && n > narrow_panel_max_rows(c))               // R_r' has n rows and goes through the unpivoted path
         return set_err(-3, "n = %lld exceeds the row limit of the unpivoted factorisation (%lld)", (long long)n,
                        (long long)narrow_panel_max_rows(c));
     if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
     if (n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_qrcp_ptr(dA, -5, "A"));
+    TRY(check_ptr(dA, -5, "A"));
     if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
     const char* name7 = factor ? "alpha" : "jpvt";
     if (n > 0 && !seventh) return set_err(-7, "null %s", name7);
-    TRY(check_qrcp_ptr(seventh, -7, name7));
+    TRY(factor ? check_ptr(seventh, -7, name7) : check_qrcp_ptr(seventh, -7, name7));
     if (rank > 0 && !dF) return set_err(-8, "null F");
-    TRY(check_qrcp_ptr(dF, -8, "F"));
+    TRY(check_ptr(dF, -8, "F"));
     if (ldf < std::max<int64_t>(1, n)) return set_err(-9, "ldf < max(1,n)");
     if (rank > 0 && !d_gamma) return set_err(-10, "null gamma");
-    TRY(check_qrcp_ptr(d_gamma, -10, "gamma"));
+    TRY(check_ptr(d_gamma, -10, "gamma"));
     if (factor && rank > 0) {                                          // F and gamma are written: neither may overlap an input
-        const size_t abytes = ((size_t)(n - 1) * lda + m) * 8, alphabytes = (size_t)n * 8;
-        const size_t fbytes = ((size_t)(rank - 1) * ldf + n) * 8, gbytes = (size_t)rank * 8;
+        const size_t abytes = ((size_t)(n - 1) * lda + m) * esz, alphabytes = (size_t)n * esz;
+        const size_t fbytes = ((size_t)(rank - 1) * ldf + n) * esz, gbytes = (size_t)rank * esz;
         if (spans_overlap(dF, fbytes, dA, abytes) || spans_overlap(dF, fbytes, seventh, alphabytes))
             return set_err(-8, "F overlaps A or alpha");
         if (spans_overlap(d_gamma, gbytes, dA, abytes) || spans_overlap(d_gamma, gbytes, seventh, alphabytes) ||
@@ -2446,6 +2468,168 @@ int dhqr_solve_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const 
         CU(cudaMemcpy2DAsync(c->xbuf, (size_t)n * 8, d_b, (size_t)ldb * 8, (size_t)n * 8, nrhs, cudaMemcpyDeviceToDevice, st));
     }
     return qrcp_scatter(c, st, n, rank > 0 ? n : 0, c->xbuf, n, d_jpvt, d_b, ldb, nrhs);
+}
+
+// ---- ComplexF64 QR with column pivoting and the complete orthogonal decomposition on it (DESIGN §2.9, dhqr_qrcp_c.cuh) ---------
+// The scheme of dhqr_qrcp_f64 in complex arithmetic, in the library's complex storage format; the trailing update after each panel is
+// the real C += V^ Y^ on the real view through the 128-instantiation (64 real vectors: two k-chunks).  Single GPU, n <= m, no row
+// limit, no synchronisation.
+static int qrcp_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double2* A, int64_t lda, double2* alpha, int64_t* jpvt) {
+    TRY(ensure_workspace(c, st, 2 * m, n));
+    const int64_t p1 = (m + QP_PROWS - 1) / QP_PROWS;                                    // k_qrcp_pivot_c CTAs
+    const int64_t smax = std::max<int64_t>(1, std::min<int64_t>((m + QP_THREADS - 1) / QP_THREADS, 8 * c->sms));
+    // in doubles: vn1, vn2 (real); F, x, the pivot partials (real, padded to keep what follows 16 B aligned) and the GEMV partials
+    const size_t need = (size_t)2 * n + (size_t)2 * QP_NB * n + (size_t)2 * m + (size_t)rup(p1, 2) + (size_t)2 * smax * n;
+    TRY(c->qp_buf.ensure(need, st));
+    TRY(c->qp_flag.ensure((size_t)n, st));
+    TRY(c->qp_ctl.ensure(1, st));
+    QrcpArgsC a;
+    a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
+    a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = (double2*)(a.vn2 + n); a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
+    a.part1 = (double*)(a.x + m); a.part2 = (double2*)(a.part1 + rup(p1, 2)); a.ldp = n;
+    TRY(launch(c, st, "k_qrcp_init_c", 16.0 * (double)m * n, [&](CwtSlot) {
+        k_qrcp_init_c<<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
+    }));
+    for (int64_t k0 = 0; k0 < n; k0 += QP_NB) {
+        const int kb = (int)std::min<int64_t>(QP_NB, n - k0);
+        const int tiles = (int)((n - k0 + QPC_GCOLS - 1) / QPC_GCOLS);
+        for (int jj = 0; jj < kb; ++jj) {
+            const int64_t j = k0 + jj, rows = m - j;
+            a.j = j; a.k0 = k0; a.jj = jj;
+            TRY(launch(c, st, "k_qrcp_pivot_c", 16.0 * ((double)m * 2 + (double)rows * (jj + 1)) + 8.0 * (double)(n - j), [&](CwtSlot) {
+                k_qrcp_pivot_c<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
+            }));
+            // row splits: about eight CTAs per SM in all, at least QP_THREADS rows each
+            const int64_t s = std::max<int64_t>(1, std::min<int64_t>((rows + QP_THREADS - 1) / QP_THREADS,
+                                                                     (8 * (int64_t)c->sms + tiles - 1) / tiles));
+            a.split_rows = rup((rows + s - 1) / s, QP_THREADS);
+            a.nsplit = (int)((rows + a.split_rows - 1) / a.split_rows);
+            TRY(launch(c, st, "k_qrcp_gemv_c", 16.0 * (double)rows * (double)(n - k0), [&](CwtSlot) {
+                k_qrcp_gemv_c<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
+            }));
+            if (j + 1 >= n) continue;
+            TRY(launch(c, st, "k_qrcp_finish_c", 0.0, [&](CwtSlot) {
+                k_qrcp_finish_c<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
+            }));
+            TRY(launch(c, st, "k_qrcp_renorm_c", 0.0, [&](CwtSlot) {
+                k_qrcp_renorm_c<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
+            }));
+        }
+        const int64_t c1 = k0 + kb;
+        if (c1 >= n) break;
+        // A[c1:, c1:] -= V F^H on the real view of the window starting at complex row k0, real rows >= 2 kb only
+        const int64_t mpc = m - k0, wrows = 2 * mpc, vrows = rup(wrows, 128);
+        const int ncols = (int)(n - c1);
+        TRY(launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) {
+            k_pack_c<<<dim3((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), 2 * QP_NB), 256, 0, st>>>(
+                A + k0 * lda + k0, lda, mpc, kb, c->vpk2[0], 0, vrows);
+        }));
+        const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * QPC_NKQ * YT * LDK;
+        TRY(launch(c, st, "k_qrcp_ypack_c", 0.0, [&](CwtSlot) {
+            k_qrcp_ypack_c<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(a.F, a.ldf, c1, ncols, kb, c->ws[0].ypk);
+        }));
+        TRY(launch_cvy(c, st, c->vpk2[0], 0, 2 * QP_NB, c->ws[0].ypk, wrows, 2 * kb, (double*)(A + c1 * lda + k0), 2 * lda, ncols, 0));
+    }
+    return 0;
+}
+
+int dhqr_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, void* dA, int64_t lda, void* d_alpha, int64_t* d_jpvt, void* stream) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the pivoted factorisation is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (n > 0 && !dA) return set_err(-4, "null A");
+    TRY(check_c64_ptr(dA, -4, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
+    if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
+    TRY(check_c64_ptr(d_alpha, -6, "alpha"));
+    if (n > 0 && !d_jpvt) return set_err(-7, "null jpvt");
+    TRY(check_qrcp_ptr(d_jpvt, -7, "jpvt"));
+    if (n == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return qrcp_c64_local(c, (cudaStream_t)stream, m, n, (double2*)dA, lda, (double2*)d_alpha, d_jpvt);
+}
+
+// complex twin of qrcp_scatter
+static int qrcp_scatter_c(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double2* z, int64_t ldz, const int64_t* d_jpvt,
+                          double2* d_b, int64_t ldb, int nrhs) {
+    for (int r0 = 0; r0 < nrhs; r0 += 65535) {
+        const int nr = std::min(nrhs - r0, 65535);
+        TRY(launch(c, st, "k_qrcp_scatter_c", 0.0, [&](CwtSlot) {
+            k_qrcp_scatter_c<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(z + (size_t)r0 * ldz, ldz, d_jpvt, n, rank,
+                                                                                           d_b + (size_t)r0 * ldb, ldb);
+        }));
+    }
+    return 0;
+}
+
+int dhqr_solve_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha,
+                        const int64_t* d_jpvt, void* d_b, int64_t ldb, int nrhs, void* stream) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the pivoted solve is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
+    if (n > 0 && !dA) return set_err(-5, "null A");
+    TRY(check_c64_ptr(dA, -5, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
+    if (n > 0 && !d_alpha) return set_err(-7, "null alpha");
+    TRY(check_c64_ptr(d_alpha, -7, "alpha"));
+    if (n > 0 && !d_jpvt) return set_err(-8, "null jpvt");
+    TRY(check_qrcp_ptr(d_jpvt, -8, "jpvt"));
+    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
+    TRY(check_c64_ptr(d_b, -9, "b"));
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
+    if (nrhs < 0) return set_err(-11, "nrhs < 0");
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
+    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
+    const double2* A = (const double2*)dA;
+    double2* b = (double2*)d_b;
+    double2* x = (double2*)c->xbuf.p;
+    if (rank > 0) {
+        TRY(apply_qt_c64_local(c, st, m, rank, A, lda, b, ldb, nrhs));
+        TRY(backsolve_c64_local(c, st, rank, A, lda, (const double2*)d_alpha, b, ldb, nrhs, x, rank));
+    }
+    return qrcp_scatter_c(c, st, n, rank, x, rank, d_jpvt, b, ldb, nrhs);
+}
+
+int dhqr_cod_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha, void* dF,
+                 int64_t ldf, void* d_gamma, void* stream) {
+    TRY(check_cod(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, true, true));
+    if (n == 0 || rank == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(launch(c, st, "k_cod_pack_c", 16.0 * (double)n * rank, [&](CwtSlot) {
+        k_cod_pack_c<<<dim3((unsigned)((n + CP_TILE - 1) / CP_TILE), (unsigned)((rank + CP_TILE - 1) / CP_TILE)), dim3(CP_TILE, CP_ROWS), 0,
+                       st>>>((const double2*)dA, lda, (const double2*)d_alpha, n, rank, (double2*)dF, ldf);
+    }));
+    return qr_c64_local(c, st, n, rank, (double2*)dF, ldf, (double2*)d_gamma);      // the body of dhqr_qr_c64
+}
+
+int dhqr_solve_cod_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const int64_t* d_jpvt,
+                       const void* dF, int64_t ldf, const void* d_gamma, void* d_b, int64_t ldb, int nrhs, void* stream) {
+    TRY(check_cod(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, false, true));
+    if (nrhs > 0 && !d_b) return set_err(-11, "null b");
+    TRY(check_c64_ptr(d_b, -11, "b"));
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-12, "ldb < max(1,m)");
+    if (nrhs < 0) return set_err(-13, "nrhs < 0");
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
+    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
+    double2* b = (double2*)d_b;
+    double2* x = (double2*)c->xbuf.p;
+    if (rank > 0) {
+        TRY(apply_qt_c64_local(c, st, m, rank, (const double2*)dA, lda, b, ldb, nrhs));
+        // b[0:n] <- Z [U^{-H} b[0:rank]; 0], rows n..m-1 untouched; then into xbuf, which the scatter reads while it writes b
+        TRY(solve_adj_c64_local(c, st, n, rank, (const double2*)dF, ldf, (const double2*)d_gamma, b, ldb, nrhs));
+        CU(cudaMemcpy2DAsync(x, (size_t)n * 16, b, (size_t)ldb * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
+    }
+    return qrcp_scatter_c(c, st, n, rank > 0 ? n : 0, x, n, d_jpvt, b, ldb, nrhs);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

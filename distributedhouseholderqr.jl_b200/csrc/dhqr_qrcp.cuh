@@ -32,6 +32,7 @@ struct QrcpCtl {
     unsigned int ticket;             // k_qrcp_pivot: zero on entry, zero again on exit
     unsigned int pad;
     unsigned long long renorms;      // exact renorms since the handle was created
+    double alpha_im;                 // dhqr_qrcp_c.cuh: imaginary part of the complex alpha in flight
 };
 
 struct QrcpArgs {

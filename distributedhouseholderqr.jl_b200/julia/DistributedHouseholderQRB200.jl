@@ -208,20 +208,12 @@ function LinearAlgebra.:(\)(Ha::AdjointQR, c::AbstractVecOrMat)
     return c isa AbstractVector ? vec(y) : y
 end
 
-# ---- QR with column pivoting (LAPACK dgeqp3; not in the reference), Float64, single GPU ----
+# ---- QR with column pivoting (LAPACK dgeqp3 / zgeqp3; not in the reference), Float64 and ComplexF64, single GPU ----
 # A[:, p] = Q R: (A, α) is the factorisation of A[:, p] in the storage format above; p is 1-based here, 0-based on the device
 struct PivotedHouseholderQRStruct{T1, T2, T3}
     A::T1
     α::T2
     jpvt::T3          # CuVector{Int64}, 0-based
-end
-function qr!(A::CuMatrix{Float64}, ::ColumnNorm)
-    m, n = size(A)
-    α = CUDA.zeros(Float64, n); jpvt = CUDA.zeros(Int64, n)
-    GC.@preserve A α jpvt check(:dhqr_qrcp_f64, ccall((:dhqr_qrcp_f64, libdhqr), Cint,
-        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Int64}, Ptr{Cvoid}),
-        handle().ptr, m, n, pointer(A), stride(A, 2), pointer(α), pointer(jpvt), stream_ptr()))
-    return PivotedHouseholderQRStruct(A, α, jpvt)
 end
 Base.getproperty(H::PivotedHouseholderQRStruct, s::Symbol) = s === :p ? Array(getfield(H, :jpvt)) .+ 1 : getfield(H, s)
 # numerical rank: the first k with |α_k| <= rtol |α_1| (reads α: synchronises)
@@ -231,21 +223,9 @@ function LinearAlgebra.rank(H::PivotedHouseholderQRStruct; rtol::Real = max(size
     k = findfirst(x -> !(x > rtol * a[1]), a)
     return k === nothing ? length(a) : k - 1
 end
-# H \ b: the basic solution x = P [R11^{-1} (Q'b)[1:r]; 0] at r = rank(H; rtol) (dhqr_solve_qrcp_f64); b is not modified
-function LinearAlgebra.ldiv!(x::AbstractVector, H::PivotedHouseholderQRStruct, b::AbstractVector; rtol::Real = max(size(H.A)...) * eps(Float64))
-    A = H.A; m, n = size(A)
-    r = rank(H; rtol)
-    s = CuVector{Float64}(b)
-    GC.@preserve A s check(:dhqr_solve_qrcp_f64, ccall((:dhqr_solve_qrcp_f64, libdhqr), Cint,
-        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Int64}, CuPtr{Float64}, Int64, Cint, Ptr{Cvoid}),
-        handle().ptr, m, n, r, pointer(A), stride(A, 2), pointer(H.α), pointer(H.jpvt), pointer(s), m, 1, stream_ptr()))
-    copyto!(x, Array(s[1:n]))
-    return x
-end
-LinearAlgebra.:(\)(H::PivotedHouseholderQRStruct, b::AbstractVector) = ldiv!(Vector{Float64}(undef, size(H.A, 2)), H, b)
 
-# ---- complete orthogonal decomposition on the pivoted QR (DESIGN §2.8), Float64, single GPU ----
-# A P ~ Q1 [U' 0] Z' at r = rank(H; rtol): (F, γ) is the factorisation R_r' = Z [U; 0] in the storage format above.  Its \ is the
+# ---- complete orthogonal decomposition on the pivoted QR (DESIGN §2.8, §2.9), single GPU ----
+# A P ~ Q1 [U^H 0] Z^H at r = rank(H; rtol): (F, γ) is the factorisation R_r^H = Z [U; 0] in the storage format above.  Its \ is the
 # minimum-norm solution, the answer the stdlib's qr(A, ColumnNorm()) \ b gives (up to how the rank is picked); \ on the pivoted
 # struct itself stays the basic solution.
 struct CompleteOrthogonalStruct{T1, T2, T3}
@@ -254,26 +234,56 @@ struct CompleteOrthogonalStruct{T1, T2, T3}
     γ::T3
     rank::Int
 end
-function complete_orthogonal(H::PivotedHouseholderQRStruct; rtol::Real = max(size(H.A)...) * eps(Float64))
-    A = H.A; m, n = size(A)
-    r = rank(H; rtol)
-    F = CUDA.zeros(Float64, n, r); γ = CUDA.zeros(Float64, r)
-    GC.@preserve A F γ check(:dhqr_cod_f64, ccall((:dhqr_cod_f64, libdhqr), Cint,
-        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, CuPtr{Float64}, Ptr{Cvoid}),
-        handle().ptr, m, n, r, pointer(A), stride(A, 2), pointer(H.α), pointer(F), max(n, 1), pointer(γ), stream_ptr()))
-    return CompleteOrthogonalStruct(H, F, γ, r)
+
+for (T, qp, sq, cd, sc) in ((Float64, :dhqr_qrcp_f64, :dhqr_solve_qrcp_f64, :dhqr_cod_f64, :dhqr_solve_cod_f64),
+                            (ComplexF64, :dhqr_qrcp_c64, :dhqr_solve_qrcp_c64, :dhqr_cod_c64, :dhqr_solve_cod_c64))
+    @eval begin
+        function qr!(A::CuMatrix{$T}, ::ColumnNorm)
+            m, n = size(A)
+            α = CUDA.zeros($T, n); jpvt = CUDA.zeros(Int64, n)
+            GC.@preserve A α jpvt check($(QuoteNode(qp)), ccall(($(QuoteNode(qp)), libdhqr), Cint,
+                (Ptr{Cvoid}, Int64, Int64, CuPtr{$T}, Int64, CuPtr{$T}, CuPtr{Int64}, Ptr{Cvoid}),
+                handle().ptr, m, n, pointer(A), stride(A, 2), pointer(α), pointer(jpvt), stream_ptr()))
+            return PivotedHouseholderQRStruct(A, α, jpvt)
+        end
+        # H \ b: the basic solution x = P [R11^{-1} (Q^H b)[1:r]; 0] at r = rank(H; rtol); b is not modified
+        function LinearAlgebra.ldiv!(x::AbstractVector, H::PivotedHouseholderQRStruct{<:CuMatrix{$T}}, b::AbstractVector;
+                                     rtol::Real = max(size(H.A)...) * eps(Float64))
+            A = H.A; m, n = size(A)
+            r = rank(H; rtol)
+            s = CuVector{$T}(b)
+            GC.@preserve A s check($(QuoteNode(sq)), ccall(($(QuoteNode(sq)), libdhqr), Cint,
+                (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{$T}, Int64, CuPtr{$T}, CuPtr{Int64}, CuPtr{$T}, Int64, Cint, Ptr{Cvoid}),
+                handle().ptr, m, n, r, pointer(A), stride(A, 2), pointer(H.α), pointer(H.jpvt), pointer(s), m, 1, stream_ptr()))
+            copyto!(x, Array(s[1:n]))
+            return x
+        end
+        LinearAlgebra.:(\)(H::PivotedHouseholderQRStruct{<:CuMatrix{$T}}, b::AbstractVector) =
+            ldiv!(Vector{$T}(undef, size(H.A, 2)), H, b)
+        function complete_orthogonal(H::PivotedHouseholderQRStruct{<:CuMatrix{$T}}; rtol::Real = max(size(H.A)...) * eps(Float64))
+            A = H.A; m, n = size(A)
+            r = rank(H; rtol)
+            F = CUDA.zeros($T, n, r); γ = CUDA.zeros($T, r)
+            GC.@preserve A F γ check($(QuoteNode(cd)), ccall(($(QuoteNode(cd)), libdhqr), Cint,
+                (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{$T}, Int64, CuPtr{$T}, CuPtr{$T}, Int64, CuPtr{$T}, Ptr{Cvoid}),
+                handle().ptr, m, n, r, pointer(A), stride(A, 2), pointer(H.α), pointer(F), max(n, 1), pointer(γ), stream_ptr()))
+            return CompleteOrthogonalStruct(H, F, γ, r)
+        end
+        function LinearAlgebra.ldiv!(x::AbstractVector, C::CompleteOrthogonalStruct{<:PivotedHouseholderQRStruct{<:CuMatrix{$T}}},
+                                     b::AbstractVector)
+            A = C.qrcp.A; m, n = size(A)
+            s = CuVector{$T}(b)
+            GC.@preserve A s check($(QuoteNode(sc)), ccall(($(QuoteNode(sc)), libdhqr), Cint,
+                (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{$T}, Int64, CuPtr{Int64}, CuPtr{$T}, Int64, CuPtr{$T}, CuPtr{$T}, Int64,
+                 Cint, Ptr{Cvoid}),
+                handle().ptr, m, n, C.rank, pointer(A), stride(A, 2), pointer(C.qrcp.jpvt), pointer(C.F), max(n, 1), pointer(C.γ),
+                pointer(s), m, 1, stream_ptr()))
+            copyto!(x, Array(s[1:n]))
+            return x
+        end
+        LinearAlgebra.:(\)(C::CompleteOrthogonalStruct{<:PivotedHouseholderQRStruct{<:CuMatrix{$T}}}, b::AbstractVector) =
+            ldiv!(Vector{$T}(undef, size(C.qrcp.A, 2)), C, b)
+    end
 end
-function LinearAlgebra.ldiv!(x::AbstractVector, C::CompleteOrthogonalStruct, b::AbstractVector)
-    A = C.qrcp.A; m, n = size(A)
-    s = CuVector{Float64}(b)
-    GC.@preserve A s check(:dhqr_solve_cod_f64, ccall((:dhqr_solve_cod_f64, libdhqr), Cint,
-        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Int64}, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64,
-         Cint, Ptr{Cvoid}),
-        handle().ptr, m, n, C.rank, pointer(A), stride(A, 2), pointer(C.qrcp.jpvt), pointer(C.F), max(n, 1), pointer(C.γ), pointer(s), m,
-        1, stream_ptr()))
-    copyto!(x, Array(s[1:n]))
-    return x
-end
-LinearAlgebra.:(\)(C::CompleteOrthogonalStruct, b::AbstractVector) = ldiv!(Vector{Float64}(undef, size(C.qrcp.A, 2)), C, b)
 
 end # module

@@ -105,7 +105,7 @@ int dhqr_destroy(dhqr_handle h);
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
- *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64; device-side, read after synchronising)
+ *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64 and dhqr_qrcp_c64; device-side, read after synchronising)
  *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
  *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys.
  *   Any other key returns -2 (unknown option). */
@@ -257,6 +257,47 @@ int dhqr_cod_f64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const double
  * -11 null or misaligned b, -12 ldb < max(1, m), -13 nrhs < 0.  n = 0 or nrhs = 0 is a no-op. */
 int dhqr_solve_cod_f64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const double *dA, int64_t lda, const int64_t *d_jpvt,
                        const double *dF, int64_t ldf, const double *d_gamma, double *d_b, int64_t ldb, int nrhs, void *stream);
+
+/* ---- ComplexF64 QR with column pivoting and the complete orthogonal decomposition (LAPACK zgeqp3 + zgelsy) --------------------
+ * The twins of dhqr_qrcp_f64, dhqr_solve_qrcp_f64, dhqr_cod_f64 and dhqr_solve_cod_f64, argument for argument, with void* for
+ * ComplexF64 data (DESIGN §2.9).  Single GPU (a handle with nranks > 1 returns -1), n <= m, no row limit.  Stream-ordered; no call
+ * synchronises apart from workspace growth (point (iv)); dhqr_cod_c64 factors R_r^H on the complex unpivoted path, which never
+ * synchronises, so it has no point (ii).  Two calls on the same input give bitwise identical results.  Nothing outside the
+ * documented operands is written.  Every ComplexF64 pointer (A, alpha, F, gamma, b) must be 16 B aligned: one that is only 8 B
+ * aligned returns minus its argument index before anything is enqueued; jpvt stays int64_t*, 8 B aligned.  Every check runs
+ * before anything is enqueued.  Error numbering is that of the Float64 twin.
+ *
+ * dhqr_qrcp_c64: factors in place.  On return (dA, lda, d_alpha) is the factorisation of A[:, jpvt] in the library's complex storage
+ * format (v scaled to ||v||^2 = 2, H_j = I - v_j v_j^H, complex alpha), so dhqr_apply_qt_c64, dhqr_backsolve_c64, dhqr_form_q_c64,
+ * dhqr_forwardsolve_c64 and dhqr_solve_adj_c64 take it as that.  Pivots as in dhqr_qrcp_f64 (largest partial norm, ties to the
+ * smallest index, a NaN norm beats every number).  alpha_k = -exp(i angle(x0)) ||x||, formed as dhqr_qr_c64 forms it, signed-zero
+ * pivots included.  Once the largest remaining norm is exactly 0, every remaining step stores v = 0 and alpha = 0 (H = I).  Exact
+ * renorms count in the read-only option "qrcp_renorms".  Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 null
+ * (n > 0) or misaligned A, -5 lda < max(1, m), -6 null or misaligned alpha, -7 null or misaligned jpvt.  n = 0 is a no-op. */
+int dhqr_qrcp_c64(dhqr_handle h, int64_t m, int64_t n, void *dA, int64_t lda, void *d_alpha, int64_t *d_jpvt, void *stream);
+/* x = P [R11^{-1} (Q^H b)[0:rank]; 0], the basic solution at the given rank, from dhqr_qrcp_c64.  d_b: m x nrhs, ldb >= max(1, m),
+ * in place: on return b[0:n] = x, and rows n..m-1 hold rows n..m-1 of H_rank ... H_1 b.  rank = 0 gives x = 0.  jpvt entries outside
+ * [0, n) are skipped.  Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 rank < 0 or rank > n, -5 null or
+ * misaligned A, -6 lda < max(1, m), -7 null or misaligned alpha, -8 null or misaligned jpvt, -9 null or misaligned b,
+ * -10 ldb < max(1, m), -11 nrhs < 0.  n = 0 or nrhs = 0 is a no-op. */
+int dhqr_solve_qrcp_c64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const void *dA, int64_t lda, const void *d_alpha,
+                        const int64_t *d_jpvt, void *d_b, int64_t ldb, int nrhs, void *stream);
+/* dhqr_cod_c64: F (n x rank, ldf >= max(1, n)) <- the factorisation of R_r^H = Z [U; 0] (a conjugating transpose of the leading rank
+ * rows of R) in the library's complex storage format, gamma (rank) <- diag(U), complex.  A and alpha are read, never written; nothing
+ * outside F's n x rank block and gamma is written.  The factorisation is the one dhqr_qr_c64 runs.  n = 0 or rank = 0 is a no-op.
+ * Errors: -1 null or multi-rank handle, -2 m < 0, -3 n < 0 or n > m, -4 rank < 0 or rank > n, -5 null or misaligned A,
+ * -6 lda < max(1, m), -7 null or misaligned alpha, -8 F null (rank > 0), misaligned, or overlapping A's m x n block or alpha,
+ * -9 ldf < max(1, n), -10 gamma null (rank > 0), misaligned, or overlapping A, alpha or F.  No row-limit error: the complex path has
+ * no row limit. */
+int dhqr_cod_c64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const void *dA, int64_t lda, const void *d_alpha, void *dF,
+                 int64_t ldf, void *d_gamma, void *stream);
+/* x = P Z [U^{-H} (Q^H b)[0:rank]; 0], the minimum-norm solution at the given rank, from dhqr_qrcp_c64's (A, jpvt) and
+ * dhqr_cod_c64's (F, gamma) at the same rank.  d_b as in dhqr_solve_qrcp_c64.  rank = 0 gives x = 0.  jpvt entries outside [0, n)
+ * are skipped.  Errors: -1 to -6 as above, -7 null or misaligned jpvt, -8 F null (rank > 0) or misaligned, -9 ldf < max(1, n),
+ * -10 gamma null (rank > 0) or misaligned, -11 null or misaligned b, -12 ldb < max(1, m), -13 nrhs < 0.  n = 0 or nrhs = 0 is a
+ * no-op. */
+int dhqr_solve_cod_c64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const void *dA, int64_t lda, const int64_t *d_jpvt,
+                       const void *dF, int64_t ldf, const void *d_gamma, void *d_b, int64_t ldb, int nrhs, void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
