@@ -49,6 +49,9 @@ SIGNATURES = {
     "dhqr_solve_qrcp_c64": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _int, _vp],
     "dhqr_cod_c64": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp],
     "dhqr_solve_cod_c64": [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _int, _vp],
+    "dhqr_qr_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp],
+    "dhqr_apply_qt_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
+    "dhqr_apply_q_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

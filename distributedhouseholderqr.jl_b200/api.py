@@ -698,3 +698,118 @@ def fill_uniform_(A: torch.Tensor, seed: int, i0: int = 0, j0: int = 0, handle: 
         _lib.call("dhqr_fill_uniform_f64", h.raw, seed, i0, j0, m, n, C.c_void_p(A.data_ptr()), _lda(A),
                   _stream_ptr(A.device))
     return A
+
+
+# --------------------------------------------------------------------------------------------
+# new rows into an existing factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10
+# --------------------------------------------------------------------------------------------
+class AppendedRows:
+    """[R; B] = Q~ [R'; 0] from ``append_rows_``: ``.B`` holds the reflector tails V2 (k x n, the caller's block, overwritten) and
+    ``.vtop`` their tops, so H~_j = I - v~_j v~_j' with v~_j = vtop[j] on row j of R and B[:, j] on the new rows."""
+
+    def __init__(self, B, vtop, handle: Handle):
+        self.B = B
+        self.vtop = vtop
+        self.handle = handle
+
+    def _apply(self, fn: str, c: torch.Tensor, e: torch.Tensor):
+        k, n = self.B.shape
+        ldc, nrhs = _rhs_args(c, n)
+        lde, nrhs_e = _rhs_args(e, k)
+        if nrhs != nrhs_e:
+            raise ValueError("c and e must have the same number of right-hand sides")
+        with torch.cuda.device(self.B.device):
+            _lib.call(fn, self.handle.raw, n, k, C.c_void_p(self.B.data_ptr()), _lda(self.B), C.c_void_p(self.vtop.data_ptr()),
+                      C.c_void_p(c.data_ptr()), ldc, C.c_void_p(e.data_ptr()), lde, nrhs, _stream_ptr(self.B.device))
+        return c, e
+
+    def apply_qt_(self, c: torch.Tensor, e: torch.Tensor):
+        """[c; e] <- Q~' [c; e] in place: c has n rows, e has k rows (vectors, or column-major blocks of equal width)."""
+        return self._apply("dhqr_apply_qt_append_f64", c, e)
+
+    def apply_q_(self, c: torch.Tensor, e: torch.Tensor):
+        """[c; e] <- Q~ [c; e] in place, the inverse of apply_qt_."""
+        return self._apply("dhqr_apply_q_append_f64", c, e)
+
+
+def append_rows_(H, B: torch.Tensor, handle: Optional[Handle] = None) -> AppendedRows:
+    """Fold the k new rows ``B`` (a column-major float64 CUDA tensor, k x n) into the factorisation ``H`` (a single-GPU
+    DistributedHouseholderQRStruct, or a pair (A, α)): afterwards (H.A, H.α) hold R' of [R; B] = Q~ [R'; 0] in A's strict upper
+    triangle and α, while A's diagonal and lower trapezoid (the original reflectors) are left as they are.  ``B`` is overwritten
+    with the reflector tails.  k may not exceed the handle's option "append_max_rows" (StreamingLeastSquares splits larger
+    blocks).  Stream-ordered, no synchronisation."""
+    A, alpha = (H.A, H.α) if isinstance(H, DistributedHouseholderQRStruct) else H
+    if isinstance(A, ColumnBlockMatrix) or not isinstance(A, torch.Tensor) or not A.is_cuda:
+        raise TypeError("append_rows_ works on a single-GPU factorisation held in a CUDA tensor")
+    if A.dtype != torch.float64 or alpha.dtype != torch.float64 or B.dtype != torch.float64:
+        raise TypeError("append_rows_ is Float64 only")
+    n = alpha.shape[0]
+    if A.shape[1] != n or A.shape[0] < n:
+        raise ValueError("A must have len(alpha) columns and at least as many rows")
+    if B.dim() != 2 or B.shape[1] != n:
+        raise ValueError(f"B must be a (k, {n}) column-major block")
+    h = handle or getattr(H, "handle", None) or default_handle(A.device.index)
+    k = B.shape[0]
+    vtop = torch.zeros(n, dtype=torch.float64, device=A.device)
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_qr_append_f64", h.raw, n, k, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+                  C.c_void_p(B.data_ptr()), _lda(B), C.c_void_p(vtop.data_ptr()), _stream_ptr(A.device))
+    return AppendedRows(B, vtop, h)
+
+
+class StreamingLeastSquares:
+    """min ||A x - b|| for an A of any height, fed block by block: each block of rows is folded into R (starting from R = 0) and
+    its right-hand sides into c = (Q'b)[0:n]; what the rotation moves out of reach adds to the residual.  Blocks above the row cap
+    of one append are split.  ``add`` takes CUDA tensors or Fortran-ordered numpy arrays (uploaded); ``solve`` returns x as an
+    (n, nrhs) tensor (a length-n vector for nrhs = 1)."""
+
+    def __init__(self, n: int, nrhs: int = 1, device=0, handle: Optional[Handle] = None):
+        self.n, self.nrhs = int(n), int(nrhs)
+        self.device = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
+        self.handle = handle or default_handle(self.device.index)
+        self.A = colmajor_empty(self.n, self.n, self.device)
+        self.A.zero_()
+        self.α = torch.zeros(self.n, dtype=torch.float64, device=self.device)
+        self.c = colmajor_empty(self.n, self.nrhs, self.device)
+        self.c.zero_()
+        self._ss = torch.zeros(self.nrhs, dtype=torch.float64, device=self.device)
+        self.rows = 0
+        self._cap = self.handle.get_option("append_max_rows")
+
+    def add(self, A_blk, b_blk) -> "StreamingLeastSquares":
+        """Fold rows ``A_blk`` (k x n) with right-hand sides ``b_blk`` (length k, or k x nrhs) into the problem."""
+        A_blk = torch.as_tensor(A_blk)
+        b_blk = torch.as_tensor(b_blk)
+        if b_blk.dim() == 1:
+            b_blk = b_blk[:, None]
+        k = A_blk.shape[0]
+        if A_blk.dim() != 2 or A_blk.shape[1] != self.n or tuple(b_blk.shape) != (k, self.nrhs):
+            raise ValueError(f"need a (k, {self.n}) block and its (k, {self.nrhs}) right-hand sides")
+        for r0 in range(0, k, self._cap):
+            r1 = min(k, r0 + self._cap)
+            B = to_colmajor(A_blk[r0:r1], device=self.device)
+            e = to_colmajor(b_blk[r0:r1], device=self.device)
+            append_rows_((self.A, self.α), B, self.handle).apply_qt_(self.c, e)
+            self._ss += (e * e).sum(0)
+        self.rows += k
+        return self
+
+    @property
+    def alpha(self):
+        return self.α
+
+    @property
+    def R(self) -> torch.Tensor:
+        """The n x n triangle R' of every row added so far."""
+        return form_r(self.A, self.α)
+
+    def solve(self) -> torch.Tensor:
+        """x = R'^{-1} c through backsolve_; neither R nor c is modified."""
+        x = colmajor_empty(self.n, self.nrhs, self.device)
+        x.copy_(self.c)
+        backsolve_(x, self.A, self.α, self.handle)
+        return x[:, 0] if self.nrhs == 1 else x
+
+    def residual_norm(self) -> torch.Tensor:
+        """||A x - b|| per right-hand side at the least-squares solution, accumulated as the blocks were folded in."""
+        return self._ss.sqrt()

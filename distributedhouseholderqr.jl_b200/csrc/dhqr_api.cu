@@ -22,6 +22,7 @@
 #include "dhqr_complex.cuh"
 #include "dhqr_qrcp.cuh"
 #include "dhqr_qrcp_c.cuh"
+#include "dhqr_append.cuh"
 
 using namespace dhqr;
 
@@ -312,6 +313,7 @@ static int set_attrs(dhqr_context* c) {
     CU(cudaFuncSetAttribute(k_ymake<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(32)));
     CU(cudaFuncSetAttribute(k_ymake2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_YMAKE2));
     CU(cudaFuncSetAttribute(k_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
+    CU(cudaFuncSetAttribute(k_tp_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
     CU(cudaFuncSetAttribute(k_chol128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_WIDE1));
     CU(cudaFuncSetAttribute(k_hr128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_WIDE1));
     CU(cudaFuncSetAttribute(k_vpk_rmul, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_RMUL));
@@ -449,15 +451,15 @@ static int pack_v(dhqr_context* c, cudaStream_t st, const double* A, int64_t lda
 // asks; nv > 0: W starts with the nv columns of V'V itself (for T), then come the ncols columns of B (`rows` rows).
 static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* vpk, dhqr_context::WSet& w, int voff, int nbp, int nv,
                                const double* B, int64_t ldb, int64_t rows, int ncols, const char* what, int* nsplit_out,
-                               int64_t* pstride_out) {
+                               int64_t* pstride_out, int reserve = 0) {
     const bool small = (nbp <= 32);
     const int NBPK = small ? 32 : 128;          // kernel instantiation
     const int bn = small ? G1S_BN : G1_BN;
     const int tiles = (nv + ncols + bn - 1) / bn;
     const int nchunks = (int)((rows + KC1 - 1) / KC1);
-    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart.n / ((size_t)bn * NBPK)));
+    const int nsplit = pick_splits(tiles, nchunks, c->sms, (int64_t)(w.wpart.n / ((size_t)bn * NBPK)) - (int64_t)reserve * tiles);
     const int64_t pstride = (int64_t)tiles * bn * NBPK;
-    if ((size_t)(pstride * nsplit) > w.wpart.n) return set_err(4001, "internal: W partial workspace too small");
+    if ((size_t)(pstride * (nsplit + reserve)) > w.wpart.n) return set_err(4001, "internal: W partial workspace too small");
     GemmVtaArgs g1;
     g1.vpk = vpk; g1.voff = voff; g1.nv = nv;
     g1.A = B; g1.lda = ldb; g1.rows = rows; g1.na = ncols; g1.nchunks = nchunks;
@@ -606,6 +608,16 @@ static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const
     });
 }
 
+// tag space of the exchange cells nearly used up: start over with clean cells (k_panel, k_tp_panel)
+static int ll_epoch_check(dhqr_context* c, cudaStream_t st) {
+    if (c->ll_epoch > 0xF0000000u) {
+        CU(cudaMemsetAsync(c->cells, 0, sizeof(unsigned long long) * (size_t)IB * (PANEL_MAXG + 2) * IB * 2, st));
+        CU(cudaMemsetAsync(c->cells2, 0, sizeof(unsigned long long) * (2 * (size_t)(PANEL_MAXG + 1) * (IB * (IB + 1) / 2) + IB * IB + 2 * IB) * 2, st));
+        c->ll_epoch = 0;
+    }
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------------
 // cooperative panel launch: factor mp x ncols (<= IB) at P, V block -> vout columns
 // ------------------------------------------------------------------------------------------------
@@ -623,11 +635,7 @@ static int launch_panel(dhqr_context* c, cudaStream_t st, double* vpk, double* P
     const int lds = (int)rpc + 4;   // rpc is a multiple of 8 -> lds == 4 mod 8
     const size_t smem = (size_t)IB * lds * 8;
     if (smem > 184 * 1024) return set_err(-2, "m too large for the resident panel kernel (%lld rows per CTA)", (long long)rpc);
-    if (c->ll_epoch > 0xF0000000u) {   // tag space nearly used up: start over with clean cells
-        CU(cudaMemsetAsync(c->cells, 0, sizeof(unsigned long long) * (size_t)IB * (PANEL_MAXG + 2) * IB * 2, st));
-        CU(cudaMemsetAsync(c->cells2, 0, sizeof(unsigned long long) * (2 * (size_t)(PANEL_MAXG + 1) * (IB * (IB + 1) / 2) + IB * IB + 2 * IB) * 2, st));
-        c->ll_epoch = 0;
-    }
+    TRY(ll_epoch_check(c, st));
     PanelArgs a;
     a.P = P; a.ldp = ldp; a.mp = mp; a.ncols = ncols; a.alpha = alpha;
     a.vpk = vpk; a.voff = voff; a.vtop = vtop; a.vrows = vrows;
@@ -1733,6 +1741,7 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
         *value = st2[!strcmp(key, "panels_fallback") ? 1 : 0];
     }
     else if (!strcmp(key, "sms")) *value = c->sms;
+    else if (!strcmp(key, "append_max_rows")) *value = narrow_panel_max_rows(c);
     else if (!strcmp(key, "rank")) *value = c->rank;
     else if (!strcmp(key, "nranks")) *value = c->nranks;
     else return set_err(-2, "unknown option '%s'", key);
@@ -2630,6 +2639,189 @@ int dhqr_solve_cod_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const 
         CU(cudaMemcpy2DAsync(x, (size_t)n * 16, b, (size_t)ldb * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
     }
     return qrcp_scatter_c(c, st, n, rank > 0 ? n : 0, x, n, d_jpvt, b, ldb, nrhs);
+}
+
+// ---- triangular-pentagonal QR: fold new rows into a factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10 ---------------------
+// One block reflector of the structured update, on the stacked operand [X; C]: X = the block's kb rows of R (or of c), C = k rows of B
+// (or of e).  V~ = [diag(vtop); V2] with V2 = packed columns [voff, voff + nbp) of vpk.  The existing sequence of
+// apply_block_reflector on C with V = V2, plus the vtop rows in two places: diag(vtop) X as one more split-K partial of W (so the
+// fixed-order reduction adds it), and X += diag(vtop) Y after Y is formed.  T comes from V2'V2 unchanged: off the diagonal it equals
+// V~'V~, and T' is built from the strict triangle alone.  trans = 1: Q~ instead of Q~'.
+static int tp_block_update(dhqr_context* c, cudaStream_t st, const double* vpk, int voff, int nbp, int kb, const double* vtop, int64_t k,
+                           double* C, int64_t ldc, double* X, int64_t ldx, int ncols, int trans) {
+    if (ncols <= 0 || k <= 0) return 0;
+    auto& w = c->ws[0];
+    const bool small = (nbp <= 32);
+    const int NBPK = small ? 32 : 128;
+    const int next = NBPK + ncols;
+    if ((size_t)next * NBPK > w.wsum.n) return set_err(4003, "internal: W workspace too small");
+    int nsplit = 0;
+    int64_t pstride = 0;
+    TRY(launch_vta_partials(c, st, vpk, w, voff, nbp, NBPK, C, ldc, k, ncols, small ? "k_gemm_vta32" : "k_gemm_vta128", &nsplit,
+                            &pstride, 1));
+    const int64_t nelem = (int64_t)next * NBPK;
+    TRY(launch(c, st, "k_tp_wpart", 8.0 * (double)kb * ncols, [&](CwtSlot) {
+        k_tp_wpart<<<wreduce_grid(c, nelem), 256, 0, st>>>(w.wpart.p + (size_t)nsplit * pstride, NBPK, NBPK, ncols, vtop, kb, X, ldx);
+    }));
+    ++nsplit;
+    const int ygrid = (ncols + YCOLS - 1) / YCOLS;
+    if (small) {
+        TRY(launch(c, st, "k_mid32", 0.0, [&](CwtSlot) { k_mid32<<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, w.linv, trans); }));
+    } else {
+        TRY(launch(c, st, "k_wreduce", 0.0, [&](CwtSlot cwt) {
+            k_wreduce<<<wreduce_grid(c, nelem), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, w.wsum, cwt);
+        }));
+        TRY(launch(c, st, "k_tinv128", 0.0, [&](CwtSlot cwt) { k_tinv<128><<<1, 512, smem_tinv(128), st>>>(w.wsum, w.linv, 0, cwt); }));
+        TRY(launch(c, st, "k_ymake128", 0.0, [&](CwtSlot cwt) {
+            k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, NBPK, ncols, w.linv, w.ypk, trans, cwt);
+        }));
+    }
+    TRY(launch_cvy(c, st, vpk, voff, nbp, w.ypk, k, 0, C, ldc, ncols, 0));
+    const int64_t nx = (int64_t)kb * ncols;
+    return launch(c, st, "k_tp_rows", 16.0 * (double)nx, [&](CwtSlot) {
+        k_tp_rows<<<(unsigned)std::min<int64_t>((nx + 255) / 256, 8 * c->sms), 256, 0, st>>>(X, ldx, ncols, vtop, kb, w.ypk, NBPK / KC);
+    });
+}
+
+// Workspace of both structured calls: the usual sets for k rows and `cols` W columns, and room for the extra W partial.
+static int tp_workspace(dhqr_context* c, cudaStream_t st, int64_t k, int64_t cols) {
+    TRY(ensure_workspace(c, st, k, cols));
+    const int64_t tiles = (NBMAX + cols + G1_BN - 1) / G1_BN;
+    return c->ws[0].wpart.ensure((size_t)std::max<int64_t>(2 * tiles, WPART_TILES) * NBMAX * G1_BN, st);
+}
+
+static int launch_tp_panel(dhqr_context* c, cudaStream_t st, double* B, int64_t ldb, int64_t k, double* R, int64_t ldr, double* alpha,
+                           double* vtop, int ncols, int voff, int64_t vrows) {
+    const int gmax = std::min(c->sms, PANEL_MAXG);
+    const int64_t rpc = rup(std::max<int64_t>((k + gmax - 1) / gmax, 64), 8);
+    const int G = (int)((k + rpc - 1) / rpc);
+    const int lds = (int)rpc + 4;
+    const size_t smem = (size_t)IB * lds * 8;
+    if (smem > 184 * 1024) return set_err(-3, "k too large for the resident panel kernel (%lld rows per CTA)", (long long)rpc);
+    TRY(ll_epoch_check(c, st));
+    TpPanelArgs a;
+    a.B = B; a.ldb = ldb; a.k = k; a.R = R; a.ldr = ldr; a.alpha = alpha; a.vtop = vtop; a.ncols = ncols;
+    a.vpk = c->vpk2[0]; a.voff = voff; a.vrows = vrows; a.rows_per_cta = (int)rpc; a.lds = lds;
+    a.cells = c->cells; a.epoch = c->ll_epoch;
+    void* args[] = {&a};
+    return launch(c, st, "k_tp_panel", 16.0 * (double)k * ncols, [&](CwtSlot) {   // work = bytes: the B panel read once + written once
+        const cudaError_t e = cudaLaunchCooperativeKernel((void*)k_tp_panel, dim3(G), dim3(PANEL_THREADS), args, smem, st);
+        if (e == cudaSuccess) c->ll_epoch += IB + 8;
+        return e;
+    });
+}
+
+// Outer panels of 128 columns, each four 32-column k_tp_panel launches with the 32-wide update of the rest of the outer panel after
+// each, then the 128-wide update of the trailing columns.  Row i of R changes only under reflector i, so each launch reads R as the
+// caller passed it.
+static int qr_append_local(dhqr_context* c, cudaStream_t st, int64_t n, int64_t k, double* R, int64_t ldr, double* alpha, double* B,
+                           int64_t ldb, double* vtop) {
+    TRY(tp_workspace(c, st, k, n));
+    const int64_t vrows = rup(k, 128);
+    for (int64_t k0 = 0; k0 < n; k0 += NBMAX) {
+        const int kb = (int)std::min<int64_t>(NBMAX, n - k0);
+        for (int o = 0; o < kb; o += IB) {
+            const int ib = std::min(IB, kb - o);
+            const int64_t cs = k0 + o;
+            TRY(launch_tp_panel(c, st, B + cs * ldb, ldb, k, R + cs * ldr + cs, ldr, alpha + cs, vtop + cs, ib, o, vrows));
+            const int rem = kb - o - ib;
+            if (rem > 0)
+                TRY(tp_block_update(c, st, c->vpk2[0], o, IB, ib, vtop + cs, k, B + (cs + ib) * ldb, ldb, R + (cs + ib) * ldr + cs, ldr,
+                                    rem, 0));
+        }
+        const int64_t trail = n - k0 - kb;
+        if (trail > 0)
+            TRY(tp_block_update(c, st, c->vpk2[0], 0, NBMAX, kb, vtop + k0, k, B + (k0 + kb) * ldb, ldb, R + (k0 + kb) * ldr + k0, ldr,
+                                (int)trail, 0));
+    }
+    return 0;
+}
+
+// [c; e] <- Q~' [c; e] (blocks first to last) or Q~ [c; e] (trans = 1, last to first); V2 packed from B, T recomputed from V2.
+static int apply_append_local(dhqr_context* c, cudaStream_t st, int64_t n, int64_t k, const double* B, int64_t ldb, const double* vtop,
+                              double* dc, int64_t ldc, double* de, int64_t lde, int nrhs, int trans) {
+    TRY(tp_workspace(c, st, k, std::max<int64_t>(n, nrhs)));
+    const int64_t vrows = rup(k, 128);
+    const int64_t ofirst = trans ? ((n - 1) / NBMAX) * NBMAX : 0, ostep = trans ? -(int64_t)NBMAX : NBMAX;
+    for (int64_t o = ofirst; o >= 0 && o < n; o += ostep) {
+        const int kb = (int)std::min<int64_t>(NBMAX, n - o);
+        const int nbp = kb <= IB ? IB : NBMAX;
+        TRY(pack_v(c, st, B + o * ldb, ldb, k, kb, 0, c->vpk2[0], 0, vrows, nbp));
+        TRY(tp_block_update(c, st, c->vpk2[0], 0, nbp, kb, vtop + o, k, de, lde, dc + o, ldc, nrhs, trans));
+    }
+    return 0;
+}
+
+// Arguments 1-3 of all three calls: handle, n, k (k capped by the panel kernel's slab capacity)
+static int check_append_head(dhqr_context* c, int64_t n, int64_t k) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "appending rows is single-GPU (the handle has %d ranks)", c->nranks);
+    if (n < 0) return set_err(-2, "n < 0");
+    if (k < 0) return set_err(-3, "k < 0");
+    if (k > narrow_panel_max_rows(c))
+        return set_err(-3, "k = %lld exceeds the rows one append can take on this device (%lld): split the block", (long long)k,
+                       (long long)narrow_panel_max_rows(c));
+    return 0;
+}
+
+int dhqr_qr_append_f64(dhqr_handle c, int64_t n, int64_t k, double* dR, int64_t ldr, double* d_alpha, double* dB, int64_t ldb,
+                       double* d_vtop, void* stream) {
+    TRY(check_append_head(c, n, k));
+    if (n > 0 && !dR) return set_err(-4, "null R");
+    TRY(check_qrcp_ptr(dR, -4, "R"));
+    if (ldr < std::max<int64_t>(1, n)) return set_err(-5, "ldr < max(1,n)");
+    if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
+    TRY(check_qrcp_ptr(d_alpha, -6, "alpha"));
+    const size_t rbytes = n > 0 ? ((size_t)(n - 1) * ldr + n) * 8 : 0, abytes = (size_t)n * 8;
+    if (n > 0 && k > 0 && !dB) return set_err(-7, "null B");
+    TRY(check_qrcp_ptr(dB, -7, "B"));
+    const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0;
+    if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-7, "B overlaps R or alpha");
+    if (ldb < std::max<int64_t>(1, k)) return set_err(-8, "ldb < max(1,k)");
+    if (n > 0 && !d_vtop) return set_err(-9, "null vtop");
+    TRY(check_qrcp_ptr(d_vtop, -9, "vtop"));
+    if (k > 0 && (spans_overlap(d_vtop, abytes, dR, rbytes) || spans_overlap(d_vtop, abytes, d_alpha, abytes) ||
+                  spans_overlap(d_vtop, abytes, dB, bbytes)))
+        return set_err(-9, "vtop overlaps R, alpha or B");
+    if (n == 0 || k == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return qr_append_local(c, (cudaStream_t)stream, n, k, dR, ldr, d_alpha, dB, ldb, d_vtop);
+}
+
+static int apply_append(dhqr_context* c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
+                        int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream, int trans) {
+    TRY(check_append_head(c, n, k));
+    if (n > 0 && k > 0 && !dB) return set_err(-4, "null B");
+    TRY(check_qrcp_ptr(dB, -4, "B"));
+    if (ldb < std::max<int64_t>(1, k)) return set_err(-5, "ldb < max(1,k)");
+    if (n > 0 && !d_vtop) return set_err(-6, "null vtop");
+    TRY(check_qrcp_ptr(d_vtop, -6, "vtop"));
+    const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0, vbytes = (size_t)n * 8;
+    const size_t cbytes = (n > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * ldc + n) * 8 : 0;
+    const size_t ebytes = (k > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * lde + k) * 8 : 0;
+    if (n > 0 && nrhs > 0 && !d_c) return set_err(-7, "null c");
+    TRY(check_qrcp_ptr(d_c, -7, "c"));
+    if (spans_overlap(d_c, cbytes, dB, bbytes) || spans_overlap(d_c, cbytes, d_vtop, vbytes)) return set_err(-7, "c overlaps B or vtop");
+    if (ldc < std::max<int64_t>(1, n)) return set_err(-8, "ldc < max(1,n)");
+    if (k > 0 && nrhs > 0 && !d_e) return set_err(-9, "null e");
+    TRY(check_qrcp_ptr(d_e, -9, "e"));
+    if (spans_overlap(d_e, ebytes, dB, bbytes) || spans_overlap(d_e, ebytes, d_vtop, vbytes) || spans_overlap(d_e, ebytes, d_c, cbytes))
+        return set_err(-9, "e overlaps B, vtop or c");
+    if (lde < std::max<int64_t>(1, k)) return set_err(-10, "lde < max(1,k)");
+    if (nrhs < 0) return set_err(-11, "nrhs < 0");
+    if (n == 0 || k == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return apply_append_local(c, (cudaStream_t)stream, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, trans);
+}
+
+int dhqr_apply_qt_append_f64(dhqr_handle c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
+                             int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream) {
+    return apply_append(c, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, stream, 0);
+}
+
+int dhqr_apply_q_append_f64(dhqr_handle c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
+                            int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream) {
+    return apply_append(c, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, stream, 1);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

@@ -172,6 +172,53 @@ function apply_q!(b::CuVecOrMat{Float64}, A::CuMatrix{Float64})
     return b
 end
 
+# ---- new rows into a factorisation (LAPACK dtpqrt / dtpmqrt; not in the reference), single GPU, DESIGN §2.10 ----
+# [R; B] = Q~ [R'; 0]: R' replaces R's strict upper triangle in A and α, B becomes the reflector tails, vtop their tops.
+struct AppendedRows
+    B::CuMatrix{Float64}
+    vtop::CuVector{Float64}
+end
+function append_rows!(H::DistributedHouseholderQRStruct{<:CuMatrix{Float64}}, B::CuMatrix{Float64})
+    k, n = size(B)
+    A = H.A
+    vtop = CUDA.zeros(Float64, n)
+    GC.@preserve A B vtop check(:dhqr_qr_append_f64, ccall((:dhqr_qr_append_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, CuPtr{Float64}, Ptr{Cvoid}),
+        handle().ptr, n, k, pointer(A), stride(A, 2), pointer(H.α), pointer(B), max(stride(B, 2), k), pointer(vtop), stream_ptr()))
+    return AppendedRows(B, vtop)
+end
+function apply_qt!(c::CuVecOrMat{Float64}, e::CuVecOrMat{Float64}, T::AppendedRows)
+    k, n = size(T.B)
+    GC.@preserve T c e check(:dhqr_apply_qt_append_f64, ccall((:dhqr_apply_qt_append_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Cint,
+         Ptr{Cvoid}),
+        handle().ptr, n, k, pointer(T.B), max(stride(T.B, 2), k), pointer(T.vtop), pointer(c), max(stride(c, 2), n), pointer(e),
+        max(stride(e, 2), k), size(c, 2), stream_ptr()))
+    return c, e
+end
+# min ||A x - b|| for A fed as row blocks (CuMatrix or Matrix; host blocks are uploaded), from R = 0: x and the residual norm.
+function streaming_lstsq(blocks, n::Integer)
+    H = DistributedHouseholderQRStruct(CUDA.zeros(Float64, n, n), CUDA.zeros(Float64, n))
+    c = CUDA.zeros(Float64, n)
+    ss = 0.0
+    cap = Ref{Int64}(0)
+    check(:dhqr_get_option, ccall((:dhqr_get_option, libdhqr), Cint, (Ptr{Cvoid}, Cstring, Ptr{Int64}), handle().ptr,
+                                  "append_max_rows", cap))
+    for (Ablk, bblk) in blocks
+        for r0 in 1:cap[]:size(Ablk, 1)
+            r1 = min(size(Ablk, 1), r0 + cap[] - 1)
+            e = CuVector{Float64}(bblk[r0:r1])
+            apply_qt!(c, e, append_rows!(H, CuMatrix{Float64}(Ablk[r0:r1, :])))
+            ss += sum(abs2, e)
+        end
+    end
+    x = copy(c)
+    GC.@preserve H x check(:dhqr_backsolve_f64, ccall((:dhqr_backsolve_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, Cint, Ptr{Cvoid}),
+        handle().ptr, n, n, 0, n, pointer(H.A), stride(H.A, 2), pointer(H.α), pointer(x), n, 1, stream_ptr()))
+    return Array(x), sqrt(ss)
+end
+
 # ---- solves with the adjoint (LAPACK ?gels with TRANS = 'C'; not in the reference), single GPU ----
 for (T, fs, sa) in ((Float64, :dhqr_forwardsolve_f64, :dhqr_solve_adj_f64), (ComplexF64, :dhqr_forwardsolve_c64, :dhqr_solve_adj_c64))
     @eval begin

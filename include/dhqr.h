@@ -105,7 +105,8 @@ int dhqr_destroy(dhqr_handle h);
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
- *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64 and dhqr_qrcp_c64; device-side, read after synchronising)
+ *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64 and dhqr_qrcp_c64; device-side, read after synchronising),
+ *                 "append_max_rows" (the largest k one dhqr_qr_append_f64 call takes on this device)
  *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
  *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys.
  *   Any other key returns -2 (unknown option). */
@@ -298,6 +299,36 @@ int dhqr_cod_c64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const void *
  * no-op. */
 int dhqr_solve_cod_c64(dhqr_handle h, int64_t m, int64_t n, int64_t rank, const void *dA, int64_t lda, const int64_t *d_jpvt,
                        const void *dF, int64_t ldf, const void *d_gamma, void *d_b, int64_t ldb, int nrhs, void *stream);
+
+/* ---- triangular-pentagonal QR: fold new rows into a factorisation (not in the reference; LAPACK dtpqrt / dtpmqrt) -----------
+ * [R; B] = Q~ [R'; 0] (DESIGN §2.10): R = triu(dR[0:n, 0:n], 1) + diag(alpha) is the n x n triangle of any factorisation in the
+ * library's storage format (dR may be the factored matrix itself), B the k x n block of new rows (ldb >= max(1, k)).  Only the strict
+ * upper triangle of dR's n x n block is read and written: its diagonal and lower trapezoid (the original reflectors) are never
+ * touched, so the original factorisation stays valid for dhqr_apply_qt_f64.  On return R' is in dR's strict upper triangle and in
+ * alpha; Q~ = H~_1 ... H~_n with H~_j = I - v~_j v~_j', v~_j = vtop[j] on row j of the R block and B[:, j] on the k new rows,
+ * ||v~_j||^2 = 2 or 0: B is overwritten with the reflector tails V2, vtop (length n) with their tops.  Each column follows the
+ * recurrences of dhqr_qr_f64 on the stacked (n + k) x n matrix, alpha_j = -sign(x0) ||x|| with x0 = R[j, j] in its current state and
+ * a zero x0 counted as positive (as in dhqr_qrcp_f64); a zero column stores v~ = 0 and alpha = 0.  In exact arithmetic R' is the R
+ * of the stacked factorisation.  Least squares needs no further entry point: x = R'^{-1} c is dhqr_backsolve_f64(h, n, n, 0, n, dR,
+ * ldr, alpha, c, ldc, nrhs, stream), which reads R's strict upper triangle and alpha only.
+ * Single GPU (a handle with nranks > 1 returns -1).  Stream-ordered, no synchronisation apart from workspace growth (point (iv)).
+ * Two calls on the same input give bitwise identical results, independent of ldr, ldb and 8 B base offsets.  Nothing outside the
+ * documented operands is written.  k is capped by the slab capacity of the panel kernel, the row limit of the blocked dhqr_qr_f64
+ * (728 x min(SMs, 160) rows; read-only option "append_max_rows"): a larger block returns -3 and is split by the caller.  n = 0 or
+ * k = 0 is a no-op.  Every check runs before anything is enqueued.  Errors: -1 null or multi-rank handle, -2 n < 0, -3 k < 0 or
+ * above the cap, -4 null (n > 0) or misaligned R, -5 ldr < max(1, n), -6 null or misaligned alpha, -7 null, misaligned B, or B
+ * overlapping R's n x n block or alpha, -8 ldb < max(1, k), -9 null or misaligned vtop, or vtop overlapping R, alpha or B. */
+int dhqr_qr_append_f64(dhqr_handle h, int64_t n, int64_t k, double *dR, int64_t ldr, double *d_alpha, double *dB, int64_t ldb,
+                       double *d_vtop, void *stream);
+/* [c; e] <- Q~' [c; e] (dhqr_apply_qt_append_f64) or Q~ [c; e] (dhqr_apply_q_append_f64), from (B, vtop) of dhqr_qr_append_f64:
+ * c is n x nrhs (ldc >= max(1, n)), e is k x nrhs (lde >= max(1, k)), both in place.  T is recomputed from V2.  Same stream and
+ * determinism rules.  n = 0, k = 0 or nrhs = 0 is a no-op.  Errors: -1 to -3 as above, -4 null or misaligned B, -5 ldb < max(1, k),
+ * -6 null or misaligned vtop, -7 null or misaligned c, or c overlapping B or vtop, -8 ldc < max(1, n), -9 null or misaligned e, or
+ * e overlapping B, vtop or c, -10 lde < max(1, k), -11 nrhs < 0. */
+int dhqr_apply_qt_append_f64(dhqr_handle h, int64_t n, int64_t k, const double *dB, int64_t ldb, const double *d_vtop,
+                             double *d_c, int64_t ldc, double *d_e, int64_t lde, int nrhs, void *stream);
+int dhqr_apply_q_append_f64(dhqr_handle h, int64_t n, int64_t k, const double *dB, int64_t ldb, const double *d_vtop,
+                            double *d_c, int64_t ldc, double *d_e, int64_t lde, int nrhs, void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
