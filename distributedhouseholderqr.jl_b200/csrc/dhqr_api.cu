@@ -608,9 +608,19 @@ static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const
     });
 }
 
+// Reset thresholds of the launch tags.  Tags are 32-bit and compared for equality with what a cell holds, so no tag may pass
+// 2^32 - 1 before its counter is reset.
+//   ll_epoch (k_panel, k_tp_panel): a launch starts at ll_epoch <= LL_EPOCH_MAX and uses tags up to ll_epoch + IB + 3 (k_panel's
+//     fast path: ftag + 2 = epoch + IB + 3; k_tp_panel: epoch + IB), at most 0xF0000023 < 2^32 - 1; it then advances the
+//     counter by IB + 8.
+//   bs_epoch (k_backsolve_wave, k_forwardsolve_wave) and uw_epoch (k_unblocked_wave): one tag per launch, ++epoch after a reset
+//     check at WAVE_EPOCH_MAX, so at most 0xFFFFFFF1 < 2^32 - 1.
+static constexpr uint32_t LL_EPOCH_MAX = 0xF0000000u;
+static constexpr uint32_t WAVE_EPOCH_MAX = 0xFFFFFFF0u;
+
 // tag space of the exchange cells nearly used up: start over with clean cells (k_panel, k_tp_panel)
 static int ll_epoch_check(dhqr_context* c, cudaStream_t st) {
-    if (c->ll_epoch > 0xF0000000u) {
+    if (c->ll_epoch > LL_EPOCH_MAX) {
         CU(cudaMemsetAsync(c->cells, 0, sizeof(unsigned long long) * (size_t)IB * (PANEL_MAXG + 2) * IB * 2, st));
         CU(cudaMemsetAsync(c->cells2, 0, sizeof(unsigned long long) * (2 * (size_t)(PANEL_MAXG + 1) * (IB * (IB + 1) / 2) + IB * IB + 2 * IB) * 2, st));
         c->ll_epoch = 0;
@@ -1313,7 +1323,7 @@ static int qr_unblocked(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
             TRY(c->uw_flags.ensure((size_t)n + 64, st));
             c->uw_epoch = 0;
         }
-        if (c->uw_epoch > 0xFFFFFFF0u) { CU(cudaMemsetAsync(c->uw_flags, 0, sizeof(unsigned int) * c->uw_flags.n, st)); c->uw_epoch = 0; }
+        if (c->uw_epoch > WAVE_EPOCH_MAX) { CU(cudaMemsetAsync(c->uw_flags, 0, sizeof(unsigned int) * c->uw_flags.n, st)); c->uw_epoch = 0; }
         const unsigned int tag = ++c->uw_epoch;
         int nn = (int)n;
         unsigned int* flags = c->uw_flags;
@@ -1484,7 +1494,7 @@ static int wave_prepare(dhqr_context* c, cudaStream_t st, int64_t nl) {
 
 // Tag of the next wave launch; the cells are cleared before the 32-bit tag could come round to a value they still hold.
 static int wave_tag(dhqr_context* c, cudaStream_t st, uint32_t* tag) {
-    if (c->bs_epoch > 0xFFFFFFF0u) {
+    if (c->bs_epoch > WAVE_EPOCH_MAX) {
         CU(cudaMemsetAsync(c->bs_cells, 0, c->bs_cells.n * sizeof(unsigned long long), st));
         c->bs_epoch = 0;
     }
@@ -1503,7 +1513,7 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
             TRY(wave_tag(c, st, &tag));
             TRY(launch(c, st, "k_backsolve_wave", 0.0, [&](CwtSlot) {
                 k_backsolve_wave<<<(unsigned)(nbk + nlow), BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx,
-                                                                              col0, nl, (int)nlow, c->bs_cells, tag);
+                                                                              col0, nl, c->bs_cells, tag);
             }));
         }
         return 0;
@@ -1696,6 +1706,13 @@ int dhqr_set_option(dhqr_handle c, const char* key, int64_t value) {
         c->wide_kappa = (double)value;
     } else if (!strcmp(key, "wide_trace")) {
         c->wide_trace = value ? 1 : 0;
+    } else if (!strcmp(key, "epoch_near_wrap")) {
+        // test hook: the tag counters two launches short of their reset (never backwards, so no tag a cell holds comes back);
+        // a counter whose buffer is allocated later starts over at 0 with it
+        if (value != 1) return set_err(-3, "epoch_near_wrap takes the value 1");
+        c->ll_epoch = std::max(c->ll_epoch, LL_EPOCH_MAX - 2 * (IB + 8) + 1);
+        c->bs_epoch = std::max(c->bs_epoch, WAVE_EPOCH_MAX - 1);
+        c->uw_epoch = std::max(c->uw_epoch, WAVE_EPOCH_MAX - 1);
     } else if (!strcmp(key, "panel_trace")) {
         if (value && !c->panel_trace) {
             // no stream here: the fill is complete before the call returns, so every later call sees it
@@ -3053,6 +3070,12 @@ int dhqr_debug_copy_f64(dhqr_handle c, const char* which, double* d_dst, int64_t
         std::vector<double> t(c->la_times.begin(), c->la_times.end());
         if ((size_t)nelems < t.size()) return set_err(-4, "need %zu elements", t.size());
         CU(cudaMemcpy(d_dst, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice));
+        return 0;
+    }
+    if (!strcmp(which, "epochs")) {   // the tag counters ll_epoch, bs_epoch, uw_epoch (exact in a double)
+        const double t[3] = {(double)c->ll_epoch, (double)c->bs_epoch, (double)c->uw_epoch};
+        if (nelems < 3) return set_err(-4, "need 3 elements");
+        CU(cudaMemcpy(d_dst, t, sizeof(t), cudaMemcpyHostToDevice));
         return 0;
     }
     if (!strcmp(which, "chain_wait")) {   // [0] = launches of the last look-ahead factorisation, then 6 doubles per launch

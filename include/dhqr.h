@@ -33,7 +33,8 @@
  *   - a handle is not thread-safe and its calls share one workspace: one handle per host thread, and
  *     consecutive calls on one handle must be on the same stream or ordered by the caller (events);
  *     the library does not order calls that arrive on different streams (the reference is not
- *     re-entrant either: Polyester @batch, S:203-206).
+ *     re-entrant either: Polyester @batch, S:203-206).  Results are bitwise independent of what the handle ran before and of
+ *     other handles at work on the same device (tests/test_gpu_history.py holds every entry point to this).
  *   - SPMD for multi-GPU: every rank (one process per GPU) makes the same call with its own
  *     column block (col0 = first global column, 0-based = the reference's LocalColumnBlock.dj, S:34).
  *   - storage format on return == the reference's (S:127-135): Householder vectors scaled to
@@ -102,13 +103,17 @@ int dhqr_destroy(dhqr_handle h);
  *                 stamps of its first CTA start and last warp end ("chain_wait": [0] = launches, then per launch unit,
  *                 stream (0 chain, 1 second apply, 2 side kernels), class index for dhqr_profile_get, event span, stamp
  *                 span, their difference, in ms; -1 for a launch without stamps)
+ *   "epoch_near_wrap" 1 (test hook, write-only): move the 32-bit launch-tag counters of the panel exchange cells (k_panel,
+ *                 k_tp_panel), the wavefront substitutions and the nb = 1 wave to two launches below their resets, so that a short
+ *                 test crosses the resets a long-lived handle meets after ~10^8 panel or ~4 x 10^9 wave launches.  Changes no result
+ *                 and nothing else; takes effect on tag buffers the handle already has (one allocated later starts over at 0)
  *   read-only:    "sms", "rank", "nranks", "panels_fast", "panels_fallback" (inner panels taken by either path; device-side
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
  *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64 and dhqr_qrcp_c64; device-side, read after synchronising),
  *                 "append_max_rows" (the largest k one dhqr_qr_append_f64 call takes on this device)
  *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
- *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys.
+ *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys (not "epoch_near_wrap").
  *   Any other key returns -2 (unknown option). */
 int dhqr_set_option(dhqr_handle h, const char *key, int64_t value);
 int dhqr_get_option(dhqr_handle h, const char *key, int64_t *value);
@@ -369,7 +374,8 @@ int dhqr_fill_uniform_f64(dhqr_handle h, uint64_t seed, int64_t i0, int64_t j0, 
 int dhqr_k_block_reflector_f64(dhqr_handle h, int64_t rows, int nbp, const double *dV, int64_t ldv,
                                int64_t row_lo, int ncols, double *dC, int64_t ldc, double *d_linv_out,
                                void *stream);
-/* Copy an internal workspace buffer ("wpart", "ybuf", "linv", "vbuf") to d_dst (debugging / tests). */
+/* Copy an internal workspace buffer ("wpart", "ybuf", "linv", "vbuf") to d_dst (debugging / tests).  "epochs": the three
+ * launch-tag counters (panel cells, wavefronts, nb = 1 wave) as doubles, copied synchronously. */
 int dhqr_debug_copy_f64(dhqr_handle h, const char *which, double *d_dst, int64_t nelems, void *stream);
 /* Panel kernel: factor the rows x ncols (ncols <= 32) panel at dP in place (reference recurrences
  * S:127-135 + S:208-209 restricted to the panel), alpha -> d_alpha[0:ncols]. */

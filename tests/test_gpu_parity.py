@@ -98,6 +98,10 @@ def test_option_keys(D):
         for key, (val, default) in SET_ONLY_OPTIONS.items():
             assert lib.dhqr_set_option(h.raw, key.encode(), val) == 0, key
             assert lib.dhqr_set_option(h.raw, key.encode(), default) == 0, key
+        # the tag-counter test hook (tests/test_gpu_history.py): write-only, value 1 only
+        assert lib.dhqr_set_option(h.raw, b"epoch_near_wrap", 1) == 0
+        assert lib.dhqr_set_option(h.raw, b"epoch_near_wrap", 0) == -3
+        assert lib.dhqr_get_option(h.raw, b"epoch_near_wrap", C.byref(v)) == -2 and v.value == -7
     finally:
         h.close()
 
