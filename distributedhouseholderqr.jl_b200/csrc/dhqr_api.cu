@@ -21,7 +21,6 @@
 #include "dhqr_wide.cuh"
 #include "dhqr_complex.cuh"
 #include "dhqr_qrcp.cuh"
-#include "dhqr_qrcp_c.cuh"
 #include "dhqr_append.cuh"
 
 using namespace dhqr;
@@ -2280,38 +2279,87 @@ int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int6
     return solve_adj_c64_local(c, (cudaStream_t)stream, m, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs);
 }
 
-// ---- QR with column pivoting (LAPACK dgeqp3 / dlaqps, dhqr_qrcp.cuh) -------------------------------------------------------
-// Panels of QP_NB columns, four launches per column, then the trailing update A[k0+32:, k0+32:] -= V F' through the 32-wide
-// C += V Y kernel.  A column whose norm downdate fails LAPACK's tol3z test is renormed exactly inside the panel, before the
-// next pivot is chosen, instead of ending the panel early: every panel has its static width and the host never needs a device
-// value, so the driver is one static loop and the call does not synchronise.  Single GPU, n <= m, no row limit.
+// ---- QR with column pivoting (LAPACK ?geqp3 / ?laqps, dhqr_qrcp.cuh), Float64 and ComplexF64 ---------------------------------
+// Panels of QP_NB columns, four launches per column, then the trailing update A[k0+32:, k0+32:] -= V F^H (qrcp_update).  A column
+// whose norm downdate fails LAPACK's tol3z test is renormed exactly inside the panel, before the next pivot is chosen, instead of
+// ending the panel early: every panel has its static width and the host never needs a device value, so the driver is one static
+// loop and the call does not synchronise.  Single GPU, n <= m, no row limit.  T = double or double2; the workspace is sized in
+// doubles, and every section of it that holds T is aligned for T.
 static int check_qrcp_ptr(const void* p, int arg, const char* name) {
     if (((uintptr_t)p & 7) != 0) return set_err(arg, "%s must be 8 B aligned", name);
     return 0;
 }
 
-static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double* A, int64_t lda, double* alpha, int64_t* jpvt) {
-    TRY(ensure_workspace(c, st, m, n));
+// Overloads and templates over the element type, which C linkage does not allow; the dhqr_* functions below keep the C linkage
+// of their declarations in dhqr.h.
+extern "C++" {
+
+// the alignment check of a pointer to T
+template <typename T>
+static int check_elem_ptr(const void* p, int arg, const char* name) {
+    return std::is_same<T, double>::value ? check_qrcp_ptr(p, arg, name) : check_c64_ptr(p, arg, name);
+}
+
+// the profile class of a launch: the Float64 kernel's name or the ComplexF64 one's
+template <typename T>
+static const char* qp_name(const char* f64, const char* c64) { return std::is_same<T, double>::value ? f64 : c64; }
+
+// A[c1:, c1:] -= V F' on the window starting at row k0 (a multiple of 32), rows >= c1 only: the 32-wide C += V Y with Y = -F'
+static int qrcp_update(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, int64_t k0, int kb, double* A, int64_t lda,
+                       const double* F, int64_t ldf) {
+    const int64_t c1 = k0 + kb, wrows = m - k0, vrows = rup(wrows, 128);
+    const int ncols = (int)(n - c1);
+    TRY(pack_v(c, st, A + k0 * lda + k0, lda, wrows, kb, 1, c->vpk2[0], 0, vrows, QP_NB));
+    const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * YT * LDK;
+    TRY(launch(c, st, "k_qrcp_ypack", 0.0, [&](CwtSlot) {
+        k_qrcp_ypack<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(F, ldf, c1, ncols, kb, c->ws[0].ypk);
+    }));
+    return launch_cvy(c, st, c->vpk2[0], 0, QP_NB, c->ws[0].ypk, wrows, kb, A + c1 * lda + k0, lda, ncols, 0);
+}
+
+// A[c1:, c1:] -= V F^H on the real view of the window starting at complex row k0, real rows >= 2 kb only: the real C += V^ Y^
+// through the 128-instantiation (64 real vectors: two k-chunks)
+static int qrcp_update(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, int64_t k0, int kb, double2* A, int64_t lda,
+                       const double2* F, int64_t ldf) {
+    const int64_t c1 = k0 + kb, mpc = m - k0, wrows = 2 * mpc, vrows = rup(wrows, 128);
+    const int ncols = (int)(n - c1);
+    TRY(launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) {
+        k_pack_c<<<dim3((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), 2 * QP_NB), 256, 0, st>>>(
+            A + k0 * lda + k0, lda, mpc, kb, c->vpk2[0], 0, vrows);
+    }));
+    const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * QPC_NKQ * YT * LDK;
+    TRY(launch(c, st, "k_qrcp_ypack_c", 0.0, [&](CwtSlot) {
+        k_qrcp_ypack_c<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(F, ldf, c1, ncols, kb, c->ws[0].ypk);
+    }));
+    return launch_cvy(c, st, c->vpk2[0], 0, 2 * QP_NB, c->ws[0].ypk, wrows, 2 * kb, (double*)(A + c1 * lda + k0), 2 * lda, ncols, 0);
+}
+
+template <typename T>
+static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, T* A, int64_t lda, T* alpha, int64_t* jpvt) {
+    constexpr int w = sizeof(T) / sizeof(double);                                      // doubles per element
+    TRY(ensure_workspace(c, st, w * m, n));
     const int64_t p1 = (m + QP_PROWS - 1) / QP_PROWS;                                    // k_qrcp_pivot CTAs
     const int64_t smax = std::max<int64_t>(1, std::min<int64_t>((m + QP_THREADS - 1) / QP_THREADS, 8 * c->sms));
-    const size_t need = (size_t)2 * n + (size_t)QP_NB * n + (size_t)m + (size_t)p1 + (size_t)smax * n;
+    // in doubles: vn1, vn2 (real); F, x, the pivot partials (real, padded to keep what follows aligned for T) and the GEMV partials
+    const size_t need = (size_t)2 * n + (size_t)w * QP_NB * n + (size_t)w * m + (size_t)rup(p1, w) + (size_t)w * smax * n;
     TRY(c->qp_buf.ensure(need, st));
     TRY(c->qp_flag.ensure((size_t)n, st));
     TRY(c->qp_ctl.ensure(1, st));
-    QrcpArgs a;
+    QrcpArgs<T> a;
     a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
-    a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = a.vn2 + n; a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
-    a.part1 = a.x + m; a.part2 = a.part1 + p1; a.ldp = n;
-    TRY(launch(c, st, "k_qrcp_init", 8.0 * (double)m * n, [&](CwtSlot) {
-        k_qrcp_init<<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
+    a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = (T*)(a.vn2 + n); a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
+    a.part1 = (double*)(a.x + m); a.part2 = (T*)(a.part1 + rup(p1, w)); a.ldp = n;
+    TRY(launch(c, st, qp_name<T>("k_qrcp_init", "k_qrcp_init_c"), (double)sizeof(T) * (double)m * n, [&](CwtSlot) {
+        k_qrcp_init<T><<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
     }));
     for (int64_t k0 = 0; k0 < n; k0 += QP_NB) {
         const int kb = (int)std::min<int64_t>(QP_NB, n - k0);
-        const int tiles = (int)((n - k0 + QP_GCOLS - 1) / QP_GCOLS);
+        const int tiles = (int)((n - k0 + QP_GCOLS<T> - 1) / QP_GCOLS<T>);
         for (int jj = 0; jj < kb; ++jj) {
             const int64_t j = k0 + jj, rows = m - j;
             a.j = j; a.k0 = k0; a.jj = jj;
-            TRY(launch(c, st, "k_qrcp_pivot", 8.0 * ((double)m * 4 + (double)rows * (jj + 1) + (double)(n - j)), [&](CwtSlot) {
+            TRY(launch(c, st, qp_name<T>("k_qrcp_pivot", "k_qrcp_pivot_c"),
+                       32.0 * (double)m + (double)sizeof(T) * (double)rows * (jj + 1) + 8.0 * (double)(n - j), [&](CwtSlot) {
                 k_qrcp_pivot<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
             }));
             // row splits: about eight CTAs per SM in all, at least QP_THREADS rows each
@@ -2319,50 +2367,42 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, do
                                                                      (8 * (int64_t)c->sms + tiles - 1) / tiles));
             a.split_rows = rup((rows + s - 1) / s, QP_THREADS);
             a.nsplit = (int)((rows + a.split_rows - 1) / a.split_rows);
-            TRY(launch(c, st, "k_qrcp_gemv", 8.0 * (double)rows * (double)(n - k0), [&](CwtSlot) {
+            TRY(launch(c, st, qp_name<T>("k_qrcp_gemv", "k_qrcp_gemv_c"), (double)sizeof(T) * (double)rows * (double)(n - k0), [&](CwtSlot) {
                 k_qrcp_gemv<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
             }));
             if (j + 1 >= n) continue;
-            TRY(launch(c, st, "k_qrcp_finish", 0.0, [&](CwtSlot) {
+            TRY(launch(c, st, qp_name<T>("k_qrcp_finish", "k_qrcp_finish_c"), 0.0, [&](CwtSlot) {
                 k_qrcp_finish<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
             }));
-            TRY(launch(c, st, "k_qrcp_renorm", 0.0, [&](CwtSlot) {
+            TRY(launch(c, st, qp_name<T>("k_qrcp_renorm", "k_qrcp_renorm_c"), 0.0, [&](CwtSlot) {
                 k_qrcp_renorm<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
             }));
         }
-        const int64_t c1 = k0 + kb;
-        if (c1 >= n) break;
-        // A[c1:, c1:] -= V F'  on the window starting at row k0 (a multiple of 32), rows >= c1 only
-        const int64_t wrows = m - k0, vrows = rup(wrows, 128);
-        const int ncols = (int)(n - c1);
-        TRY(pack_v(c, st, A + k0 * lda + k0, lda, wrows, kb, 1, c->vpk2[0], 0, vrows, QP_NB));
-        const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * YT * LDK;
-        TRY(launch(c, st, "k_qrcp_ypack", 0.0, [&](CwtSlot) {
-            k_qrcp_ypack<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(a.F, a.ldf, c1, ncols, kb, c->ws[0].ypk);
-        }));
-        TRY(launch_cvy(c, st, c->vpk2[0], 0, QP_NB, c->ws[0].ypk, wrows, kb, A + c1 * lda + k0, lda, ncols, 0));
+        if (k0 + kb >= n) break;
+        TRY(qrcp_update(c, st, m, n, k0, kb, A, lda, a.F, a.ldf));
     }
     return 0;
 }
 
-int dhqr_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, double* dA, int64_t lda, double* d_alpha, int64_t* d_jpvt, void* stream) {
+template <typename T>
+static int qrcp_factor(dhqr_context* c, int64_t m, int64_t n, void* dA, int64_t lda, void* d_alpha, int64_t* d_jpvt, void* stream) {
     if (!c) return set_err(-1, "null handle");
     if (c->nranks != 1) return set_err(-1, "the pivoted factorisation is single-GPU (the handle has %d ranks)", c->nranks);
     if (m < 0) return set_err(-2, "m < 0");
     if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
     if (n > 0 && !dA) return set_err(-4, "null A");
-    TRY(check_qrcp_ptr(dA, -4, "A"));
+    TRY(check_elem_ptr<T>(dA, -4, "A"));
     if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
     if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
-    TRY(check_qrcp_ptr(d_alpha, -6, "alpha"));
+    TRY(check_elem_ptr<T>(d_alpha, -6, "alpha"));
     if (n > 0 && !d_jpvt) return set_err(-7, "null jpvt");
     TRY(check_qrcp_ptr(d_jpvt, -7, "jpvt"));
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
-    return qrcp_local(c, (cudaStream_t)stream, m, n, dA, lda, d_alpha, d_jpvt);
+    return qrcp_local(c, (cudaStream_t)stream, m, n, (T*)dA, lda, (T*)d_alpha, d_jpvt);
 }
 
-// (Q'b)[0:rank]: the first `rank` reflectors of a pivoted factorisation on b, the first stage of both pivoted solves
+// (Q^H b)[0:rank]: the first `rank` reflectors of a pivoted factorisation on b, the first stage of both pivoted solves
 static int qrcp_qtb(dhqr_context* c, cudaStream_t st, int64_t m, int64_t rank, const double* dA, int64_t lda, double* d_b, int64_t ldb,
                     int nrhs) {
     if (qt_vec_ok(c, m, nrhs)) {
@@ -2372,84 +2412,129 @@ static int qrcp_qtb(dhqr_context* c, cudaStream_t st, int64_t m, int64_t rank, c
     return apply_qt_local(c, st, m, 0, rank, dA, lda, d_b, ldb, nrhs);
 }
 
+static int qrcp_qtb(dhqr_context* c, cudaStream_t st, int64_t m, int64_t rank, const double2* A, int64_t lda, double2* b, int64_t ldb,
+                    int nrhs) {
+    return apply_qt_c64_local(c, st, m, rank, A, lda, b, ldb, nrhs);
+}
+
+// z = R11^{-1} b[0:rank] of the basic solution
+static int qrcp_backsolve(dhqr_context* c, cudaStream_t st, int64_t rank, const double* A, int64_t lda, const double* alpha, double* b,
+                          int64_t ldb, int nrhs, double* z) {
+    TRY(wave_prepare(c, st, rank));
+    return backsolve_local(c, st, 0, rank, A, lda, alpha, b, ldb, nrhs, z, rank);
+}
+
+static int qrcp_backsolve(dhqr_context* c, cudaStream_t st, int64_t rank, const double2* A, int64_t lda, const double2* alpha, double2* b,
+                          int64_t ldb, int nrhs, double2* z) {
+    return backsolve_c64_local(c, st, rank, A, lda, alpha, b, ldb, nrhs, z, rank);
+}
+
 // b[jpvt[i]] = z[i] for i < rank, 0 for rank <= i < n, on every right-hand side; jpvt entries outside [0, n) are skipped
-static int qrcp_scatter(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double* z, int64_t ldz, const int64_t* d_jpvt,
-                        double* d_b, int64_t ldb, int nrhs) {
+template <typename T>
+static int qrcp_scatter(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const T* z, int64_t ldz, const int64_t* d_jpvt,
+                        T* d_b, int64_t ldb, int nrhs) {
     for (int r0 = 0; r0 < nrhs; r0 += 65535) {
         const int nr = std::min(nrhs - r0, 65535);
-        TRY(launch(c, st, "k_qrcp_scatter", 0.0, [&](CwtSlot) {
-            k_qrcp_scatter<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(z + (size_t)r0 * ldz, ldz, d_jpvt, n, rank,
-                                                                                         d_b + (size_t)r0 * ldb, ldb);
+        TRY(launch(c, st, qp_name<T>("k_qrcp_scatter", "k_qrcp_scatter_c"), 0.0, [&](CwtSlot) {
+            k_qrcp_scatter<T><<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(z + (size_t)r0 * ldz, ldz, d_jpvt, n, rank,
+                                                                                            d_b + (size_t)r0 * ldb, ldb);
         }));
     }
     return 0;
 }
 
-int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha,
-                        const int64_t* d_jpvt, double* d_b, int64_t ldb, int nrhs, void* stream) {
+template <typename T>
+static int qrcp_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha,
+                      const int64_t* d_jpvt, void* d_b, int64_t ldb, int nrhs, void* stream) {
     if (!c) return set_err(-1, "null handle");
     if (c->nranks != 1) return set_err(-1, "the pivoted solve is single-GPU (the handle has %d ranks)", c->nranks);
     if (m < 0) return set_err(-2, "m < 0");
     if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
     if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
     if (n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_qrcp_ptr(dA, -5, "A"));
+    TRY(check_elem_ptr<T>(dA, -5, "A"));
     if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
     if (n > 0 && !d_alpha) return set_err(-7, "null alpha");
-    TRY(check_qrcp_ptr(d_alpha, -7, "alpha"));
+    TRY(check_elem_ptr<T>(d_alpha, -7, "alpha"));
     if (n > 0 && !d_jpvt) return set_err(-8, "null jpvt");
     TRY(check_qrcp_ptr(d_jpvt, -8, "jpvt"));
     if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    TRY(check_qrcp_ptr(d_b, -9, "b"));
+    TRY(check_elem_ptr<T>(d_b, -9, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
     if (nrhs < 0) return set_err(-11, "nrhs < 0");
     if (n == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
-    TRY(c->xbuf.ensure((size_t)n * nrhs, st));
+    constexpr int w = sizeof(T) / sizeof(double);
+    TRY(ensure_workspace(c, st, w * m, std::max<int64_t>(n, nrhs)));
+    TRY(c->xbuf.ensure((size_t)w * n * nrhs, st));
+    const T* A = (const T*)dA;
+    T* b = (T*)d_b;
+    T* z = (T*)c->xbuf.p;
     if (rank > 0) {
-        TRY(qrcp_qtb(c, st, m, rank, dA, lda, d_b, ldb, nrhs));
-        TRY(wave_prepare(c, st, rank));
-        TRY(backsolve_local(c, st, 0, rank, dA, lda, d_alpha, d_b, ldb, nrhs, c->xbuf, rank));
+        TRY(qrcp_qtb(c, st, m, rank, A, lda, b, ldb, nrhs));
+        TRY(qrcp_backsolve(c, st, rank, A, lda, (const T*)d_alpha, b, ldb, nrhs, z));
     }
-    return qrcp_scatter(c, st, n, rank, c->xbuf, rank, d_jpvt, d_b, ldb, nrhs);
+    return qrcp_scatter(c, st, n, rank, z, rank, d_jpvt, b, ldb, nrhs);
 }
 
-// ---- complete orthogonal decomposition on the pivoted QR (DESIGN §2.8) -------------------------------------------------------
-// A P = Q R at rank r: R_r = R[0:r, 0:n] (r x n, upper trapezoidal), and its transpose factored by the unpivoted QR, R_r' = Z [U; 0],
-// gives A P ~ Q1 [U' 0] Z'.  The minimum-norm solution of the rank-r problem is x = P Z [U^{-T} (Q'b)[0:r]; 0], and the step after
-// Q'b is exactly the minimum-norm solution of R_r y = c that dhqr_solve_adj_f64 computes from the factorisation (F, gamma) of R_r'.
+}  // extern "C++"
+
+int dhqr_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, double* dA, int64_t lda, double* d_alpha, int64_t* d_jpvt, void* stream) {
+    return qrcp_factor<double>(c, m, n, dA, lda, d_alpha, d_jpvt, stream);
+}
+
+int dhqr_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, void* dA, int64_t lda, void* d_alpha, int64_t* d_jpvt, void* stream) {
+    return qrcp_factor<double2>(c, m, n, dA, lda, d_alpha, d_jpvt, stream);
+}
+
+int dhqr_solve_qrcp_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha,
+                        const int64_t* d_jpvt, double* d_b, int64_t ldb, int nrhs, void* stream) {
+    return qrcp_solve<double>(c, m, n, rank, dA, lda, d_alpha, d_jpvt, d_b, ldb, nrhs, stream);
+}
+
+int dhqr_solve_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha,
+                        const int64_t* d_jpvt, void* d_b, int64_t ldb, int nrhs, void* stream) {
+    return qrcp_solve<double2>(c, m, n, rank, dA, lda, d_alpha, d_jpvt, d_b, ldb, nrhs, stream);
+}
+
+// ---- complete orthogonal decomposition on the pivoted QR (DESIGN §2.8, §2.9) ------------------------------------------------
+// A P = Q R at rank r: R_r = R[0:r, 0:n] (r x n, upper trapezoidal), and its adjoint factored by the unpivoted QR, R_r^H = Z [U; 0],
+// gives A P ~ Q1 [U^H 0] Z^H.  The minimum-norm solution of the rank-r problem is x = P Z [U^{-H} (Q^H b)[0:r]; 0], and the step
+// after Q^H b is exactly the minimum-norm solution of R_r y = c that dhqr_solve_adj_* computes from the factorisation (F, gamma) of
+// R_r^H.
 static bool spans_overlap(const void* p, size_t pbytes, const void* q, size_t qbytes) {
     const uintptr_t p0 = (uintptr_t)p, q0 = (uintptr_t)q;
     return pbytes > 0 && qbytes > 0 && p0 < q0 + qbytes && q0 < p0 + pbytes;
 }
 
+extern "C++" {   // as for the pivoted QR above
+
 // Arguments 1-10, which both entry points share but for the 7th: alpha (dhqr_cod_*, factor = true) or jpvt (dhqr_solve_cod_*).
-// cplx: the _c64 twins, whose A, alpha, F and gamma are ComplexF64 (16 B aligned, 16 B elements) and have no row limit.
+// Only the Float64 factorisation has a row limit: the ComplexF64 unpivoted path has none.
+template <typename T>
 static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* seventh,
-                     const void* dF, int64_t ldf, const void* d_gamma, bool factor, bool cplx = false) {
-    auto check_ptr = [cplx](const void* p, int arg, const char* name) { return cplx ? check_c64_ptr(p, arg, name) : check_qrcp_ptr(p, arg, name); };
-    const size_t esz = cplx ? 16 : 8;
+                     const void* dF, int64_t ldf, const void* d_gamma, bool factor) {
+    const size_t esz = sizeof(T);
     if (!c) return set_err(-1, "null handle");
     if (c->nranks != 1) return set_err(-1, "the complete orthogonal decomposition is single-GPU (the handle has %d ranks)", c->nranks);
     if (m < 0) return set_err(-2, "m < 0");
     if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (factor && !cplx && n > narrow_panel_max_rows(c))               // R_r' has n rows and goes through the unpivoted path
+    if (factor && std::is_same<T, double>::value && n > narrow_panel_max_rows(c))   // R_r' has n rows and goes through the unpivoted path
         return set_err(-3, "n = %lld exceeds the row limit of the unpivoted factorisation (%lld)", (long long)n,
                        (long long)narrow_panel_max_rows(c));
     if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
     if (n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_ptr(dA, -5, "A"));
+    TRY(check_elem_ptr<T>(dA, -5, "A"));
     if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
     const char* name7 = factor ? "alpha" : "jpvt";
     if (n > 0 && !seventh) return set_err(-7, "null %s", name7);
-    TRY(factor ? check_ptr(seventh, -7, name7) : check_qrcp_ptr(seventh, -7, name7));
+    TRY(factor ? check_elem_ptr<T>(seventh, -7, name7) : check_qrcp_ptr(seventh, -7, name7));
     if (rank > 0 && !dF) return set_err(-8, "null F");
-    TRY(check_ptr(dF, -8, "F"));
+    TRY(check_elem_ptr<T>(dF, -8, "F"));
     if (ldf < std::max<int64_t>(1, n)) return set_err(-9, "ldf < max(1,n)");
     if (rank > 0 && !d_gamma) return set_err(-10, "null gamma");
-    TRY(check_ptr(d_gamma, -10, "gamma"));
+    TRY(check_elem_ptr<T>(d_gamma, -10, "gamma"));
     if (factor && rank > 0) {                                          // F and gamma are written: neither may overlap an input
         const size_t abytes = ((size_t)(n - 1) * lda + m) * esz, alphabytes = (size_t)n * esz;
         const size_t fbytes = ((size_t)(rank - 1) * ldf + n) * esz, gbytes = (size_t)rank * esz;
@@ -2462,200 +2547,85 @@ static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const 
     return 0;
 }
 
-int dhqr_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha, double* dF,
-                 int64_t ldf, double* d_gamma, void* stream) {
-    TRY(check_cod(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, true));
+// (F, gamma) <- the unpivoted factorisation of R_r^H (n x rank) in place
+static int qr_rrh(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, double* F, int64_t ldf, double* gamma) {
+    return qr_blocked(c, st, n, rank, 0, rank, F, ldf, gamma, c->nb);     // what dhqr_qr_f64 runs for nb = 0
+}
+
+static int qr_rrh(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, double2* F, int64_t ldf, double2* gamma) {
+    return qr_c64_local(c, st, n, rank, F, ldf, gamma);                  // the body of dhqr_qr_c64
+}
+
+template <typename T>
+static int cod_factor(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha, void* dF,
+                      int64_t ldf, void* d_gamma, void* stream) {
+    TRY(check_cod<T>(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, true));
     if (n == 0 || rank == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(launch(c, st, "k_cod_pack", 8.0 * (double)n * rank, [&](CwtSlot) {
-        k_cod_pack<<<dim3((unsigned)((n + CP_TILE - 1) / CP_TILE), (unsigned)((rank + CP_TILE - 1) / CP_TILE)), dim3(CP_TILE, CP_ROWS), 0,
-                     st>>>(dA, lda, d_alpha, n, rank, dF, ldf);
+    TRY(launch(c, st, qp_name<T>("k_cod_pack", "k_cod_pack_c"), (double)sizeof(T) * (double)n * rank, [&](CwtSlot) {
+        k_cod_pack<T><<<dim3((unsigned)((n + CP_TILE - 1) / CP_TILE), (unsigned)((rank + CP_TILE - 1) / CP_TILE)), dim3(CP_TILE, CP_ROWS), 0,
+                        st>>>((const T*)dA, lda, (const T*)d_alpha, n, rank, (T*)dF, ldf);
     }));
-    return qr_blocked(c, st, n, rank, 0, rank, dF, ldf, d_gamma, c->nb);   // what dhqr_qr_f64 runs for nb = 0
+    return qr_rrh(c, st, n, rank, (T*)dF, ldf, (T*)d_gamma);
 }
 
-int dhqr_solve_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const int64_t* d_jpvt,
-                       const double* dF, int64_t ldf, const double* d_gamma, double* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_cod(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, false));
+// b[0:n] <- Z [U^{-H} b[0:rank]; 0] from the factorisation (F, gamma) of R_r^H, rows n..m-1 of b untouched
+static int cod_adj(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double* F, int64_t ldf, const double* gamma,
+                   double* b, int64_t ldb, int nrhs) {
+    return solve_adj_local(c, st, n, rank, F, ldf, gamma, b, ldb, nrhs);
+}
+
+static int cod_adj(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double2* F, int64_t ldf, const double2* gamma,
+                   double2* b, int64_t ldb, int nrhs) {
+    return solve_adj_c64_local(c, st, n, rank, F, ldf, gamma, b, ldb, nrhs);
+}
+
+template <typename T>
+static int cod_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const int64_t* d_jpvt,
+                     const void* dF, int64_t ldf, const void* d_gamma, void* d_b, int64_t ldb, int nrhs, void* stream) {
+    TRY(check_cod<T>(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, false));
     if (nrhs > 0 && !d_b) return set_err(-11, "null b");
-    TRY(check_qrcp_ptr(d_b, -11, "b"));
+    TRY(check_elem_ptr<T>(d_b, -11, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-12, "ldb < max(1,m)");
     if (nrhs < 0) return set_err(-13, "nrhs < 0");
     if (n == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
-    TRY(c->xbuf.ensure((size_t)n * nrhs, st));
+    constexpr int w = sizeof(T) / sizeof(double);
+    TRY(ensure_workspace(c, st, w * m, std::max<int64_t>(n, nrhs)));
+    TRY(c->xbuf.ensure((size_t)w * n * nrhs, st));
+    T* b = (T*)d_b;
+    T* z = (T*)c->xbuf.p;
     if (rank > 0) {
-        TRY(qrcp_qtb(c, st, m, rank, dA, lda, d_b, ldb, nrhs));
-        // b[0:n] <- Z [U^{-T} b[0:rank]; 0], rows n..m-1 untouched; then into xbuf, which the scatter reads while it writes b
-        TRY(solve_adj_local(c, st, n, rank, dF, ldf, d_gamma, d_b, ldb, nrhs));
-        CU(cudaMemcpy2DAsync(c->xbuf, (size_t)n * 8, d_b, (size_t)ldb * 8, (size_t)n * 8, nrhs, cudaMemcpyDeviceToDevice, st));
+        TRY(qrcp_qtb(c, st, m, rank, (const T*)dA, lda, b, ldb, nrhs));
+        // b[0:n] <- Z [U^{-H} b[0:rank]; 0]; then into xbuf, which the scatter reads while it writes b
+        TRY(cod_adj(c, st, n, rank, (const T*)dF, ldf, (const T*)d_gamma, b, ldb, nrhs));
+        CU(cudaMemcpy2DAsync(z, (size_t)n * sizeof(T), b, (size_t)ldb * sizeof(T), (size_t)n * sizeof(T), nrhs, cudaMemcpyDeviceToDevice, st));
     }
-    return qrcp_scatter(c, st, n, rank > 0 ? n : 0, c->xbuf, n, d_jpvt, d_b, ldb, nrhs);
+    return qrcp_scatter(c, st, n, rank > 0 ? n : 0, z, n, d_jpvt, b, ldb, nrhs);
 }
 
-// ---- ComplexF64 QR with column pivoting and the complete orthogonal decomposition on it (DESIGN §2.9, dhqr_qrcp_c.cuh) ---------
-// The scheme of dhqr_qrcp_f64 in complex arithmetic, in the library's complex storage format; the trailing update after each panel is
-// the real C += V^ Y^ on the real view through the 128-instantiation (64 real vectors: two k-chunks).  Single GPU, n <= m, no row
-// limit, no synchronisation.
-static int qrcp_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double2* A, int64_t lda, double2* alpha, int64_t* jpvt) {
-    TRY(ensure_workspace(c, st, 2 * m, n));
-    const int64_t p1 = (m + QP_PROWS - 1) / QP_PROWS;                                    // k_qrcp_pivot_c CTAs
-    const int64_t smax = std::max<int64_t>(1, std::min<int64_t>((m + QP_THREADS - 1) / QP_THREADS, 8 * c->sms));
-    // in doubles: vn1, vn2 (real); F, x, the pivot partials (real, padded to keep what follows 16 B aligned) and the GEMV partials
-    const size_t need = (size_t)2 * n + (size_t)2 * QP_NB * n + (size_t)2 * m + (size_t)rup(p1, 2) + (size_t)2 * smax * n;
-    TRY(c->qp_buf.ensure(need, st));
-    TRY(c->qp_flag.ensure((size_t)n, st));
-    TRY(c->qp_ctl.ensure(1, st));
-    QrcpArgsC a;
-    a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
-    a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = (double2*)(a.vn2 + n); a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
-    a.part1 = (double*)(a.x + m); a.part2 = (double2*)(a.part1 + rup(p1, 2)); a.ldp = n;
-    TRY(launch(c, st, "k_qrcp_init_c", 16.0 * (double)m * n, [&](CwtSlot) {
-        k_qrcp_init_c<<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
-    }));
-    for (int64_t k0 = 0; k0 < n; k0 += QP_NB) {
-        const int kb = (int)std::min<int64_t>(QP_NB, n - k0);
-        const int tiles = (int)((n - k0 + QPC_GCOLS - 1) / QPC_GCOLS);
-        for (int jj = 0; jj < kb; ++jj) {
-            const int64_t j = k0 + jj, rows = m - j;
-            a.j = j; a.k0 = k0; a.jj = jj;
-            TRY(launch(c, st, "k_qrcp_pivot_c", 16.0 * ((double)m * 2 + (double)rows * (jj + 1)) + 8.0 * (double)(n - j), [&](CwtSlot) {
-                k_qrcp_pivot_c<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
-            }));
-            // row splits: about eight CTAs per SM in all, at least QP_THREADS rows each
-            const int64_t s = std::max<int64_t>(1, std::min<int64_t>((rows + QP_THREADS - 1) / QP_THREADS,
-                                                                     (8 * (int64_t)c->sms + tiles - 1) / tiles));
-            a.split_rows = rup((rows + s - 1) / s, QP_THREADS);
-            a.nsplit = (int)((rows + a.split_rows - 1) / a.split_rows);
-            TRY(launch(c, st, "k_qrcp_gemv_c", 16.0 * (double)rows * (double)(n - k0), [&](CwtSlot) {
-                k_qrcp_gemv_c<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
-            }));
-            if (j + 1 >= n) continue;
-            TRY(launch(c, st, "k_qrcp_finish_c", 0.0, [&](CwtSlot) {
-                k_qrcp_finish_c<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
-            }));
-            TRY(launch(c, st, "k_qrcp_renorm_c", 0.0, [&](CwtSlot) {
-                k_qrcp_renorm_c<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
-            }));
-        }
-        const int64_t c1 = k0 + kb;
-        if (c1 >= n) break;
-        // A[c1:, c1:] -= V F^H on the real view of the window starting at complex row k0, real rows >= 2 kb only
-        const int64_t mpc = m - k0, wrows = 2 * mpc, vrows = rup(wrows, 128);
-        const int ncols = (int)(n - c1);
-        TRY(launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) {
-            k_pack_c<<<dim3((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), 2 * QP_NB), 256, 0, st>>>(
-                A + k0 * lda + k0, lda, mpc, kb, c->vpk2[0], 0, vrows);
-        }));
-        const int64_t ytot = (int64_t)((ncols + YT - 1) / YT) * QPC_NKQ * YT * LDK;
-        TRY(launch(c, st, "k_qrcp_ypack_c", 0.0, [&](CwtSlot) {
-            k_qrcp_ypack_c<<<(unsigned)((ytot + 255) / 256), 256, 0, st>>>(a.F, a.ldf, c1, ncols, kb, c->ws[0].ypk);
-        }));
-        TRY(launch_cvy(c, st, c->vpk2[0], 0, 2 * QP_NB, c->ws[0].ypk, wrows, 2 * kb, (double*)(A + c1 * lda + k0), 2 * lda, ncols, 0));
-    }
-    return 0;
-}
+}  // extern "C++"
 
-int dhqr_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, void* dA, int64_t lda, void* d_alpha, int64_t* d_jpvt, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the pivoted factorisation is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (n > 0 && !dA) return set_err(-4, "null A");
-    TRY(check_c64_ptr(dA, -4, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
-    if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
-    TRY(check_c64_ptr(d_alpha, -6, "alpha"));
-    if (n > 0 && !d_jpvt) return set_err(-7, "null jpvt");
-    TRY(check_qrcp_ptr(d_jpvt, -7, "jpvt"));
-    if (n == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    return qrcp_c64_local(c, (cudaStream_t)stream, m, n, (double2*)dA, lda, (double2*)d_alpha, d_jpvt);
-}
-
-// complex twin of qrcp_scatter
-static int qrcp_scatter_c(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double2* z, int64_t ldz, const int64_t* d_jpvt,
-                          double2* d_b, int64_t ldb, int nrhs) {
-    for (int r0 = 0; r0 < nrhs; r0 += 65535) {
-        const int nr = std::min(nrhs - r0, 65535);
-        TRY(launch(c, st, "k_qrcp_scatter_c", 0.0, [&](CwtSlot) {
-            k_qrcp_scatter_c<<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(z + (size_t)r0 * ldz, ldz, d_jpvt, n, rank,
-                                                                                           d_b + (size_t)r0 * ldb, ldb);
-        }));
-    }
-    return 0;
-}
-
-int dhqr_solve_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha,
-                        const int64_t* d_jpvt, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the pivoted solve is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
-    if (n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_c64_ptr(dA, -5, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
-    if (n > 0 && !d_alpha) return set_err(-7, "null alpha");
-    TRY(check_c64_ptr(d_alpha, -7, "alpha"));
-    if (n > 0 && !d_jpvt) return set_err(-8, "null jpvt");
-    TRY(check_qrcp_ptr(d_jpvt, -8, "jpvt"));
-    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    TRY(check_c64_ptr(d_b, -9, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
-    if (nrhs < 0) return set_err(-11, "nrhs < 0");
-    if (n == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
-    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
-    const double2* A = (const double2*)dA;
-    double2* b = (double2*)d_b;
-    double2* x = (double2*)c->xbuf.p;
-    if (rank > 0) {
-        TRY(apply_qt_c64_local(c, st, m, rank, A, lda, b, ldb, nrhs));
-        TRY(backsolve_c64_local(c, st, rank, A, lda, (const double2*)d_alpha, b, ldb, nrhs, x, rank));
-    }
-    return qrcp_scatter_c(c, st, n, rank, x, rank, d_jpvt, b, ldb, nrhs);
+int dhqr_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const double* d_alpha, double* dF,
+                 int64_t ldf, double* d_gamma, void* stream) {
+    return cod_factor<double>(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, stream);
 }
 
 int dhqr_cod_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha, void* dF,
                  int64_t ldf, void* d_gamma, void* stream) {
-    TRY(check_cod(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, true, true));
-    if (n == 0 || rank == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    TRY(launch(c, st, "k_cod_pack_c", 16.0 * (double)n * rank, [&](CwtSlot) {
-        k_cod_pack_c<<<dim3((unsigned)((n + CP_TILE - 1) / CP_TILE), (unsigned)((rank + CP_TILE - 1) / CP_TILE)), dim3(CP_TILE, CP_ROWS), 0,
-                       st>>>((const double2*)dA, lda, (const double2*)d_alpha, n, rank, (double2*)dF, ldf);
-    }));
-    return qr_c64_local(c, st, n, rank, (double2*)dF, ldf, (double2*)d_gamma);      // the body of dhqr_qr_c64
+    return cod_factor<double2>(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, stream);
+}
+
+int dhqr_solve_cod_f64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const double* dA, int64_t lda, const int64_t* d_jpvt,
+                       const double* dF, int64_t ldf, const double* d_gamma, double* d_b, int64_t ldb, int nrhs, void* stream) {
+    return cod_solve<double>(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, d_b, ldb, nrhs, stream);
 }
 
 int dhqr_solve_cod_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const int64_t* d_jpvt,
                        const void* dF, int64_t ldf, const void* d_gamma, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_cod(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, false, true));
-    if (nrhs > 0 && !d_b) return set_err(-11, "null b");
-    TRY(check_c64_ptr(d_b, -11, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-12, "ldb < max(1,m)");
-    if (nrhs < 0) return set_err(-13, "nrhs < 0");
-    if (n == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
-    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
-    double2* b = (double2*)d_b;
-    double2* x = (double2*)c->xbuf.p;
-    if (rank > 0) {
-        TRY(apply_qt_c64_local(c, st, m, rank, (const double2*)dA, lda, b, ldb, nrhs));
-        // b[0:n] <- Z [U^{-H} b[0:rank]; 0], rows n..m-1 untouched; then into xbuf, which the scatter reads while it writes b
-        TRY(solve_adj_c64_local(c, st, n, rank, (const double2*)dF, ldf, (const double2*)d_gamma, b, ldb, nrhs));
-        CU(cudaMemcpy2DAsync(x, (size_t)n * 16, b, (size_t)ldb * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
-    }
-    return qrcp_scatter_c(c, st, n, rank > 0 ? n : 0, x, n, d_jpvt, b, ldb, nrhs);
+    return cod_solve<double2>(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, d_b, ldb, nrhs, stream);
 }
 
 // ---- triangular-pentagonal QR: fold new rows into a factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10 ---------------------

@@ -35,9 +35,28 @@ __device__ __forceinline__ double2 block_sum2(double2 v, double2* red, int tid, 
 // sin(pi) in Float64 (Julia's sin(pi), numpy's np.sin(np.pi)): written out rather than left to the device sin
 constexpr double SIN_PI = 1.2246467991473532e-16;
 
-// S:129-135 for one complex column (one CTA): s = |x|, alpha = -exp(i angle(x0)) s  (S:9), f = 1 / sqrt(s (s + |x0|)),
-// x0 -= alpha, x *= f.  angle = atan2(im, re) sees the signs of a zero pivot: angle(+0 +- 0i) = +-0 gives alpha = -s,
-// angle(-0 +- 0i) = +-pi gives alpha = -s (cos pi, +-sin pi) = s (1, -+1.2246e-16).
+// alpha = -exp(i angle(x0)) s  (S:9) of the reflector of a complex column with leading entry x0 and norm s, and a0 = |x0| for its
+// scale f = 1 / sqrt(s (s + |x0|)).  angle = atan2(im, re) sees the signs of a zero pivot: angle(+0 +- 0i) = +-0 gives
+// alpha = -s, angle(-0 +- 0i) = +-pi gives alpha = -s (cos pi, +-sin pi) = s (1, -+1.2246e-16).  Shared by k_house1_c and the
+// pivoted factorisation (dhqr_qrcp.cuh), so both write the same storage format.
+__device__ __forceinline__ double2 house_alpha(double2 x0, double s, double& a0) {
+    a0 = hypot(x0.x, x0.y);
+    // -exp(i angle(x0)) = -(x0 / |x0|); exp(i angle(x0)) = (cos, sin) of +-0 or +-pi for a zero x0
+    double ux, uy;
+    if (a0 > 0.0) {
+        ux = x0.x / a0;
+        uy = x0.y / a0;
+    } else if (!signbit(x0.x)) {
+        ux = 1.0;
+        uy = x0.y;
+    } else {
+        ux = -1.0;
+        uy = copysign(SIN_PI, x0.y);
+    }
+    return make_double2(-ux * s, -uy * s);
+}
+
+// S:129-135 for one complex column (one CTA): s = |x|, alpha (house_alpha), f = 1 / sqrt(s (s + |x0|)), x0 -= alpha, x *= f
 __global__ void __launch_bounds__(1024, 1) k_house1_c(double2* __restrict__ col, int64_t len, double2* __restrict__ alpha) {
     __shared__ double2 red[32];
     __shared__ double sc[3];
@@ -51,20 +70,8 @@ __global__ void __launch_bounds__(1024, 1) k_house1_c(double2* __restrict__ col,
     if (tid == 0) {
         const double2 x0 = col[0];
         const double s = sqrt(acc.x);
-        const double a0 = hypot(x0.x, x0.y);
-        // -exp(i angle(x0)) = -(x0 / |x0|); exp(i angle(x0)) = (cos, sin) of +-0 or +-pi for a zero x0
-        double ux, uy;
-        if (a0 > 0.0) {
-            ux = x0.x / a0;
-            uy = x0.y / a0;
-        } else if (!signbit(x0.x)) {
-            ux = 1.0;
-            uy = x0.y;
-        } else {
-            ux = -1.0;
-            uy = copysign(SIN_PI, x0.y);
-        }
-        const double2 al = make_double2(-ux * s, -uy * s);
+        double a0;
+        const double2 al = house_alpha(x0, s, a0);
         *alpha = al;
         sc[0] = al.x;
         sc[1] = al.y;
