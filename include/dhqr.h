@@ -133,7 +133,9 @@ int dhqr_profile_get(dhqr_handle h, int index, char *name, int name_len, double 
  * (m x n_local, lda).  In place.  d_alpha (length n_global) receives diag(R) on every rank.
  * nb: 0 = handle default (blocked, compact-WY trailing update on the fp64 tensor pipe);
  *     1 = unblocked column-by-column path (BASELINE config 2);
- *     otherwise a multiple of 32 in [32,128]. */
+ *     otherwise a multiple of 32 in [32,128].
+ * The blocked paths (nb != 1) take m <= 728 x min(SMs, 160) rows (the 32-column panel kernel keeps its slab of rows in shared
+ * memory; read-only option "append_max_rows") and return -2 beyond that, with A untouched; nb = 1 has no row limit. */
 int dhqr_qr_f64(dhqr_handle h, int64_t m, int64_t n_global, int64_t col0, int64_t n_local,
                 double *dA_local, int64_t lda, double *d_alpha, int nb, void *stream);
 

@@ -204,7 +204,7 @@ def test_form_q_ext(D, h, coracle, oracle, family):
 # past the Float64 row limit, and two full panels at scale
 # ---------------------------------------------------------------------------------------------------------------------
 def test_tall(D, h, coracle, oracle):
-    # the blocked Float64 path stops at 728 min(SMs, 160) rows (test_gpu_ext.py::test_row_limit); the complex path has no limit
+    # the blocked Float64 path stops at 728 min(SMs, 160) rows (test_gpu_tall.py::test_row_limit); the complex path has no limit
     m, n = 728 * min(h.get_option("sms"), 160) + 1000, 128
     ref = Ref(coracle, oracle, "normal", m, n, cplx=True, keep_h64=True)
     ref.check_oracles_agree()

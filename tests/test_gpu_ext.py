@@ -239,21 +239,3 @@ def test_large_shapes_leading_columns(D, oracle, coracle, shape, family):
     gpu, absolute = factor_checks(f"{m}x{n} nb={nb}", ref, H, alpha, note)
     check(f"{m}x{n} nb={nb}", ref, gpu, ref.e64, absolute, note)
 
-
-def test_row_limit(D, oracle, coracle):
-    # the resident 32-column panel kernel holds 728 rows per CTA on at most 160 CTAs: m = 728 min(SMs, 160) is the tallest
-    # matrix the blocked paths take (96 096 on a 132-SM H100 SXM); one row more is refused with -2 before anything runs
-    h = D.default_handle(0)
-    lim = 728 * min(h.get_option("sms"), 160)
-    ref = Ref(coracle, oracle, "normal", lim, 256, k=128, solve=False)
-    dA, st, note, _ = run_qr(D, ref.A)
-    H, alpha = dA[:, :128].cpu().numpy(), st.α[:128].cpu().numpy()
-    gpu, absolute = factor_checks("row limit", ref, H, alpha, note)
-    check(f"row limit m={lim}", ref, gpu, ref.e64, absolute, note)
-    A1 = F.make("normal", lim + 1, 256)
-    dB = D.to_colmajor(A1, "cuda:0")
-    with pytest.raises(D._lib.DhqrError) as e:
-        D.qr_(dB)
-    assert e.value.code == -2
-    torch.cuda.synchronize()
-    assert np.array_equal(dB.cpu().numpy(), A1)
