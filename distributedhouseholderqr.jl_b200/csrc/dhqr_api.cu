@@ -708,6 +708,20 @@ static int check_common(dhqr_context* c, int64_t m, int64_t n_global, int64_t co
     return 0;
 }
 
+// The alignment check of a pointer to T, before anything is enqueued instead of a fault on the device.  The complex kernels load
+// and store whole double2 elements, so a ComplexF64 pointer must be 16 B aligned.  The C-ABI takes void* and an 8 B aligned one is
+// legal C (double _Complex, Julia's ComplexF64, a reinterpreted view of a Float64 vector).
+template <typename T>
+static int check_elem_ptr(const void* p, int arg, const char* name) {
+    if ((uintptr_t)p % alignof(T) == 0) return 0;
+    if (std::is_same<T, double2>::value) return set_err(arg, "%s is not 16-byte aligned (ComplexF64 data needs the alignment of double2)", name);
+    return set_err(arg, "%s must be 8 B aligned", name);
+}
+
+// the profile class of a launch: the Float64 kernel's name or the ComplexF64 one's
+template <typename T>
+static const char* kname(const char* f64, const char* c64) { return std::is_same<T, double>::value ? f64 : c64; }
+
 // ------------------------------------------------------------------------------------------------
 // qr!: blocked driver  (S:113-148, S:198-213)
 // ------------------------------------------------------------------------------------------------
@@ -1501,6 +1515,22 @@ static int wave_tag(dhqr_context* c, cudaStream_t st, uint32_t* tag) {
     return 0;
 }
 
+// x <- R^{-1} y by blocks of BS_BLK columns, last to first (S:260: i = n:-1:1), one k_backsolve_step launch per block: the
+// fallback of backsolve_local and every ComplexF64 back-substitution.  y[0:col0 + nl] is overwritten on the way.
+template <typename T>
+static int backsolve_steps(dhqr_context* c, cudaStream_t st, int64_t col0, int64_t nl, const T* A, int64_t lda, const T* alpha, T* y,
+                           int64_t ldy, int nrhs, T* x, int64_t ldx) {
+    for (int64_t o = ((nl - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {
+        const int bs = (int)std::min<int64_t>(BS_BLK, nl - o);
+        const int64_t c0 = col0 + o;
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((c0 + 255) / 256, 2 * c->sms));
+        TRY(launch(c, st, kname<T>("k_backsolve_step", "k_backsolve_step_c"), 0.0, [&](CwtSlot) {
+            k_backsolve_step<T><<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs);
+        }));
+    }
+    return 0;
+}
+
 static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64_t nl, const double* A, int64_t lda,
                            const double* alpha, double* y, int64_t ldy, int nrhs, double* x, int64_t ldx) {
     if (nl <= 0) return 0;
@@ -1517,48 +1547,105 @@ static int backsolve_local(dhqr_context* c, cudaStream_t st, int64_t col0, int64
         }
         return 0;
     }
-    // fallback: blocks of BS_BLK columns, last to first (S:260: i = n:-1:1), one launch per block
-    for (int64_t o = ((nl - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {
-        const int bs = (int)std::min<int64_t>(BS_BLK, nl - o);
-        const int64_t c0 = col0 + o;
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((c0 + 255) / 256, 2 * c->sms));
-        TRY(launch(c, st, "k_backsolve_step", 0.0, [&](CwtSlot) {
-            k_backsolve_step<<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs);
-        }));
+    return backsolve_steps(c, st, col0, nl, A, lda, alpha, y, ldy, nrhs, x, ldx);
+}
+
+// x (n x nrhs, leading dimension n) <- R^{-1} y[0:n] on one GPU, n > 0: backsolve_local for Float64, the steps for ComplexF64
+template <typename T>
+static int backsolve_single(dhqr_context* c, cudaStream_t st, int64_t n, const T* A, int64_t lda, const T* alpha, T* y, int64_t ldy,
+                            int nrhs, T* x) {
+    if constexpr (std::is_same<T, double>::value) {
+        TRY(wave_prepare(c, st, n));
+        return backsolve_local(c, st, 0, n, A, lda, alpha, y, ldy, nrhs, x, n);
+    } else {
+        return backsolve_steps(c, st, 0, n, A, lda, alpha, y, ldy, nrhs, x, n);
+    }
+}
+
+// y[0:n] <- R^{-H} y[0:n] on one GPU, through c->xbuf.  Float64: the wavefront of k_forwardsolve_wave (first strip to last) when
+// every CTA fits on the device at once.  Otherwise (or with "bs_wave" = 0), and always for ComplexF64: blocks of BS_BLK columns,
+// first to last, one k_forwardsolve_step each.  Every CTA of a step reads the block's y, so z goes to xbuf and is copied back at
+// the end, as in the back-substitution.
+template <typename T>
+static int forwardsolve_local(dhqr_context* c, cudaStream_t st, int64_t n, const T* A, int64_t lda, const T* alpha, T* y, int64_t ldy,
+                              int nrhs) {
+    if (n <= 0 || nrhs <= 0) return 0;
+    constexpr int w = sizeof(T) / sizeof(double);
+    TRY(c->xbuf.ensure((size_t)w * n * nrhs, st));
+    T* x = (T*)c->xbuf.p;
+    const int64_t ldx = n, nbk = (n + 31) / 32;
+    bool wave = false;
+    if constexpr (std::is_same<T, double>::value) {
+        TRY(wave_prepare(c, st, n));
+        wave = c->bs_wave && nbk <= c->fs_wave_max_ctas && nbk <= (int64_t)c->bs_blocks();
+        if (wave) {
+            for (int rhs = 0; rhs < nrhs; ++rhs) {
+                uint32_t tag;
+                TRY(wave_tag(c, st, &tag));
+                TRY(launch(c, st, "k_forwardsolve_wave", 0.0, [&](CwtSlot) {
+                    k_forwardsolve_wave<<<(unsigned)nbk, BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx,
+                                                                             n, c->bs_cells, tag);
+                }));
+            }
+        }
+    }
+    if (!wave) {
+        for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
+            const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
+            const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
+            TRY(launch(c, st, kname<T>("k_forwardsolve_step", "k_forwardsolve_step_c"), 0.0, [&](CwtSlot) {
+                k_forwardsolve_step<T><<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs, n);
+            }));
+        }
+    }
+    CU(cudaMemcpy2DAsync(y, (size_t)ldy * sizeof(T), x, (size_t)ldx * sizeof(T), (size_t)n * sizeof(T), nrhs, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+// V^ of a complex panel (64 complex reflectors, 128 real vectors) into vpk2[0]
+static int pack_complex_panel(dhqr_context* c, cudaStream_t st, const double2* P, int64_t lda, int64_t mpc, int kb, int64_t vrows) {
+    dim3 grid((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), NBMAX);
+    return launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) { k_pack_c<<<grid, 256, 0, st>>>(P, lda, mpc, kb, c->vpk2[0], 0, vrows); });
+}
+
+// b <- Q^H b (notrans = 0) or b <- Q b = H_1 ... H_n b (notrans = 1) with the first n reflectors of a single-GPU factorisation,
+// n > 0.  Float64: the one-vector sweep (qt_vec_ok) or the 128-column panels of apply_qt_local.
+static int apply_q_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double* A, int64_t lda, double* b, int64_t ldb,
+                         int nrhs, int notrans) {
+    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
+    if (qt_vec_ok(c, m, nrhs)) {
+        TRY(qt_prepare(c, st, m, 0, n, A, lda));
+        return apply_qt_local_vec(c, st, m, 0, n, A, lda, b, notrans);
+    }
+    return apply_qt_local(c, st, m, 0, n, A, lda, b, ldb, nrhs, notrans);
+}
+
+// ComplexF64 (S:232-242): panel by panel, last to first for Q b, each as the real block reflector of its 128 vectors [v_r, v_i]
+// on the real view of b (I - V T' V' for Q^H b, I - V T V' for Q b)
+static int apply_q_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b, int64_t ldb,
+                         int nrhs, int notrans) {
+    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
+    const int64_t last = ((n - 1) / CPW) * CPW;
+    for (int64_t p = 0; p <= last; p += CPW) {
+        const int64_t c0 = notrans ? last - p : p;
+        const int kb = (int)std::min<int64_t>(CPW, n - c0);
+        const int64_t mpc = m - c0, rows = 2 * mpc, vrows = rup(rows, 128);
+        TRY(pack_complex_panel(c, st, A + c0 * lda + c0, lda, mpc, kb, vrows));
+        TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, (double*)(b + c0), 2 * ldb, nrhs, false, nullptr, 0,
+                                  notrans));
     }
     return 0;
 }
 
-// y[0:n] <- R^{-T} y[0:n] on one GPU, through c->xbuf: the wavefront of k_forwardsolve_wave (first strip to last) when every CTA
-// fits on the device at once, otherwise (or with "bs_wave" = 0) blocks of BS_BLK columns, first to last, one k_forwardsolve_step
-// each.  Every CTA of a step reads the block's y, so z goes to xbuf and is copied back at the end, as in the back-substitution.
-static int forwardsolve_local(dhqr_context* c, cudaStream_t st, int64_t n, const double* A, int64_t lda, const double* alpha,
-                              double* y, int64_t ldy, int nrhs) {
-    if (n <= 0 || nrhs <= 0) return 0;
-    TRY(c->xbuf.ensure((size_t)n * nrhs, st));
-    TRY(wave_prepare(c, st, n));
-    double* x = c->xbuf;
-    const int64_t ldx = n, nbk = (n + 31) / 32;
-    if (c->bs_wave && nbk <= c->fs_wave_max_ctas && nbk <= (int64_t)c->bs_blocks()) {
-        for (int rhs = 0; rhs < nrhs; ++rhs) {
-            uint32_t tag;
-            TRY(wave_tag(c, st, &tag));
-            TRY(launch(c, st, "k_forwardsolve_wave", 0.0, [&](CwtSlot) {
-                k_forwardsolve_wave<<<(unsigned)nbk, BW_THREADS, 0, st>>>(A, lda, alpha, y + (int64_t)rhs * ldy, x + (int64_t)rhs * ldx, n,
-                                                                         c->bs_cells, tag);
-            }));
-        }
-    } else {
-        for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
-            const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
-            const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
-            TRY(launch(c, st, "k_forwardsolve_step", 0.0, [&](CwtSlot) {
-                k_forwardsolve_step<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, ldx, c0, bs, n);
-            }));
-        }
-    }
-    CU(cudaMemcpy2DAsync(y, (size_t)ldy * 8, x, (size_t)ldx * 8, (size_t)n * 8, nrhs, cudaMemcpyDeviceToDevice, st));
-    return 0;
+// The minimum-norm solution of A^H y = c, y = Q [R^{-H} c; 0], in place on b[0:m] (c = b[0:n]): forward substitution on rows
+// [0, n), zero rows [n, m), then b <- H_1 ... H_n b.  The body of dhqr_solve_adj_*, also the second stage of dhqr_solve_cod_*.
+template <typename T>
+static int solve_adj_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const T* A, int64_t lda, const T* alpha, T* b,
+                           int64_t ldb, int nrhs) {
+    TRY(forwardsolve_local(c, st, n, A, lda, alpha, b, ldb, nrhs));
+    if (m > n) CU(cudaMemset2DAsync(b + n, (size_t)ldb * sizeof(T), 0, (size_t)(m - n) * sizeof(T), nrhs, st));   // n = 0: y = 0, as in ?gels
+    if (n == 0) return 0;
+    return apply_q_local(c, st, m, n, A, lda, b, ldb, nrhs, 1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1831,8 +1918,10 @@ static int rhs_copy(cudaStream_t st, double* dst, int64_t lddst, const double* s
     return 0;
 }
 
-int dhqr_apply_qt_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
-                      int64_t lda, double* d_b, int64_t ldb, int nrhs, void* stream) {
+// b <- Q^H b (notrans = 0) or b <- Q b (notrans = 1).  The owners act on b one after the other and b travels rank to rank: in rank
+// order for Q^H b (C3, S:227-229), in reverse rank order for Q b = H_1 ... H_n b.  The last owner to act broadcasts the result.
+static int apply_q_dist(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA, int64_t lda,
+                        double* d_b, int64_t ldb, int nrhs, void* stream, int notrans) {
     TRY(check_common(c, m, n_global, col0, n_local, dA, lda));
     if (nrhs < 0) return set_err(-10, "nrhs < 0");
     if (nrhs > 0 && !d_b) return set_err(-8, "null b");
@@ -1844,59 +1933,35 @@ int dhqr_apply_qt_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
     TRY(gather_partition(c, st, col0, n_local, col0s, nls));
     TRY(check_partition(col0s, nls, n_global));
     TRY(ensure_workspace(c, st, m, std::max<int64_t>(n_local, nrhs)));
-    // C3 (S:227-229): owners act on b one after the other; b travels rank -> rank
+    const int step = notrans ? -1 : 1, first = notrans ? c->nranks - 1 : 0, last = notrans ? 0 : c->nranks - 1;
     const size_t cnt = (size_t)m * nrhs;
     double* msg = d_b;
     if (c->nranks > 1) TRY(rhs_message(c, st, d_b, ldb, m, nrhs, &msg));
     const bool vec = qt_vec_ok(c, m, nrhs);
     if (vec) TRY(qt_prepare(c, st, m, col0, n_local, dA, lda));
-    if (c->nranks > 1 && c->rank > 0) {
-        NC(g_nccl.Recv(msg, cnt, ncclFloat64, c->rank - 1, c->comm, st));
+    if (c->nranks > 1 && c->rank != first) {
+        NC(g_nccl.Recv(msg, cnt, ncclFloat64, c->rank - step, c->comm, st));
         TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
     }
-    if (vec) TRY(apply_qt_local_vec(c, st, m, col0, n_local, dA, lda, d_b, 0));
-    else TRY(apply_qt_local(c, st, m, col0, n_local, dA, lda, d_b, ldb, nrhs));
+    if (vec) TRY(apply_qt_local_vec(c, st, m, col0, n_local, dA, lda, d_b, notrans));
+    else TRY(apply_qt_local(c, st, m, col0, n_local, dA, lda, d_b, ldb, nrhs, notrans));
     if (c->nranks > 1) {
         TRY(rhs_copy(st, msg, m, d_b, ldb, m, nrhs));
-        if (c->rank + 1 < c->nranks) NC(g_nccl.Send(msg, cnt, ncclFloat64, c->rank + 1, c->comm, st));
-        NC(g_nccl.Broadcast(msg, msg, cnt, ncclFloat64, c->nranks - 1, c->comm, st));
-        if (c->rank + 1 < c->nranks) TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
+        if (c->rank != last) NC(g_nccl.Send(msg, cnt, ncclFloat64, c->rank + step, c->comm, st));
+        NC(g_nccl.Broadcast(msg, msg, cnt, ncclFloat64, last, c->comm, st));
+        if (c->rank != last) TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
     }
     return 0;
 }
 
+int dhqr_apply_qt_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
+                      int64_t lda, double* d_b, int64_t ldb, int nrhs, void* stream) {
+    return apply_q_dist(c, m, n_global, col0, n_local, dA, lda, d_b, ldb, nrhs, stream, 0);
+}
+
 int dhqr_apply_q_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
                      int64_t lda, double* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_common(c, m, n_global, col0, n_local, dA, lda));
-    if (nrhs < 0) return set_err(-10, "nrhs < 0");
-    if (nrhs > 0 && !d_b) return set_err(-8, "null b");
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-9, "ldb < max(1,m)");
-    if (n_global == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    std::vector<int64_t> col0s, nls;
-    TRY(gather_partition(c, st, col0, n_local, col0s, nls));
-    TRY(check_partition(col0s, nls, n_global));
-    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n_local, nrhs)));
-    // b <- H_1 ... H_n b: the owners act in reverse rank order, b travels rank -> rank - 1
-    const size_t cnt = (size_t)m * nrhs;
-    double* msg = d_b;
-    if (c->nranks > 1) TRY(rhs_message(c, st, d_b, ldb, m, nrhs, &msg));
-    const bool vec = qt_vec_ok(c, m, nrhs);
-    if (vec) TRY(qt_prepare(c, st, m, col0, n_local, dA, lda));
-    if (c->nranks > 1 && c->rank + 1 < c->nranks) {
-        NC(g_nccl.Recv(msg, cnt, ncclFloat64, c->rank + 1, c->comm, st));
-        TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
-    }
-    if (vec) TRY(apply_qt_local_vec(c, st, m, col0, n_local, dA, lda, d_b, 1));
-    else TRY(apply_qt_local(c, st, m, col0, n_local, dA, lda, d_b, ldb, nrhs, 1));
-    if (c->nranks > 1) {
-        TRY(rhs_copy(st, msg, m, d_b, ldb, m, nrhs));
-        if (c->rank > 0) NC(g_nccl.Send(msg, cnt, ncclFloat64, c->rank - 1, c->comm, st));
-        NC(g_nccl.Broadcast(msg, msg, cnt, ncclFloat64, 0, c->comm, st));
-        if (c->rank > 0) TRY(rhs_copy(st, d_b, ldb, msg, m, m, nrhs));
-    }
-    return 0;
+    return apply_q_dist(c, m, n_global, col0, n_local, dA, lda, d_b, ldb, nrhs, stream, 1);
 }
 
 int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
@@ -1953,31 +2018,18 @@ static int check_complex(dhqr_context* c, int64_t m, int64_t n_global, int64_t c
     return 0;
 }
 
-// The complex kernels load and store whole double2 elements, so a ComplexF64 pointer must be 16 B aligned.  The C-ABI takes void*
-// and an 8 B aligned one is legal C (double _Complex, Julia's ComplexF64, a reinterpreted view of a Float64 vector); it is turned
-// down here, before anything is enqueued, instead of faulting on the device.
-static int check_c64_ptr(const void* p, int arg, const char* name) {
-    if ((uintptr_t)p % alignof(double2)) return set_err(arg, "%s is not 16-byte aligned (ComplexF64 data needs the alignment of double2)", name);
-    return 0;
-}
-
 // arguments of dhqr_backsolve_c64 and dhqr_solve_c64 (same signature)
 static int check_c64_args(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                           const void* d_alpha, const void* d_b, int64_t ldb, int nrhs) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    TRY(check_c64_ptr(dA, -6, "A"));
+    TRY(check_elem_ptr<double2>(dA, -6, "A"));
     if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
-    TRY(check_c64_ptr(d_alpha, -8, "alpha"));
+    TRY(check_elem_ptr<double2>(d_alpha, -8, "alpha"));
     if (nrhs < 0) return set_err(-11, "nrhs < 0");
     if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    TRY(check_c64_ptr(d_b, -9, "b"));
+    TRY(check_elem_ptr<double2>(d_b, -9, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
     return 0;
-}
-
-static int pack_complex_panel(dhqr_context* c, cudaStream_t st, const double2* P, int64_t lda, int64_t mpc, int kb, int64_t vrows) {
-    dim3 grid((unsigned)std::min<int64_t>((vrows + 255) / 256, 4 * c->sms), NBMAX);
-    return launch(c, st, "k_pack_c", 0.0, [&](CwtSlot) { k_pack_c<<<grid, 256, 0, st>>>(P, lda, mpc, kb, c->vpk2[0], 0, vrows); });
 }
 
 static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double2* A, int64_t lda, double2* alpha);
@@ -1985,9 +2037,9 @@ static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
 int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, void* dA, int64_t lda, void* d_alpha,
                 void* stream) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    TRY(check_c64_ptr(dA, -6, "A"));
+    TRY(check_elem_ptr<double2>(dA, -6, "A"));
     if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
-    TRY(check_c64_ptr(d_alpha, -8, "alpha"));
+    TRY(check_elem_ptr<double2>(d_alpha, -8, "alpha"));
     if (n_global == 0) return 0;
     CU(cudaSetDevice(c->device));
     return qr_c64_local(c, (cudaStream_t)stream, m, n_global, (double2*)dA, lda, (double2*)d_alpha);
@@ -2019,46 +2071,17 @@ static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
     return 0;
 }
 
-static int apply_qt_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b,
-                              int64_t ldb, int nrhs);
-
 int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                       void* d_b, int64_t ldb, int nrhs, void* stream) {
     TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    TRY(check_c64_ptr(dA, -6, "A"));
+    TRY(check_elem_ptr<double2>(dA, -6, "A"));
     if (nrhs < 0) return set_err(-10, "nrhs < 0");
     if (nrhs > 0 && !d_b) return set_err(-8, "null b");
-    TRY(check_c64_ptr(d_b, -8, "b"));
+    TRY(check_elem_ptr<double2>(d_b, -8, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-9, "ldb < max(1,m)");
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
-    return apply_qt_c64_local(c, (cudaStream_t)stream, m, n_global, (const double2*)dA, lda, (double2*)d_b, ldb, nrhs);
-}
-
-// the body of dhqr_apply_qt_c64 (n > 0, nrhs > 0), also the (Q^H b)[0:rank] stage of the complex pivoted solves
-static int apply_qt_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b,
-                              int64_t ldb, int nrhs) {
-    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
-    for (int64_t c0 = 0; c0 < n; c0 += CPW) {                // S:232-242, panel by panel
-        const int kb = (int)std::min<int64_t>(CPW, n - c0);
-        const int64_t mpc = m - c0, rows = 2 * mpc, vrows = rup(rows, 128);
-        TRY(pack_complex_panel(c, st, A + c0 * lda + c0, lda, mpc, kb, vrows));
-        TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, (double*)(b + c0), 2 * ldb, nrhs));
-    }
-    return 0;
-}
-
-// x (n x nrhs, ldx) <- R^{-1} b[0:n] for complex R = triu(A, 1) + diag(alpha); b[0:n] is overwritten on the way
-static int backsolve_c64_local(dhqr_context* c, cudaStream_t st, int64_t n, const double2* A, int64_t lda, const double2* alpha, double2* b,
-                               int64_t ldb, int nrhs, double2* x, int64_t ldx) {
-    for (int64_t o = ((n - 1) / BS_BLK) * BS_BLK; o >= 0; o -= BS_BLK) {     // S:260: i = n:-1:1, by blocks
-        const int bs = (int)std::min<int64_t>(BS_BLK, n - o);
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((o + 255) / 256, 2 * c->sms));
-        TRY(launch(c, st, "k_backsolve_step_c", 0.0, [&](CwtSlot) {
-            k_backsolve_step_c<<<grid, 256, 0, st>>>(A + o * lda, lda, alpha, b, ldb, nrhs, x, ldx, o, bs);
-        }));
-    }
-    return 0;
+    return apply_q_local(c, (cudaStream_t)stream, m, n_global, (const double2*)dA, lda, (double2*)d_b, ldb, nrhs, 0);
 }
 
 int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
@@ -2070,7 +2093,7 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
     const int64_t n = n_global;
     TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
     double2* x = (double2*)c->xbuf.p;
-    TRY(backsolve_c64_local(c, st, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs, x, n));
+    TRY(backsolve_single(c, st, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs, x));
     CU(cudaMemcpy2DAsync(d_b, (size_t)ldb * 16, x, (size_t)n * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
     return 0;
 }
@@ -2082,30 +2105,19 @@ int dhqr_solve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int
     return dhqr_backsolve_c64(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs, stream);       // S:291
 }
 
-int dhqr_partialdot_c64(dhqr_handle c, const void* d_a, const void* d_b, int64_t i0, int64_t i1, void* d_out, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (!d_a) return set_err(-2, "null a");
-    if (!d_b) return set_err(-3, "null b");
-    if (i0 < 0) return set_err(-4, "i0 < 0");
-    if (i1 < i0) return set_err(-5, "i1 < i0");
-    if (!d_out) return set_err(-6, "null out");
-    TRY(check_c64_ptr(d_a, -2, "a"));
-    TRY(check_c64_ptr(d_b, -3, "b"));
-    TRY(check_c64_ptr(d_out, -6, "out"));
-    CU(cudaSetDevice(c->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    return launch(c, st, "k_partialdot_c", 0.0, [&](CwtSlot) {
-        k_partialdot_c<<<1, 1024, 0, st>>>((const double2*)d_a, (const double2*)d_b, i0, i1, (double2*)d_out);
-    });
-}
-
 // ---- explicit thin Q (LAPACK orgqr / ungqr) ---------------------------------------------------------------------------------
 // Q <- H_1 ... H_n [I_n; 0], accumulated backwards over panels p = last .. 0 with columns [cs, cs + kb): pack V_p from A, make the
 // panel's columns of Q those of the identity (all m rows, which also clears R's rows when Q is A), then apply I - V_p T_p V_p'
 // (T, not T') to rows >= cs, columns [cs, n) of Q.  Columns left of cs are still unit vectors with zeros in rows >= cs, so the
 // panel leaves them alone: 2mn^2 - 2n^3/3 flops instead of the 4mn^2 - 2n^3 of Q applied to [I; 0].  V_p is packed before its
 // columns are overwritten, so in place and out of place are the same sweep.
-static int check_form_q(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* Q, int64_t ldq, size_t esz) {
+// Templates and overloads over the element type, which C linkage does not allow, sit in extern "C++" blocks; the dhqr_* functions
+// keep the C linkage of their declarations in dhqr.h.
+extern "C++" {
+
+template <typename T>
+static int check_form_q(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* Q, int64_t ldq) {
+    const size_t esz = sizeof(T);
     if (!c) return set_err(-1, "null handle");
     if (c->nranks != 1) return set_err(-1, "form_q is single-GPU (the handle has %d ranks)", c->nranks);
     if (m < 0) return set_err(-2, "m < 0");
@@ -2120,8 +2132,14 @@ static int check_form_q(dhqr_context* c, int64_t m, int64_t n, const void* A, in
         if (q0 < a1 && a0 < q1 && !(Q == A && ldq == lda))
             return set_err(-6, "Q overlaps A without being A itself (Q == A needs ldq == lda)");
     }
+    if (std::is_same<T, double2>::value) {                  // Float64 pointers are not checked for alignment here
+        TRY(check_elem_ptr<T>(A, -4, "A"));
+        TRY(check_elem_ptr<T>(Q, -6, "Q"));
+    }
     return 0;
 }
+
+}  // extern "C++"
 
 static int eye_cols(dhqr_context* c, cudaStream_t st, void* Q, bool cplx, int64_t ldq, int64_t m, int64_t c0, int kb) {
     const dim3 grid((unsigned)std::min<int64_t>((m + 255) / 256, 64), kb);
@@ -2132,7 +2150,7 @@ static int eye_cols(dhqr_context* c, cudaStream_t st, void* Q, bool cplx, int64_
 }
 
 int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, double* dQ, int64_t ldq, void* stream) {
-    TRY(check_form_q(c, m, n, dA, lda, dQ, ldq, sizeof(double)));
+    TRY(check_form_q<double>(c, m, n, dA, lda, dQ, ldq));
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2152,9 +2170,7 @@ int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64
 // ComplexF64: the same sweep over 64-column complex panels on the real view of Q (2m x n, leading dimension 2 ldq), each panel the
 // real block reflector of its 128 vectors [v_r, v_i] (dhqr_complex.cuh); T from the Gram block of the update itself.
 int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, void* dQ, int64_t ldq, void* stream) {
-    TRY(check_form_q(c, m, n, dA, lda, dQ, ldq, sizeof(double2)));
-    TRY(check_c64_ptr(dA, -4, "A"));
-    TRY(check_c64_ptr(dQ, -6, "Q"));
+    TRY(check_form_q<double2>(c, m, n, dA, lda, dQ, ldq));
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2173,110 +2189,67 @@ int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t
 }
 
 // ---- solves with the adjoint (LAPACK ?gels, TRANS = 'C') ------------------------------------------------------------------
-// forwardsolve: b[0:n] <- R^{-H} b[0:n].  solve_adj: the minimum-norm solution of A^H y = c, y = Q [R^{-H} c; 0]: forward
-// substitution on rows [0, n), zero rows [n, m), then b <- H_1 ... H_n b.  Single GPU.
+// forwardsolve: b[0:n] <- R^{-H} b[0:n].  solve_adj: the minimum-norm solution of A^H y = c (solve_adj_local).  Single GPU.
+extern "C++" {   // as for form_q above
+
+template <typename T>
 static int check_adj(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* alpha, const void* b, int64_t ldb,
-                     int nrhs, bool cplx) {
+                     int nrhs) {
+    constexpr bool cplx = std::is_same<T, double2>::value;       // Float64 pointers are not checked for alignment here
     if (!c) return set_err(-1, "null handle");
     if (c->nranks != 1) return set_err(-1, "the adjoint solves are single-GPU (the handle has %d ranks)", c->nranks);
     if (m < 0) return set_err(-2, "m < 0");
     if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
     if (n > 0 && !A) return set_err(-4, "null A");
-    if (cplx) TRY(check_c64_ptr(A, -4, "A"));
+    if (cplx) TRY(check_elem_ptr<T>(A, -4, "A"));
     if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
     if (n > 0 && !alpha) return set_err(-6, "null alpha");
-    if (cplx) TRY(check_c64_ptr(alpha, -6, "alpha"));
+    if (cplx) TRY(check_elem_ptr<T>(alpha, -6, "alpha"));
     if (nrhs > 0 && !b) return set_err(-7, "null b");
-    if (cplx) TRY(check_c64_ptr(b, -7, "b"));
+    if (cplx) TRY(check_elem_ptr<T>(b, -7, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-8, "ldb < max(1,m)");
     if (nrhs < 0) return set_err(-9, "nrhs < 0");
     return 0;
 }
 
-// complex y[0:n] <- R^{-H} y[0:n], blocks of BS_BLK columns first to last, through c->xbuf
-static int forwardsolve_c64_local(dhqr_context* c, cudaStream_t st, int64_t n, const double2* A, int64_t lda, const double2* alpha,
-                                  double2* y, int64_t ldy, int nrhs) {
-    TRY(c->xbuf.ensure((size_t)2 * n * nrhs, st));
-    double2* x = (double2*)c->xbuf.p;
-    for (int64_t c0 = 0; c0 < n; c0 += BS_BLK) {
-        const int bs = (int)std::min<int64_t>(BS_BLK, n - c0);
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n - c0 - bs + 7) / 8, 4 * c->sms));
-        TRY(launch(c, st, "k_forwardsolve_step_c", 0.0, [&](CwtSlot) {
-            k_forwardsolve_step_c<<<grid, 256, 0, st>>>(A, lda, alpha, y, ldy, nrhs, x, n, c0, bs, n);
-        }));
-    }
-    CU(cudaMemcpy2DAsync(y, (size_t)ldy * 16, x, (size_t)n * 16, (size_t)n * 16, nrhs, cudaMemcpyDeviceToDevice, st));
-    return 0;
+template <typename T>
+static int forwardsolve(dhqr_context* c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
+                        int nrhs, void* stream) {
+    TRY(check_adj<T>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs));
+    if (n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return forwardsolve_local(c, (cudaStream_t)stream, n, (const T*)dA, lda, (const T*)d_alpha, (T*)d_b, ldb, nrhs);
 }
 
-// complex b <- Q b = H_1 ... H_n b: the panel loop of dhqr_apply_qt_c64 run backwards, each panel as I - V T V' (T, not T')
-static int apply_q_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, double2* b,
-                             int64_t ldb, int nrhs) {
-    TRY(ensure_workspace(c, st, 2 * m, std::max<int64_t>(n, nrhs)));
-    for (int64_t c0 = ((n - 1) / CPW) * CPW; c0 >= 0; c0 -= CPW) {
-        const int kb = (int)std::min<int64_t>(CPW, n - c0);
-        const int64_t mpc = m - c0, rows = 2 * mpc, vrows = rup(rows, 128);
-        TRY(pack_complex_panel(c, st, A + c0 * lda + c0, lda, mpc, kb, vrows));
-        TRY(apply_block_reflector(c, st, c->vpk2[0], c->ws[0], 0, NBMAX, rows, 0, (double*)(b + c0), 2 * ldb, nrhs, false, nullptr, 0, 1));
-    }
-    return 0;
+template <typename T>
+static int solve_adj(dhqr_context* c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
+                     int nrhs, void* stream) {
+    TRY(check_adj<T>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs));
+    if (m == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    return solve_adj_local(c, (cudaStream_t)stream, m, n, (const T*)dA, lda, (const T*)d_alpha, (T*)d_b, ldb, nrhs);
 }
+
+}  // extern "C++"
 
 int dhqr_forwardsolve_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
                           int64_t ldb, int nrhs, void* stream) {
-    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, false));
-    if (n == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    return forwardsolve_local(c, (cudaStream_t)stream, n, dA, lda, d_alpha, d_b, ldb, nrhs);
+    return forwardsolve<double>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
 }
 
 int dhqr_forwardsolve_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b,
                           int64_t ldb, int nrhs, void* stream) {
-    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, true));
-    if (n == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    return forwardsolve_c64_local(c, (cudaStream_t)stream, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs);
-}
-
-// y = Q [R^{-T} c; 0] in place on b[0:m] (c = b[0:n]): the body of dhqr_solve_adj_f64, also the second stage of dhqr_solve_cod_f64
-static int solve_adj_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha,
-                           double* d_b, int64_t ldb, int nrhs) {
-    TRY(forwardsolve_local(c, st, n, dA, lda, d_alpha, d_b, ldb, nrhs));
-    if (m > n) CU(cudaMemset2DAsync(d_b + n, (size_t)ldb * 8, 0, (size_t)(m - n) * 8, nrhs, st));    // n = 0: y = 0, as in ?gels
-    if (n == 0) return 0;
-    TRY(ensure_workspace(c, st, m, std::max<int64_t>(n, nrhs)));
-    if (qt_vec_ok(c, m, nrhs)) {
-        TRY(qt_prepare(c, st, m, 0, n, dA, lda));
-        TRY(apply_qt_local_vec(c, st, m, 0, n, dA, lda, d_b, 1));
-    } else {
-        TRY(apply_qt_local(c, st, m, 0, n, dA, lda, d_b, ldb, nrhs, 1));
-    }
-    return 0;
+    return forwardsolve<double2>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
 }
 
 int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
                        int64_t ldb, int nrhs, void* stream) {
-    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, false));
-    if (m == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    return solve_adj_local(c, (cudaStream_t)stream, m, n, dA, lda, d_alpha, d_b, ldb, nrhs);
-}
-
-// y = Q [R^{-H} c; 0] in place on complex b[0:m]: the body of dhqr_solve_adj_c64, also the second stage of dhqr_solve_cod_c64
-static int solve_adj_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, const double2* A, int64_t lda, const double2* alpha,
-                               double2* b, int64_t ldb, int nrhs) {
-    if (n > 0) TRY(forwardsolve_c64_local(c, st, n, A, lda, alpha, b, ldb, nrhs));
-    if (m > n) CU(cudaMemset2DAsync(b + n, (size_t)ldb * 16, 0, (size_t)(m - n) * 16, nrhs, st));
-    if (n == 0) return 0;
-    return apply_q_c64_local(c, st, m, n, A, lda, b, ldb, nrhs);
+    return solve_adj<double>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
 }
 
 int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
                        int nrhs, void* stream) {
-    TRY(check_adj(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, true));
-    if (m == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
-    return solve_adj_c64_local(c, (cudaStream_t)stream, m, n, (const double2*)dA, lda, (const double2*)d_alpha, (double2*)d_b, ldb, nrhs);
+    return solve_adj<double2>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
 }
 
 // ---- QR with column pivoting (LAPACK ?geqp3 / ?laqps, dhqr_qrcp.cuh), Float64 and ComplexF64 ---------------------------------
@@ -2285,24 +2258,7 @@ int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int6
 // ending the panel early: every panel has its static width and the host never needs a device value, so the driver is one static
 // loop and the call does not synchronise.  Single GPU, n <= m, no row limit.  T = double or double2; the workspace is sized in
 // doubles, and every section of it that holds T is aligned for T.
-static int check_qrcp_ptr(const void* p, int arg, const char* name) {
-    if (((uintptr_t)p & 7) != 0) return set_err(arg, "%s must be 8 B aligned", name);
-    return 0;
-}
-
-// Overloads and templates over the element type, which C linkage does not allow; the dhqr_* functions below keep the C linkage
-// of their declarations in dhqr.h.
-extern "C++" {
-
-// the alignment check of a pointer to T
-template <typename T>
-static int check_elem_ptr(const void* p, int arg, const char* name) {
-    return std::is_same<T, double>::value ? check_qrcp_ptr(p, arg, name) : check_c64_ptr(p, arg, name);
-}
-
-// the profile class of a launch: the Float64 kernel's name or the ComplexF64 one's
-template <typename T>
-static const char* qp_name(const char* f64, const char* c64) { return std::is_same<T, double>::value ? f64 : c64; }
+extern "C++" {   // as for form_q above
 
 // A[c1:, c1:] -= V F' on the window starting at row k0 (a multiple of 32), rows >= c1 only: the 32-wide C += V Y with Y = -F'
 static int qrcp_update(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, int64_t k0, int kb, double* A, int64_t lda,
@@ -2349,7 +2305,7 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, T*
     a.A = A; a.lda = lda; a.m = m; a.n = n; a.alpha = alpha; a.jpvt = jpvt; a.flag = c->qp_flag; a.ctl = c->qp_ctl;
     a.vn1 = c->qp_buf; a.vn2 = a.vn1 + n; a.F = (T*)(a.vn2 + n); a.ldf = n; a.x = a.F + (size_t)QP_NB * n;
     a.part1 = (double*)(a.x + m); a.part2 = (T*)(a.part1 + rup(p1, w)); a.ldp = n;
-    TRY(launch(c, st, qp_name<T>("k_qrcp_init", "k_qrcp_init_c"), (double)sizeof(T) * (double)m * n, [&](CwtSlot) {
+    TRY(launch(c, st, kname<T>("k_qrcp_init", "k_qrcp_init_c"), (double)sizeof(T) * (double)m * n, [&](CwtSlot) {
         k_qrcp_init<T><<<(unsigned)n, QP_THREADS, 0, st>>>(A, lda, m, a.vn1, a.vn2, jpvt, c->qp_flag);
     }));
     for (int64_t k0 = 0; k0 < n; k0 += QP_NB) {
@@ -2358,7 +2314,7 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, T*
         for (int jj = 0; jj < kb; ++jj) {
             const int64_t j = k0 + jj, rows = m - j;
             a.j = j; a.k0 = k0; a.jj = jj;
-            TRY(launch(c, st, qp_name<T>("k_qrcp_pivot", "k_qrcp_pivot_c"),
+            TRY(launch(c, st, kname<T>("k_qrcp_pivot", "k_qrcp_pivot_c"),
                        32.0 * (double)m + (double)sizeof(T) * (double)rows * (jj + 1) + 8.0 * (double)(n - j), [&](CwtSlot) {
                 k_qrcp_pivot<<<(unsigned)p1, QP_THREADS, 0, st>>>(a);
             }));
@@ -2367,14 +2323,14 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, T*
                                                                      (8 * (int64_t)c->sms + tiles - 1) / tiles));
             a.split_rows = rup((rows + s - 1) / s, QP_THREADS);
             a.nsplit = (int)((rows + a.split_rows - 1) / a.split_rows);
-            TRY(launch(c, st, qp_name<T>("k_qrcp_gemv", "k_qrcp_gemv_c"), (double)sizeof(T) * (double)rows * (double)(n - k0), [&](CwtSlot) {
+            TRY(launch(c, st, kname<T>("k_qrcp_gemv", "k_qrcp_gemv_c"), (double)sizeof(T) * (double)rows * (double)(n - k0), [&](CwtSlot) {
                 k_qrcp_gemv<<<dim3((unsigned)tiles, (unsigned)a.nsplit), QP_THREADS, 0, st>>>(a);
             }));
             if (j + 1 >= n) continue;
-            TRY(launch(c, st, qp_name<T>("k_qrcp_finish", "k_qrcp_finish_c"), 0.0, [&](CwtSlot) {
+            TRY(launch(c, st, kname<T>("k_qrcp_finish", "k_qrcp_finish_c"), 0.0, [&](CwtSlot) {
                 k_qrcp_finish<<<(unsigned)((n - j - 1 + QP_THREADS - 1) / QP_THREADS), QP_THREADS, 0, st>>>(a);
             }));
-            TRY(launch(c, st, qp_name<T>("k_qrcp_renorm", "k_qrcp_renorm_c"), 0.0, [&](CwtSlot) {
+            TRY(launch(c, st, kname<T>("k_qrcp_renorm", "k_qrcp_renorm_c"), 0.0, [&](CwtSlot) {
                 k_qrcp_renorm<<<(unsigned)std::min<int64_t>(n - j - 1, 2 * (int64_t)c->sms), QP_THREADS, 0, st>>>(a);
             }));
         }
@@ -2396,37 +2352,10 @@ static int qrcp_factor(dhqr_context* c, int64_t m, int64_t n, void* dA, int64_t 
     if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
     TRY(check_elem_ptr<T>(d_alpha, -6, "alpha"));
     if (n > 0 && !d_jpvt) return set_err(-7, "null jpvt");
-    TRY(check_qrcp_ptr(d_jpvt, -7, "jpvt"));
+    TRY(check_elem_ptr<int64_t>(d_jpvt, -7, "jpvt"));
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     return qrcp_local(c, (cudaStream_t)stream, m, n, (T*)dA, lda, (T*)d_alpha, d_jpvt);
-}
-
-// (Q^H b)[0:rank]: the first `rank` reflectors of a pivoted factorisation on b, the first stage of both pivoted solves
-static int qrcp_qtb(dhqr_context* c, cudaStream_t st, int64_t m, int64_t rank, const double* dA, int64_t lda, double* d_b, int64_t ldb,
-                    int nrhs) {
-    if (qt_vec_ok(c, m, nrhs)) {
-        TRY(qt_prepare(c, st, m, 0, rank, dA, lda));
-        return apply_qt_local_vec(c, st, m, 0, rank, dA, lda, d_b, 0);
-    }
-    return apply_qt_local(c, st, m, 0, rank, dA, lda, d_b, ldb, nrhs);
-}
-
-static int qrcp_qtb(dhqr_context* c, cudaStream_t st, int64_t m, int64_t rank, const double2* A, int64_t lda, double2* b, int64_t ldb,
-                    int nrhs) {
-    return apply_qt_c64_local(c, st, m, rank, A, lda, b, ldb, nrhs);
-}
-
-// z = R11^{-1} b[0:rank] of the basic solution
-static int qrcp_backsolve(dhqr_context* c, cudaStream_t st, int64_t rank, const double* A, int64_t lda, const double* alpha, double* b,
-                          int64_t ldb, int nrhs, double* z) {
-    TRY(wave_prepare(c, st, rank));
-    return backsolve_local(c, st, 0, rank, A, lda, alpha, b, ldb, nrhs, z, rank);
-}
-
-static int qrcp_backsolve(dhqr_context* c, cudaStream_t st, int64_t rank, const double2* A, int64_t lda, const double2* alpha, double2* b,
-                          int64_t ldb, int nrhs, double2* z) {
-    return backsolve_c64_local(c, st, rank, A, lda, alpha, b, ldb, nrhs, z, rank);
 }
 
 // b[jpvt[i]] = z[i] for i < rank, 0 for rank <= i < n, on every right-hand side; jpvt entries outside [0, n) are skipped
@@ -2435,7 +2364,7 @@ static int qrcp_scatter(dhqr_context* c, cudaStream_t st, int64_t n, int64_t ran
                         T* d_b, int64_t ldb, int nrhs) {
     for (int r0 = 0; r0 < nrhs; r0 += 65535) {
         const int nr = std::min(nrhs - r0, 65535);
-        TRY(launch(c, st, qp_name<T>("k_qrcp_scatter", "k_qrcp_scatter_c"), 0.0, [&](CwtSlot) {
+        TRY(launch(c, st, kname<T>("k_qrcp_scatter", "k_qrcp_scatter_c"), 0.0, [&](CwtSlot) {
             k_qrcp_scatter<T><<<dim3((unsigned)((n + 255) / 256), (unsigned)nr), 256, 0, st>>>(z + (size_t)r0 * ldz, ldz, d_jpvt, n, rank,
                                                                                             d_b + (size_t)r0 * ldb, ldb);
         }));
@@ -2457,7 +2386,7 @@ static int qrcp_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const
     if (n > 0 && !d_alpha) return set_err(-7, "null alpha");
     TRY(check_elem_ptr<T>(d_alpha, -7, "alpha"));
     if (n > 0 && !d_jpvt) return set_err(-8, "null jpvt");
-    TRY(check_qrcp_ptr(d_jpvt, -8, "jpvt"));
+    TRY(check_elem_ptr<int64_t>(d_jpvt, -8, "jpvt"));
     if (nrhs > 0 && !d_b) return set_err(-9, "null b");
     TRY(check_elem_ptr<T>(d_b, -9, "b"));
     if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
@@ -2472,8 +2401,8 @@ static int qrcp_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const
     T* b = (T*)d_b;
     T* z = (T*)c->xbuf.p;
     if (rank > 0) {
-        TRY(qrcp_qtb(c, st, m, rank, A, lda, b, ldb, nrhs));
-        TRY(qrcp_backsolve(c, st, rank, A, lda, (const T*)d_alpha, b, ldb, nrhs, z));
+        TRY(apply_q_local(c, st, m, rank, A, lda, b, ldb, nrhs, 0));                 // (Q^H b)[0:rank]
+        TRY(backsolve_single(c, st, rank, A, lda, (const T*)d_alpha, b, ldb, nrhs, z));   // z = R11^{-1} b[0:rank]
     }
     return qrcp_scatter(c, st, n, rank, z, rank, d_jpvt, b, ldb, nrhs);
 }
@@ -2529,7 +2458,7 @@ static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const 
     if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
     const char* name7 = factor ? "alpha" : "jpvt";
     if (n > 0 && !seventh) return set_err(-7, "null %s", name7);
-    TRY(factor ? check_elem_ptr<T>(seventh, -7, name7) : check_qrcp_ptr(seventh, -7, name7));
+    TRY(factor ? check_elem_ptr<T>(seventh, -7, name7) : check_elem_ptr<int64_t>(seventh, -7, name7));
     if (rank > 0 && !dF) return set_err(-8, "null F");
     TRY(check_elem_ptr<T>(dF, -8, "F"));
     if (ldf < std::max<int64_t>(1, n)) return set_err(-9, "ldf < max(1,n)");
@@ -2563,22 +2492,11 @@ static int cod_factor(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const
     if (n == 0 || rank == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    TRY(launch(c, st, qp_name<T>("k_cod_pack", "k_cod_pack_c"), (double)sizeof(T) * (double)n * rank, [&](CwtSlot) {
+    TRY(launch(c, st, kname<T>("k_cod_pack", "k_cod_pack_c"), (double)sizeof(T) * (double)n * rank, [&](CwtSlot) {
         k_cod_pack<T><<<dim3((unsigned)((n + CP_TILE - 1) / CP_TILE), (unsigned)((rank + CP_TILE - 1) / CP_TILE)), dim3(CP_TILE, CP_ROWS), 0,
                         st>>>((const T*)dA, lda, (const T*)d_alpha, n, rank, (T*)dF, ldf);
     }));
     return qr_rrh(c, st, n, rank, (T*)dF, ldf, (T*)d_gamma);
-}
-
-// b[0:n] <- Z [U^{-H} b[0:rank]; 0] from the factorisation (F, gamma) of R_r^H, rows n..m-1 of b untouched
-static int cod_adj(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double* F, int64_t ldf, const double* gamma,
-                   double* b, int64_t ldb, int nrhs) {
-    return solve_adj_local(c, st, n, rank, F, ldf, gamma, b, ldb, nrhs);
-}
-
-static int cod_adj(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, const double2* F, int64_t ldf, const double2* gamma,
-                   double2* b, int64_t ldb, int nrhs) {
-    return solve_adj_c64_local(c, st, n, rank, F, ldf, gamma, b, ldb, nrhs);
 }
 
 template <typename T>
@@ -2598,9 +2516,10 @@ static int cod_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const 
     T* b = (T*)d_b;
     T* z = (T*)c->xbuf.p;
     if (rank > 0) {
-        TRY(qrcp_qtb(c, st, m, rank, (const T*)dA, lda, b, ldb, nrhs));
-        // b[0:n] <- Z [U^{-H} b[0:rank]; 0]; then into xbuf, which the scatter reads while it writes b
-        TRY(cod_adj(c, st, n, rank, (const T*)dF, ldf, (const T*)d_gamma, b, ldb, nrhs));
+        TRY(apply_q_local(c, st, m, rank, (const T*)dA, lda, b, ldb, nrhs, 0));
+        // b[0:n] <- Z [U^{-H} b[0:rank]; 0] from the factorisation (F, gamma) of R_r^H, rows n..m-1 of b untouched; then into xbuf,
+        // which the scatter reads while it writes b
+        TRY(solve_adj_local(c, st, n, rank, (const T*)dF, ldf, (const T*)d_gamma, b, ldb, nrhs));
         CU(cudaMemcpy2DAsync(z, (size_t)n * sizeof(T), b, (size_t)ldb * sizeof(T), (size_t)n * sizeof(T), nrhs, cudaMemcpyDeviceToDevice, st));
     }
     return qrcp_scatter(c, st, n, rank > 0 ? n : 0, z, n, d_jpvt, b, ldb, nrhs);
@@ -2755,18 +2674,18 @@ int dhqr_qr_append_f64(dhqr_handle c, int64_t n, int64_t k, double* dR, int64_t 
                        double* d_vtop, void* stream) {
     TRY(check_append_head(c, n, k));
     if (n > 0 && !dR) return set_err(-4, "null R");
-    TRY(check_qrcp_ptr(dR, -4, "R"));
+    TRY(check_elem_ptr<double>(dR, -4, "R"));
     if (ldr < std::max<int64_t>(1, n)) return set_err(-5, "ldr < max(1,n)");
     if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
-    TRY(check_qrcp_ptr(d_alpha, -6, "alpha"));
+    TRY(check_elem_ptr<double>(d_alpha, -6, "alpha"));
     const size_t rbytes = n > 0 ? ((size_t)(n - 1) * ldr + n) * 8 : 0, abytes = (size_t)n * 8;
     if (n > 0 && k > 0 && !dB) return set_err(-7, "null B");
-    TRY(check_qrcp_ptr(dB, -7, "B"));
+    TRY(check_elem_ptr<double>(dB, -7, "B"));
     const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0;
     if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-7, "B overlaps R or alpha");
     if (ldb < std::max<int64_t>(1, k)) return set_err(-8, "ldb < max(1,k)");
     if (n > 0 && !d_vtop) return set_err(-9, "null vtop");
-    TRY(check_qrcp_ptr(d_vtop, -9, "vtop"));
+    TRY(check_elem_ptr<double>(d_vtop, -9, "vtop"));
     if (k > 0 && (spans_overlap(d_vtop, abytes, dR, rbytes) || spans_overlap(d_vtop, abytes, d_alpha, abytes) ||
                   spans_overlap(d_vtop, abytes, dB, bbytes)))
         return set_err(-9, "vtop overlaps R, alpha or B");
@@ -2779,19 +2698,19 @@ static int apply_append(dhqr_context* c, int64_t n, int64_t k, const double* dB,
                         int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream, int trans) {
     TRY(check_append_head(c, n, k));
     if (n > 0 && k > 0 && !dB) return set_err(-4, "null B");
-    TRY(check_qrcp_ptr(dB, -4, "B"));
+    TRY(check_elem_ptr<double>(dB, -4, "B"));
     if (ldb < std::max<int64_t>(1, k)) return set_err(-5, "ldb < max(1,k)");
     if (n > 0 && !d_vtop) return set_err(-6, "null vtop");
-    TRY(check_qrcp_ptr(d_vtop, -6, "vtop"));
+    TRY(check_elem_ptr<double>(d_vtop, -6, "vtop"));
     const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0, vbytes = (size_t)n * 8;
     const size_t cbytes = (n > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * ldc + n) * 8 : 0;
     const size_t ebytes = (k > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * lde + k) * 8 : 0;
     if (n > 0 && nrhs > 0 && !d_c) return set_err(-7, "null c");
-    TRY(check_qrcp_ptr(d_c, -7, "c"));
+    TRY(check_elem_ptr<double>(d_c, -7, "c"));
     if (spans_overlap(d_c, cbytes, dB, bbytes) || spans_overlap(d_c, cbytes, d_vtop, vbytes)) return set_err(-7, "c overlaps B or vtop");
     if (ldc < std::max<int64_t>(1, n)) return set_err(-8, "ldc < max(1,n)");
     if (k > 0 && nrhs > 0 && !d_e) return set_err(-9, "null e");
-    TRY(check_qrcp_ptr(d_e, -9, "e"));
+    TRY(check_elem_ptr<double>(d_e, -9, "e"));
     if (spans_overlap(d_e, ebytes, dB, bbytes) || spans_overlap(d_e, ebytes, d_vtop, vbytes) || spans_overlap(d_e, ebytes, d_c, cbytes))
         return set_err(-9, "e overlaps B, vtop or c");
     if (lde < std::max<int64_t>(1, k)) return set_err(-10, "lde < max(1,k)");
@@ -2985,17 +2904,39 @@ int dhqr_ldiv_host_f64(dhqr_handle c, int64_t m, int64_t n, const double* hA, in
 }
 
 // ---- primitives ---------------------------------------------------------------------------------
-int dhqr_partialdot_f64(dhqr_handle c, const double* d_a, const double* d_b, int64_t i0, int64_t i1, double* d_out,
-                        void* stream) {
+extern "C++" {   // as for form_q above
+
+template <typename T>
+static int partialdot(dhqr_context* c, const void* d_a, const void* d_b, int64_t i0, int64_t i1, void* d_out, void* stream) {
     if (!c) return set_err(-1, "null handle");
     if (!d_a) return set_err(-2, "null a");
     if (!d_b) return set_err(-3, "null b");
     if (i0 < 0) return set_err(-4, "i0 < 0");
     if (i1 < i0) return set_err(-5, "i1 < i0");
     if (!d_out) return set_err(-6, "null out");
+    if (std::is_same<T, double2>::value) {                  // Float64 pointers are not checked for alignment here
+        TRY(check_elem_ptr<T>(d_a, -2, "a"));
+        TRY(check_elem_ptr<T>(d_b, -3, "b"));
+        TRY(check_elem_ptr<T>(d_out, -6, "out"));
+    }
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
-    return launch(c, st, "k_partialdot", 0.0, [&](CwtSlot) { k_partialdot<<<1, 1024, 0, st>>>(d_a, d_b, i0, i1, d_out); });
+    return launch(c, st, kname<T>("k_partialdot", "k_partialdot_c"), 0.0, [&](CwtSlot) {
+        // k_partialdot_c sums its block in its own order, so the kernels stay one per type
+        if constexpr (std::is_same<T, double>::value) k_partialdot<<<1, 1024, 0, st>>>((const T*)d_a, (const T*)d_b, i0, i1, (T*)d_out);
+        else k_partialdot_c<<<1, 1024, 0, st>>>((const T*)d_a, (const T*)d_b, i0, i1, (T*)d_out);
+    });
+}
+
+}  // extern "C++"
+
+int dhqr_partialdot_f64(dhqr_handle c, const double* d_a, const double* d_b, int64_t i0, int64_t i1, double* d_out,
+                        void* stream) {
+    return partialdot<double>(c, d_a, d_b, i0, i1, d_out, stream);
+}
+
+int dhqr_partialdot_c64(dhqr_handle c, const void* d_a, const void* d_b, int64_t i0, int64_t i1, void* d_out, void* stream) {
+    return partialdot<double2>(c, d_a, d_b, i0, i1, d_out, stream);
 }
 
 int dhqr_fill_uniform_f64(dhqr_handle c, uint64_t seed, int64_t i0, int64_t j0, int64_t m, int64_t n, double* dA,

@@ -7,9 +7,11 @@
 // reflectors IS the real block-reflector update with V^ = [v1_r, v1_i, v2_r, v2_i, ...] (2 kb real vectors) on the real view of
 // the trailing matrix (2m x n, leading dimension 2 lda), T^{-1} = I + striu(V^' V^): the fp64 tensor-pipe GEMM pair of the real
 // path is reused as is (this is the 4M real decomposition of the complex rank-k update).  New here: the complex panel
-// factorisation (column by column, S:127-135 with alphafactor(::Complex) S:9), the packing of V^, the complex back-substitution
-// (S:256-282) and the conjugating partialdot primitive.
+// factorisation (column by column, S:127-135 with alphafactor(::Complex) S:9), the packing of V^ and the conjugating partialdot
+// primitive.  The back- and forward-substitution steps (S:256-282) are here too, written once for Float64 and ComplexF64.
 #pragma once
+#include <type_traits>
+
 #include "dhqr_kernels.cuh"
 
 namespace dhqr {
@@ -127,49 +129,51 @@ __global__ void k_pack_c(const double2* __restrict__ A, int64_t lda, int64_t mpc
     }
 }
 
-// back-substitution step (S:256-282) for complex R = triu(A,1) + diag(alpha): like k_backsolve_step
-__global__ void __launch_bounds__(256) k_backsolve_step_c(const double2* __restrict__ Ablk, int64_t lda, const double2* __restrict__ alpha,
-                                                          double2* __restrict__ y, int64_t ldy, int nrhs, double2* __restrict__ x,
-                                                          int64_t ldx, int64_t c0, int bs) {
-    __shared__ double2 sx[BS_BLK];
-    const int tid = threadIdx.x, lane = tid & 31;
-    for (int rhs = 0; rhs < nrhs; ++rhs) {
-        double2* yr = y + (int64_t)rhs * ldy;
-        if (tid < 32) {
-            double2 yk = lane < bs ? yr[c0 + lane] : make_double2(0.0, 0.0);
-            for (int i = bs - 1; i >= 0; --i) {
-                const double2 al = alpha[c0 + i];
-                const double den = al.x * al.x + al.y * al.y;
-                const double nx = __shfl_sync(0xffffffffu, yk.x, i), ny = __shfl_sync(0xffffffffu, yk.y, i);
-                const double2 xi = make_double2((nx * al.x + ny * al.y) / den, (ny * al.x - nx * al.y) / den);   // (nx + i ny) / alpha
-                if (lane == i) yk = xi;
-                if (lane < i) {
-                    const double2 t = cmul(Ablk[(int64_t)i * lda + c0 + lane], xi);
-                    yk.x -= t.x;
-                    yk.y -= t.y;
-                }
-            }
-            sx[lane] = yk;
-        }
-        __syncthreads();
-        if (blockIdx.x == 0 && tid < bs) x[(int64_t)rhs * ldx + c0 + tid] = sx[tid];
-        for (int64_t r = (int64_t)blockIdx.x * blockDim.x + tid; r < c0; r += (int64_t)gridDim.x * blockDim.x) {
-            double2 acc = make_double2(0.0, 0.0);
-            for (int k = 0; k < bs; ++k) {
-                const double2 t = cmul(Ablk[(int64_t)k * lda + r], sx[k]);
-                acc.x += t.x;
-                acc.y += t.y;
-            }
-            yr[r].x -= acc.x;
-            yr[r].y -= acc.y;
-        }
-        __syncthreads();
-    }
+// ---- substitution steps, T = double or double2 ---------------------------------------------------------------------------------
+// What the two step kernels below need of their element type, in overloads.  Each double2 helper fixes the order of its two
+// component operations, so every instantiation compiles to the kernel it replaces.
+template <typename T> __device__ T zero();
+template <> __device__ __forceinline__ double zero<double>() { return 0.0; }
+template <> __device__ __forceinline__ double2 zero<double2>() { return make_double2(0.0, 0.0); }
+
+// x -= y and x += y for double2 (y by reference: a copy of it would change the generated code)
+__device__ __forceinline__ void operator-=(double2& x, const double2& y) { x.x -= y.x; x.y -= y.y; }
+__device__ __forceinline__ void operator+=(double2& x, const double2& y) { x.x += y.x; x.y += y.y; }
+
+// a b and conj(a) b
+__device__ __forceinline__ double mul(double a, double b) { return a * b; }
+__device__ __forceinline__ double2 mul(double2 a, double2 b) { return cmul(a, b); }
+__device__ __forceinline__ double conj_mul(double a, double b) { return a * b; }
+__device__ __forceinline__ double2 conj_mul(double2 a, double2 b) { return cmulc(a, b); }
+
+// lane i's v in every lane of the warp, and the sum of v over the warp
+__device__ __forceinline__ double shfl(double v, int i) { return __shfl_sync(0xffffffffu, v, i); }
+__device__ __forceinline__ double2 shfl(const double2& v, int i) {
+    const double x = __shfl_sync(0xffffffffu, v.x, i);
+    const double y = __shfl_sync(0xffffffffu, v.y, i);
+    return make_double2(x, y);
+}
+__device__ __forceinline__ double2 warp_sum(const double2& v) {
+    const double x = warp_sum(v.x);
+    const double y = warp_sum(v.y);
+    return make_double2(x, y);
 }
 
-// n / conj(a) by Smith's algorithm: the ratio of the smaller to the larger part of a is formed first, so neither |a|^2 nor a
-// partial product overflows or underflows when n and a lie many decades apart (columns scaled by 10^+-120).  a = 0 gives NaN.
-__device__ __forceinline__ double2 cdiv_conj(double2 n, double2 a) {
+// lane i's y over *a in every lane of the warp: the pivot step of the back-substitution.  For double2 *a and |*a|^2 (unscaled) come
+// before the shuffles.
+__device__ __forceinline__ double shfl_div_alpha(double y, int i, const double* a) { return __shfl_sync(0xffffffffu, y, i) / *a; }
+__device__ __forceinline__ double2 shfl_div_alpha(const double2& y, int i, const double2* a) {
+    const double2 al = *a;
+    const double den = al.x * al.x + al.y * al.y;
+    const double nx = __shfl_sync(0xffffffffu, y.x, i), ny = __shfl_sync(0xffffffffu, y.y, i);
+    return make_double2((nx * al.x + ny * al.y) / den, (ny * al.x - nx * al.y) / den);
+}
+
+// n / conj(a) of the forward substitution.  For double2 by Smith's algorithm: the ratio of the smaller to the larger part of a is
+// formed first, so neither |a|^2 nor a partial product overflows or underflows when n and a lie many decades apart (columns scaled
+// by 10^+-120).  a = 0 gives NaN.
+__device__ __forceinline__ double div_conj(double n, double a) { return n / a; }
+__device__ __forceinline__ double2 div_conj(double2 n, double2 a) {
     const double p = a.x, q = -a.y;                                          // conj(a) = p + i q
     if (fabs(p) >= fabs(q)) {
         const double r = q / p, d = p + q * r;
@@ -179,44 +183,72 @@ __device__ __forceinline__ double2 cdiv_conj(double2 n, double2 a) {
     return make_double2((n.x * r + n.y) / d, (n.y * r - n.x) / d);
 }
 
-// forward substitution with R^H (z = R^{-H} y) for complex R = triu(A,1) + diag(alpha): like k_forwardsolve_step, with the
-// conjugated products z_i = (y_i - sum_{j<i} conj(R[j,i]) z_j) / conj(alpha_i)
-__global__ void __launch_bounds__(256, 1) k_forwardsolve_step_c(const double2* __restrict__ A, int64_t lda, const double2* __restrict__ alpha,
-                                                             double2* __restrict__ y, int64_t ldy, int nrhs, double2* __restrict__ x,
-                                                             int64_t ldx, int64_t c0, int bs, int64_t n) {
-    __shared__ double2 sx[BS_BLK], sD[BS_BLK][BS_BLK + 1];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int e = tid; e < BS_BLK * BS_BLK; e += 256) {                      // sD[j][i] = R[c0 + i, c0 + j], i < j: column j of A
-        const int i = e & 31, j = e >> 5;
-        sD[j][i] = (i < j && j < bs) ? A[(c0 + j) * lda + c0 + i] : make_double2(0.0, 0.0);
-    }
-    __syncthreads();
+// Back-substitution step (S:256-282), column oriented, for R = triu(A, 1) + diag(alpha): solve the bs x bs diagonal block
+//   x_blk = R_bb^{-1} y_blk  in every CTA (one warp), then y[0:c0) -= R[0:c0, blk] x_blk on the CTA's slice of rows.  CTA 0
+// publishes x_blk.  Ablk points at (row 0, first column of the block) in local storage; c0 is the global index of that column.
+constexpr int BS_BLK = 32;
+template <typename T>
+__global__ void __launch_bounds__(256) k_backsolve_step(const T* __restrict__ Ablk, int64_t lda, const T* __restrict__ alpha,
+                                                        T* __restrict__ y, int64_t ldy, int nrhs, T* __restrict__ x, int64_t ldx,
+                                                        int64_t c0, int bs) {
+    __shared__ T sx[BS_BLK];
+    const int tid = threadIdx.x, lane = tid & 31;
     for (int rhs = 0; rhs < nrhs; ++rhs) {
-        double2* yr = y + (int64_t)rhs * ldy;
+        T* yr = y + (int64_t)rhs * ldy;
         if (tid < 32) {
-            double2 yk = lane < bs ? yr[c0 + lane] : make_double2(0.0, 0.0);
-            for (int i = 0; i < bs; ++i) {
-                const double nx = __shfl_sync(0xffffffffu, yk.x, i), ny = __shfl_sync(0xffffffffu, yk.y, i);
-                const double2 zi = cdiv_conj(make_double2(nx, ny), alpha[c0 + i]);
-                if (lane == i) yk = zi;
-                if (lane > i) {
-                    const double2 t = cmulc(sD[lane][i], zi);
-                    yk.x -= t.x;
-                    yk.y -= t.y;
-                }
+            T yk = lane < bs ? yr[c0 + lane] : zero<T>();
+            for (int i = bs - 1; i >= 0; --i) {
+                const T xi = shfl_div_alpha(yk, i, alpha + c0 + i);
+                if (lane == i) yk = xi;
+                if (lane < i) yk -= mul(Ablk[(int64_t)i * lda + c0 + lane], xi);
             }
             sx[lane] = yk;
         }
         __syncthreads();
         if (blockIdx.x == 0 && tid < bs) x[(int64_t)rhs * ldx + c0 + tid] = sx[tid];
-        const double2 zl = lane < bs ? sx[lane] : make_double2(0.0, 0.0);
-        for (int64_t r = c0 + bs + (int64_t)blockIdx.x * 8 + warp; r < n; r += (int64_t)gridDim.x * 8) {
-            const double2 t = lane < bs ? cmulc(A[r * lda + c0 + lane], zl) : make_double2(0.0, 0.0);
-            const double sre = warp_sum(t.x), sim = warp_sum(t.y);
-            if (lane == 0) {
-                yr[r].x -= sre;
-                yr[r].y -= sim;
+        for (int64_t r = (int64_t)blockIdx.x * blockDim.x + tid; r < c0; r += (int64_t)gridDim.x * blockDim.x) {
+            T acc = zero<T>();
+            for (int k = 0; k < bs; ++k) acc += mul(Ablk[(int64_t)k * lda + r], sx[k]);
+            yr[r] -= acc;
+        }
+        __syncthreads();
+    }
+}
+
+// Forward substitution with R^H (the adjoint solve z = R^{-H} y), column oriented: the mirror of k_backsolve_step.  Every CTA
+// solves the bs x bs diagonal block z_i = (y_i - sum_{j<i} conj(R[j,i]) z_j) / conj(alpha_i) (one warp, first row to last), then
+// y[r] -= sum_k conj(R[c0 + k, r]) z_k for the rows r in [c0 + bs, n) of its warps (one warp per row: row r of R^H is column r of
+// A, so the bs entries it needs are contiguous and a warp reads them in one coalesced load).  CTA 0 publishes z_blk.
+// The double2 kernel keeps its minimum of one CTA per SM (0 leaves the double one without a minimum).
+template <typename T>
+__global__ void __launch_bounds__(256, std::is_same<T, double2>::value ? 1 : 0)
+    k_forwardsolve_step(const T* __restrict__ A, int64_t lda, const T* __restrict__ alpha, T* __restrict__ y, int64_t ldy, int nrhs,
+                        T* __restrict__ x, int64_t ldx, int64_t c0, int bs, int64_t n) {
+    __shared__ T sx[BS_BLK], sD[BS_BLK][BS_BLK + 1];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int e = tid; e < BS_BLK * BS_BLK; e += 256) {                      // sD[j][i] = R[c0 + i, c0 + j], i < j: column j of A
+        const int i = e & 31, j = e >> 5;
+        sD[j][i] = (i < j && j < bs) ? A[(c0 + j) * lda + c0 + i] : zero<T>();
+    }
+    __syncthreads();
+    for (int rhs = 0; rhs < nrhs; ++rhs) {
+        T* yr = y + (int64_t)rhs * ldy;
+        if (tid < 32) {
+            T yk = lane < bs ? yr[c0 + lane] : zero<T>();
+            for (int i = 0; i < bs; ++i) {
+                const T zi = div_conj(shfl(yk, i), alpha[c0 + i]);
+                if (lane == i) yk = zi;
+                if (lane > i) yk -= conj_mul(sD[lane][i], zi);
             }
+            sx[lane] = yk;
+        }
+        __syncthreads();
+        if (blockIdx.x == 0 && tid < bs) x[(int64_t)rhs * ldx + c0 + tid] = sx[tid];
+        const T zl = lane < bs ? sx[lane] : zero<T>();
+        for (int64_t r = c0 + bs + (int64_t)blockIdx.x * 8 + warp; r < n; r += (int64_t)gridDim.x * 8) {
+            const T t = lane < bs ? conj_mul(A[r * lda + c0 + lane], zl) : zero<T>();
+            const T acc = warp_sum(t);
+            if (lane == 0) yr[r] -= acc;
         }
         __syncthreads();
     }

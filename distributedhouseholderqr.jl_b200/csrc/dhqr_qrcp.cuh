@@ -66,20 +66,15 @@ struct QrcpArgs {
     QrcpCtl* ctl;
 };
 
-template <typename T> __device__ T qp_zero();
-template <> __device__ __forceinline__ double qp_zero<double>() { return 0.0; }
-template <> __device__ __forceinline__ double2 qp_zero<double2>() { return make_double2(0.0, 0.0); }
-
 __device__ __forceinline__ double qp_abs2(double v) { return v * v; }
 __device__ __forceinline__ double qp_abs2(double2 v) { return v.x * v.x + v.y * v.y; }
 
 __device__ __forceinline__ double2 cmulcb(double2 a, double2 b) {   // a * conj(b)
     return make_double2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y);
 }
-// a conj(b), and x -= y for double2 (y by reference: a copy of it would change the generated code)
+// a conj(b)
 __device__ __forceinline__ double qp_mul_conj(double a, double b) { return a * b; }
 __device__ __forceinline__ double2 qp_mul_conj(double2 a, double2 b) { return cmulcb(a, b); }
-__device__ __forceinline__ void operator-=(double2& x, const double2& y) { x.x -= y.x; x.y -= y.y; }
 
 // alpha and the scale 1 / sqrt(nrm (nrm + |x0|)) of the reflector of a column with leading entry x0 and norm nrm > 0; for double2
 // alpha is k_house1_c's (house_alpha, dhqr_complex.cuh)
@@ -219,7 +214,7 @@ __global__ void __launch_bounds__(QP_THREADS) k_qrcp_pivot(QrcpArgs<T> a) {
         T al;
         double sc;
         if (vmax == 0.0 || nrm == 0.0) {         // every remaining column is zero in working precision: H = I
-            al = qp_zero<T>(); sc = 0.0;
+            al = zero<T>(); sc = 0.0;
         } else {
             qp_alpha(x0, nrm, al, sc);
         }
@@ -513,7 +508,7 @@ __global__ void k_qrcp_scatter(const T* __restrict__ z, int64_t ldz, const int64
     if (i >= n) return;
     const int64_t d = jpvt[i];
     if (d < 0 || d >= n) return;
-    b[d + (int64_t)blockIdx.y * ldb] = i < rank ? z[i + (int64_t)blockIdx.y * ldz] : qp_zero<T>();
+    b[d + (int64_t)blockIdx.y * ldb] = i < rank ? z[i + (int64_t)blockIdx.y * ldz] : zero<T>();
 }
 
 // Complete orthogonal decomposition (dhqr_cod_*): F (n x rank) <- R_r^H, R_r = rows [0, rank) of R = triu(A, 1) + diag(alpha), so
@@ -537,7 +532,7 @@ __global__ void __launch_bounds__(CP_TILE * CP_ROWS) k_cod_pack(const T* __restr
     }
     for (int r = ty; r < CP_TILE; r += CP_ROWS) {
         const int64_t i = i0 + r, j = j0 + tx;                         // row j of column i of F
-        if (i < rank && j < n) F[j + i * ldf] = lower ? t[tx][r] : qp_zero<T>();
+        if (i < rank && j < n) F[j + i * ldf] = lower ? t[tx][r] : zero<T>();
     }
 }
 
