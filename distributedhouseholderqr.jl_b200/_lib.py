@@ -52,6 +52,8 @@ SIGNATURES = {
     "dhqr_qr_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp],
     "dhqr_apply_qt_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
     "dhqr_apply_q_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
+    "dhqr_qr_downdate_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp],
+    "dhqr_apply_downdate_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

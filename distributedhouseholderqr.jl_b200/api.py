@@ -701,11 +701,11 @@ def fill_uniform_(A: torch.Tensor, seed: int, i0: int = 0, j0: int = 0, handle: 
 
 
 # --------------------------------------------------------------------------------------------
-# new rows into an existing factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10
+# new rows into an existing factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10, and rows out of it again (§2.11)
 # --------------------------------------------------------------------------------------------
-class AppendedRows:
-    """[R; B] = Q~ [R'; 0] from ``append_rows_``: ``.B`` holds the reflector tails V2 (k x n, the caller's block, overwritten) and
-    ``.vtop`` their tops, so H~_j = I - v~_j v~_j' with v~_j = vtop[j] on row j of R and B[:, j] on the new rows."""
+class _RowReflectors:
+    """The reflectors of an append or a downdate: ``.B`` holds their tails V2 (k x n, the caller's block, overwritten) and
+    ``.vtop`` their tops."""
 
     def __init__(self, B, vtop, handle: Handle):
         self.B = B
@@ -723,6 +723,11 @@ class AppendedRows:
                       C.c_void_p(c.data_ptr()), ldc, C.c_void_p(e.data_ptr()), lde, nrhs, _stream_ptr(self.B.device))
         return c, e
 
+
+class AppendedRows(_RowReflectors):
+    """[R; B] = Q~ [R'; 0] from ``append_rows_``: ``.B`` holds the reflector tails V2 (k x n, the caller's block, overwritten) and
+    ``.vtop`` their tops, so H~_j = I - v~_j v~_j' with v~_j = vtop[j] on row j of R and B[:, j] on the new rows."""
+
     def apply_qt_(self, c: torch.Tensor, e: torch.Tensor):
         """[c; e] <- Q~' [c; e] in place: c has n rows, e has k rows (vectors, or column-major blocks of equal width)."""
         return self._apply("dhqr_apply_qt_append_f64", c, e)
@@ -732,24 +737,44 @@ class AppendedRows:
         return self._apply("dhqr_apply_q_append_f64", c, e)
 
 
-def append_rows_(H, B: torch.Tensor, handle: Optional[Handle] = None) -> AppendedRows:
-    """Fold the k new rows ``B`` (a column-major float64 CUDA tensor, k x n) into the factorisation ``H`` (a single-GPU
-    DistributedHouseholderQRStruct, or a pair (A, α)): afterwards (H.A, H.α) hold R' of [R; B] = Q~ [R'; 0] in A's strict upper
-    triangle and α, while A's diagonal and lower trapezoid (the original reflectors) are left as they are.  ``B`` is overwritten
-    with the reflector tails.  k may not exceed the handle's option "append_max_rows" (StreamingLeastSquares splits larger
-    blocks).  Stream-ordered, no synchronisation."""
+class DowndatedRows(_RowReflectors):
+    """Theta [R; Z] = [R'; 0] from ``downdate_rows_``: ``.B`` holds the hyperbolic reflector tails V2 (k x n, the caller's block,
+    overwritten), ``.vtop`` their tops, so Theta_j = I - v~_j v~_j' J with J = diag(I_n, -I_k).  ``.info`` is a one-element int64
+    CUDA tensor: 0, or the 1-based column at which the removal proved impossible (R'R - Z'Z not positive definite); reading it
+    synchronises with the device."""
+
+    def __init__(self, B, vtop, info, handle: Handle):
+        super().__init__(B, vtop, handle)
+        self.info = info
+
+    def apply_(self, c: torch.Tensor, e: torch.Tensor):
+        """[c; e] <- Theta [c; e] in place: c = (Q'b)[0:n] (n rows) and e the removed rows' right-hand sides (k rows) become c' and
+        e'; x' = R'^{-1} c', and the residual sum of squares drops by ||e'||^2."""
+        return self._apply("dhqr_apply_downdate_f64", c, e)
+
+
+def _row_block_args(H, B: torch.Tensor, handle: Optional[Handle], what: str):
     A, alpha = (H.A, H.α) if isinstance(H, DistributedHouseholderQRStruct) else H
     if isinstance(A, ColumnBlockMatrix) or not isinstance(A, torch.Tensor) or not A.is_cuda:
-        raise TypeError("append_rows_ works on a single-GPU factorisation held in a CUDA tensor")
+        raise TypeError(f"{what} works on a single-GPU factorisation held in a CUDA tensor")
     if A.dtype != torch.float64 or alpha.dtype != torch.float64 or B.dtype != torch.float64:
-        raise TypeError("append_rows_ is Float64 only")
+        raise TypeError(f"{what} is Float64 only")
     n = alpha.shape[0]
     if A.shape[1] != n or A.shape[0] < n:
         raise ValueError("A must have len(alpha) columns and at least as many rows")
     if B.dim() != 2 or B.shape[1] != n:
         raise ValueError(f"B must be a (k, {n}) column-major block")
     h = handle or getattr(H, "handle", None) or default_handle(A.device.index)
-    k = B.shape[0]
+    return A, alpha, n, B.shape[0], h
+
+
+def append_rows_(H, B: torch.Tensor, handle: Optional[Handle] = None) -> AppendedRows:
+    """Fold the k new rows ``B`` (a column-major float64 CUDA tensor, k x n) into the factorisation ``H`` (a single-GPU
+    DistributedHouseholderQRStruct, or a pair (A, α)): afterwards (H.A, H.α) hold R' of [R; B] = Q~ [R'; 0] in A's strict upper
+    triangle and α, while A's diagonal and lower trapezoid (the original reflectors) are left as they are.  ``B`` is overwritten
+    with the reflector tails.  k may not exceed the handle's option "append_max_rows" (StreamingLeastSquares splits larger
+    blocks).  Stream-ordered, no synchronisation."""
+    A, alpha, n, k, h = _row_block_args(H, B, handle, "append_rows_")
     vtop = torch.zeros(n, dtype=torch.float64, device=A.device)
     with torch.cuda.device(A.device):
         _lib.call("dhqr_qr_append_f64", h.raw, n, k, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
@@ -757,11 +782,36 @@ def append_rows_(H, B: torch.Tensor, handle: Optional[Handle] = None) -> Appende
     return AppendedRows(B, vtop, h)
 
 
+def downdate_rows_(H, Z: torch.Tensor, handle: Optional[Handle] = None) -> DowndatedRows:
+    """Remove the k rows ``Z`` (a column-major float64 CUDA tensor, k x n) from the factorisation ``H`` (as for append_rows_):
+    afterwards (H.A, H.α) hold R' with R''R' = R'R - Z'Z in A's strict upper triangle and α; A's diagonal and lower trapezoid are
+    left as they are.  ``Z`` is overwritten with the reflector tails.  Only rows that were folded into R may be removed: when the
+    removal is impossible, ``.info`` names the first column that showed it, and from that column on α is NaN.  k is capped by
+    "append_max_rows" as for the append.  Stream-ordered, no synchronisation."""
+    A, alpha, n, k, h = _row_block_args(H, Z, handle, "downdate_rows_")
+    vtop = torch.zeros(n, dtype=torch.float64, device=A.device)
+    info = torch.zeros(1, dtype=torch.int64, device=A.device)     # an n = 0 or k = 0 no-op leaves it untouched
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_qr_downdate_f64", h.raw, n, k, C.c_void_p(A.data_ptr()), _lda(A), C.c_void_p(alpha.data_ptr()),
+                  C.c_void_p(Z.data_ptr()), _lda(Z), C.c_void_p(vtop.data_ptr()), C.c_void_p(info.data_ptr()), _stream_ptr(A.device))
+    return DowndatedRows(Z, vtop, info, h)
+
+
 class StreamingLeastSquares:
     """min ||A x - b|| for an A of any height, fed block by block: each block of rows is folded into R (starting from R = 0) and
     its right-hand sides into c = (Q'b)[0:n]; what the rotation moves out of reach adds to the residual.  Blocks above the row cap
     of one append are split.  ``add`` takes CUDA tensors or Fortran-ordered numpy arrays (uploaded); ``solve`` returns x as an
-    (n, nrhs) tensor (a length-n vector for nrhs = 1)."""
+    (n, nrhs) tensor (a length-n vector for nrhs = 1).  ``remove`` takes rows out again, so ``add`` of the newest block followed
+    by ``remove`` of the oldest keeps a sliding window::
+
+        ls = StreamingLeastSquares(n)
+        for A_blk, b_blk in blocks:
+            ls.add(A_blk, b_blk)
+            window.append((A_blk, b_blk))
+            if len(window) > w:
+                ls.remove(*window.pop(0))
+            x = ls.solve()
+    """
 
     def __init__(self, n: int, nrhs: int = 1, device=0, handle: Optional[Handle] = None):
         self.n, self.nrhs = int(n), int(nrhs)
@@ -794,6 +844,45 @@ class StreamingLeastSquares:
         self.rows += k
         return self
 
+    def remove(self, A_blk, b_blk) -> "StreamingLeastSquares":
+        """Take rows ``A_blk`` (k x n) with right-hand sides ``b_blk`` out of the problem again: they must be rows that were added.
+        R, α and c are downdated as copies and swapped in only when every block succeeded; the call reads the downdates' status
+        once (one synchronisation).  An impossible removal (the rows were never added, or the remaining rows are rank-deficient)
+        raises ValueError and leaves the solver as it was."""
+        A_blk = torch.as_tensor(A_blk)
+        b_blk = torch.as_tensor(b_blk)
+        if b_blk.dim() == 1:
+            b_blk = b_blk[:, None]
+        k = A_blk.shape[0]
+        if A_blk.dim() != 2 or A_blk.shape[1] != self.n or tuple(b_blk.shape) != (k, self.nrhs):
+            raise ValueError(f"need a (k, {self.n}) block and its (k, {self.nrhs}) right-hand sides")
+        if k > self.rows:
+            raise ValueError(f"cannot remove {k} rows from a problem of {self.rows}")
+        A = colmajor_empty(self.n, self.n, self.device)
+        A.copy_(self.A)
+        α, c = self.α.clone(), colmajor_empty(self.n, self.nrhs, self.device)
+        c.copy_(self.c)
+        drop = torch.zeros_like(self._ss)
+        infos = []
+        for r0 in range(0, k, self._cap):
+            r1 = min(k, r0 + self._cap)
+            Z = to_colmajor(A_blk[r0:r1], device=self.device)
+            e = to_colmajor(b_blk[r0:r1], device=self.device)
+            d = downdate_rows_((A, α), Z, self.handle)
+            d.apply_(c, e)
+            drop += (e * e).sum(0)
+            infos.append(d.info)
+        info = torch.cat(infos).cpu() if infos else torch.zeros(0, dtype=torch.int64)
+        bad = info.nonzero()
+        if len(bad):
+            b = int(bad[0, 0])
+            raise ValueError(f"removing these rows is impossible: the downdate fails at column {int(info[b])} (rows "
+                             f"{b * self._cap}..{min(k, (b + 1) * self._cap) - 1} of the block); were they ever added?")
+        self.A, self.α, self.c = A, α, c
+        self._ss -= drop
+        self.rows -= k
+        return self
+
     @property
     def alpha(self):
         return self.α
@@ -811,5 +900,6 @@ class StreamingLeastSquares:
         return x[:, 0] if self.nrhs == 1 else x
 
     def residual_norm(self) -> torch.Tensor:
-        """||A x - b|| per right-hand side at the least-squares solution, accumulated as the blocks were folded in."""
-        return self._ss.sqrt()
+        """||A x - b|| per right-hand side at the least-squares solution, accumulated as the blocks were folded in (and taken out:
+        rounding can then take the accumulated sum of squares slightly below 0 when the residual is about 0, so it is clamped)."""
+        return self._ss.clamp(min=0).sqrt()

@@ -310,9 +310,12 @@ static int set_attrs(dhqr_context* c) {
     CU(cudaFuncSetAttribute(k_tinv<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(32)));
     CU(cudaFuncSetAttribute(k_ymake<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(128)));
     CU(cudaFuncSetAttribute(k_ymake<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(32)));
+    CU(cudaFuncSetAttribute(k_tinv<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(128)));
+    CU(cudaFuncSetAttribute(k_ymake<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ymake(128)));
     CU(cudaFuncSetAttribute(k_ymake2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_YMAKE2));
     CU(cudaFuncSetAttribute(k_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
-    CU(cudaFuncSetAttribute(k_tp_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
+    CU(cudaFuncSetAttribute(k_tp_panel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
+    CU(cudaFuncSetAttribute(k_tp_panel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 184 * 1024));
     CU(cudaFuncSetAttribute(k_chol128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_WIDE1));
     CU(cudaFuncSetAttribute(k_hr128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_WIDE1));
     CU(cudaFuncSetAttribute(k_vpk_rmul, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_RMUL));
@@ -500,7 +503,7 @@ static int apply_block_reflector(dhqr_context* c, cudaStream_t st, const double*
     const int ygrid = (ncols + YCOLS - 1) / YCOLS;
     if (small && !reuse_T) {
         TRY(launch(c, st, "k_mid32", 0.0, [&](CwtSlot) {
-            k_mid32<<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, linv, trans);
+            k_mid32<><<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, linv, trans);
         }));
     } else {
         const int64_t nelem = (int64_t)next * NBPK;
@@ -2547,14 +2550,16 @@ int dhqr_solve_cod_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const 
     return cod_solve<double2>(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, d_b, ldb, nrhs, stream);
 }
 
-// ---- triangular-pentagonal QR: fold new rows into a factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10 ---------------------
+// ---- triangular-pentagonal QR: fold new rows into a factorisation (LAPACK dtpqrt / dtpmqrt), DESIGN §2.10, or delete rows (§2.11) -
 // One block reflector of the structured update, on the stacked operand [X; C]: X = the block's kb rows of R (or of c), C = k rows of B
 // (or of e).  V~ = [diag(vtop); V2] with V2 = packed columns [voff, voff + nbp) of vpk.  The existing sequence of
 // apply_block_reflector on C with V = V2, plus the vtop rows in two places: diag(vtop) X as one more split-K partial of W (so the
 // fixed-order reduction adds it), and X += diag(vtop) Y after Y is formed.  T comes from V2'V2 unchanged: off the diagonal it equals
 // V~'V~, and T' is built from the strict triangle alone.  trans = 1: Q~ instead of Q~'.
+// hyp (the downdate, §2.11): Theta = I - V~ T' V~'J with T^{-1} = I - striu(V2'V2); the W partial is -diag(vtop) X, so the reduced
+// W is -(V~'J [X; C]), and Y = +T'W.  The launches are the append's, one for one.
 static int tp_block_update(dhqr_context* c, cudaStream_t st, const double* vpk, int voff, int nbp, int kb, const double* vtop, int64_t k,
-                           double* C, int64_t ldc, double* X, int64_t ldx, int ncols, int trans) {
+                           double* C, int64_t ldc, double* X, int64_t ldx, int ncols, int trans, bool hyp) {
     if (ncols <= 0 || k <= 0) return 0;
     auto& w = c->ws[0];
     const bool small = (nbp <= 32);
@@ -2567,19 +2572,28 @@ static int tp_block_update(dhqr_context* c, cudaStream_t st, const double* vpk, 
                             &pstride, 1));
     const int64_t nelem = (int64_t)next * NBPK;
     TRY(launch(c, st, "k_tp_wpart", 8.0 * (double)kb * ncols, [&](CwtSlot) {
-        k_tp_wpart<<<wreduce_grid(c, nelem), 256, 0, st>>>(w.wpart.p + (size_t)nsplit * pstride, NBPK, NBPK, ncols, vtop, kb, X, ldx);
+        double* const wp = w.wpart.p + (size_t)nsplit * pstride;
+        if (hyp) k_tp_wpart<true><<<wreduce_grid(c, nelem), 256, 0, st>>>(wp, NBPK, NBPK, ncols, vtop, kb, X, ldx);
+        else k_tp_wpart<false><<<wreduce_grid(c, nelem), 256, 0, st>>>(wp, NBPK, NBPK, ncols, vtop, kb, X, ldx);
     }));
     ++nsplit;
     const int ygrid = (ncols + YCOLS - 1) / YCOLS;
     if (small) {
-        TRY(launch(c, st, "k_mid32", 0.0, [&](CwtSlot) { k_mid32<<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, w.linv, trans); }));
+        TRY(launch(c, st, "k_mid32", 0.0, [&](CwtSlot) {
+            if (hyp) k_mid32<true><<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, w.linv, trans);
+            else k_mid32<false><<<ygrid, 512, 0, st>>>(w.wpart, pstride, nsplit, ncols, w.ypk, w.linv, trans);
+        }));
     } else {
         TRY(launch(c, st, "k_wreduce", 0.0, [&](CwtSlot cwt) {
             k_wreduce<<<wreduce_grid(c, nelem), 256, 0, st>>>(w.wpart, pstride, nsplit, nelem, w.wsum, cwt);
         }));
-        TRY(launch(c, st, "k_tinv128", 0.0, [&](CwtSlot cwt) { k_tinv<128><<<1, 512, smem_tinv(128), st>>>(w.wsum, w.linv, 0, cwt); }));
+        TRY(launch(c, st, "k_tinv128", 0.0, [&](CwtSlot cwt) {
+            if (hyp) k_tinv<128, true><<<1, 512, smem_tinv(128), st>>>(w.wsum, w.linv, 0, cwt);
+            else k_tinv<128, false><<<1, 512, smem_tinv(128), st>>>(w.wsum, w.linv, 0, cwt);
+        }));
         TRY(launch(c, st, "k_ymake128", 0.0, [&](CwtSlot cwt) {
-            k_ymake<128><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, NBPK, ncols, w.linv, w.ypk, trans, cwt);
+            if (hyp) k_ymake<128, true><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, NBPK, ncols, w.linv, w.ypk, trans, cwt);
+            else k_ymake<128, false><<<ygrid, 256, smem_ymake(128), st>>>(w.wsum, NBPK, ncols, w.linv, w.ypk, trans, cwt);
         }));
     }
     TRY(launch_cvy(c, st, vpk, voff, nbp, w.ypk, k, 0, C, ldc, ncols, 0));
@@ -2597,7 +2611,7 @@ static int tp_workspace(dhqr_context* c, cudaStream_t st, int64_t k, int64_t col
 }
 
 static int launch_tp_panel(dhqr_context* c, cudaStream_t st, double* B, int64_t ldb, int64_t k, double* R, int64_t ldr, double* alpha,
-                           double* vtop, int ncols, int voff, int64_t vrows) {
+                           double* vtop, int ncols, int voff, int64_t vrows, int64_t* info, int64_t col0) {
     const int gmax = std::min(c->sms, PANEL_MAXG);
     const int64_t rpc = rup(std::max<int64_t>((k + gmax - 1) / gmax, 64), 8);
     const int G = (int)((k + rpc - 1) / rpc);
@@ -2608,10 +2622,11 @@ static int launch_tp_panel(dhqr_context* c, cudaStream_t st, double* B, int64_t 
     TpPanelArgs a;
     a.B = B; a.ldb = ldb; a.k = k; a.R = R; a.ldr = ldr; a.alpha = alpha; a.vtop = vtop; a.ncols = ncols;
     a.vpk = c->vpk2[0]; a.voff = voff; a.vrows = vrows; a.rows_per_cta = (int)rpc; a.lds = lds;
-    a.cells = c->cells; a.epoch = c->ll_epoch;
+    a.cells = c->cells; a.epoch = c->ll_epoch; a.info = info; a.col0 = col0;
     void* args[] = {&a};
+    void* const kern = info ? (void*)k_tp_panel<true> : (void*)k_tp_panel<false>;
     return launch(c, st, "k_tp_panel", 16.0 * (double)k * ncols, [&](CwtSlot) {   // work = bytes: the B panel read once + written once
-        const cudaError_t e = cudaLaunchCooperativeKernel((void*)k_tp_panel, dim3(G), dim3(PANEL_THREADS), args, smem, st);
+        const cudaError_t e = cudaLaunchCooperativeKernel(kern, dim3(G), dim3(PANEL_THREADS), args, smem, st);
         if (e == cudaSuccess) c->ll_epoch += IB + 8;
         return e;
     });
@@ -2619,33 +2634,36 @@ static int launch_tp_panel(dhqr_context* c, cudaStream_t st, double* B, int64_t 
 
 // Outer panels of 128 columns, each four 32-column k_tp_panel launches with the 32-wide update of the rest of the outer panel after
 // each, then the 128-wide update of the trailing columns.  Row i of R changes only under reflector i, so each launch reads R as the
-// caller passed it.
+// caller passed it.  info != nullptr: the downdate (hyperbolic reflectors, §2.11), which first zero-fills *info in stream order.
 static int qr_append_local(dhqr_context* c, cudaStream_t st, int64_t n, int64_t k, double* R, int64_t ldr, double* alpha, double* B,
-                           int64_t ldb, double* vtop) {
+                           int64_t ldb, double* vtop, int64_t* info) {
     TRY(tp_workspace(c, st, k, n));
+    const bool hyp = info != nullptr;
+    if (hyp) CU(cudaMemsetAsync(info, 0, sizeof(int64_t), st));
     const int64_t vrows = rup(k, 128);
     for (int64_t k0 = 0; k0 < n; k0 += NBMAX) {
         const int kb = (int)std::min<int64_t>(NBMAX, n - k0);
         for (int o = 0; o < kb; o += IB) {
             const int ib = std::min(IB, kb - o);
             const int64_t cs = k0 + o;
-            TRY(launch_tp_panel(c, st, B + cs * ldb, ldb, k, R + cs * ldr + cs, ldr, alpha + cs, vtop + cs, ib, o, vrows));
+            TRY(launch_tp_panel(c, st, B + cs * ldb, ldb, k, R + cs * ldr + cs, ldr, alpha + cs, vtop + cs, ib, o, vrows, info, cs));
             const int rem = kb - o - ib;
             if (rem > 0)
                 TRY(tp_block_update(c, st, c->vpk2[0], o, IB, ib, vtop + cs, k, B + (cs + ib) * ldb, ldb, R + (cs + ib) * ldr + cs, ldr,
-                                    rem, 0));
+                                    rem, 0, hyp));
         }
         const int64_t trail = n - k0 - kb;
         if (trail > 0)
             TRY(tp_block_update(c, st, c->vpk2[0], 0, NBMAX, kb, vtop + k0, k, B + (k0 + kb) * ldb, ldb, R + (k0 + kb) * ldr + k0, ldr,
-                                (int)trail, 0));
+                                (int)trail, 0, hyp));
     }
     return 0;
 }
 
 // [c; e] <- Q~' [c; e] (blocks first to last) or Q~ [c; e] (trans = 1, last to first); V2 packed from B, T recomputed from V2.
+// hyp: [c; e] <- Theta [c; e] of the downdate (trans = 0).
 static int apply_append_local(dhqr_context* c, cudaStream_t st, int64_t n, int64_t k, const double* B, int64_t ldb, const double* vtop,
-                              double* dc, int64_t ldc, double* de, int64_t lde, int nrhs, int trans) {
+                              double* dc, int64_t ldc, double* de, int64_t lde, int nrhs, int trans, bool hyp) {
     TRY(tp_workspace(c, st, k, std::max<int64_t>(n, nrhs)));
     const int64_t vrows = rup(k, 128);
     const int64_t ofirst = trans ? ((n - 1) / NBMAX) * NBMAX : 0, ostep = trans ? -(int64_t)NBMAX : NBMAX;
@@ -2653,53 +2671,74 @@ static int apply_append_local(dhqr_context* c, cudaStream_t st, int64_t n, int64
         const int kb = (int)std::min<int64_t>(NBMAX, n - o);
         const int nbp = kb <= IB ? IB : NBMAX;
         TRY(pack_v(c, st, B + o * ldb, ldb, k, kb, 0, c->vpk2[0], 0, vrows, nbp));
-        TRY(tp_block_update(c, st, c->vpk2[0], 0, nbp, kb, vtop + o, k, de, lde, dc + o, ldc, nrhs, trans));
+        TRY(tp_block_update(c, st, c->vpk2[0], 0, nbp, kb, vtop + o, k, de, lde, dc + o, ldc, nrhs, trans, hyp));
     }
     return 0;
 }
 
-// Arguments 1-3 of all three calls: handle, n, k (k capped by the panel kernel's slab capacity)
-static int check_append_head(dhqr_context* c, int64_t n, int64_t k) {
+// Arguments 1-3 of every append and downdate call: handle, n, k (k capped by the panel kernel's slab capacity)
+static int check_append_head(dhqr_context* c, int64_t n, int64_t k, const char* what = "appending") {
     if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "appending rows is single-GPU (the handle has %d ranks)", c->nranks);
+    if (c->nranks != 1) return set_err(-1, "%s rows is single-GPU (the handle has %d ranks)", what, c->nranks);
     if (n < 0) return set_err(-2, "n < 0");
     if (k < 0) return set_err(-3, "k < 0");
     if (k > narrow_panel_max_rows(c))
-        return set_err(-3, "k = %lld exceeds the rows one append can take on this device (%lld): split the block", (long long)k,
-                       (long long)narrow_panel_max_rows(c));
+        return set_err(-3, "k = %lld exceeds the rows one %s can take on this device (%lld): split the block", (long long)k,
+                       what[0] == 'a' ? "append" : "downdate", (long long)narrow_panel_max_rows(c));
     return 0;
 }
 
-int dhqr_qr_append_f64(dhqr_handle c, int64_t n, int64_t k, double* dR, int64_t ldr, double* d_alpha, double* dB, int64_t ldb,
-                       double* d_vtop, void* stream) {
-    TRY(check_append_head(c, n, k));
+// dhqr_qr_append_f64 (d_info == nullptr, the rows are B) and dhqr_qr_downdate_f64 (the rows are Z): the same checks and driver
+static int qr_tp(dhqr_context* c, int64_t n, int64_t k, double* dR, int64_t ldr, double* d_alpha, double* dB, int64_t ldb, double* d_vtop,
+                 int64_t* d_info, bool hyp, void* stream) {
+    const char* b = hyp ? "Z" : "B";
+    TRY(check_append_head(c, n, k, hyp ? "deleting" : "appending"));
     if (n > 0 && !dR) return set_err(-4, "null R");
     TRY(check_elem_ptr<double>(dR, -4, "R"));
     if (ldr < std::max<int64_t>(1, n)) return set_err(-5, "ldr < max(1,n)");
     if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
     TRY(check_elem_ptr<double>(d_alpha, -6, "alpha"));
     const size_t rbytes = n > 0 ? ((size_t)(n - 1) * ldr + n) * 8 : 0, abytes = (size_t)n * 8;
-    if (n > 0 && k > 0 && !dB) return set_err(-7, "null B");
-    TRY(check_elem_ptr<double>(dB, -7, "B"));
+    if (n > 0 && k > 0 && !dB) return set_err(-7, "null %s", b);
+    TRY(check_elem_ptr<double>(dB, -7, b));
     const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0;
-    if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-7, "B overlaps R or alpha");
-    if (ldb < std::max<int64_t>(1, k)) return set_err(-8, "ldb < max(1,k)");
+    if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-7, "%s overlaps R or alpha", b);
+    if (ldb < std::max<int64_t>(1, k)) return set_err(-8, hyp ? "ldz < max(1,k)" : "ldb < max(1,k)");
     if (n > 0 && !d_vtop) return set_err(-9, "null vtop");
     TRY(check_elem_ptr<double>(d_vtop, -9, "vtop"));
     if (k > 0 && (spans_overlap(d_vtop, abytes, dR, rbytes) || spans_overlap(d_vtop, abytes, d_alpha, abytes) ||
                   spans_overlap(d_vtop, abytes, dB, bbytes)))
-        return set_err(-9, "vtop overlaps R, alpha or B");
+        return set_err(-9, "vtop overlaps R, alpha or %s", b);
+    if (hyp) {
+        if (n > 0 && k > 0 && !d_info) return set_err(-10, "null info");
+        TRY(check_elem_ptr<int64_t>(d_info, -10, "info"));
+        if (n > 0 && k > 0 && (spans_overlap(d_info, 8, dR, rbytes) || spans_overlap(d_info, 8, d_alpha, abytes) ||
+                               spans_overlap(d_info, 8, dB, bbytes) || spans_overlap(d_info, 8, d_vtop, abytes)))
+            return set_err(-10, "info overlaps R, alpha, Z or vtop");
+    }
     if (n == 0 || k == 0) return 0;
     CU(cudaSetDevice(c->device));
-    return qr_append_local(c, (cudaStream_t)stream, n, k, dR, ldr, d_alpha, dB, ldb, d_vtop);
+    return qr_append_local(c, (cudaStream_t)stream, n, k, dR, ldr, d_alpha, dB, ldb, d_vtop, hyp ? d_info : nullptr);
 }
 
+int dhqr_qr_append_f64(dhqr_handle c, int64_t n, int64_t k, double* dR, int64_t ldr, double* d_alpha, double* dB, int64_t ldb,
+                       double* d_vtop, void* stream) {
+    return qr_tp(c, n, k, dR, ldr, d_alpha, dB, ldb, d_vtop, nullptr, false, stream);
+}
+
+int dhqr_qr_downdate_f64(dhqr_handle c, int64_t n, int64_t k, double* dR, int64_t ldr, double* d_alpha, double* dZ, int64_t ldz,
+                         double* d_vtop, int64_t* d_info, void* stream) {
+    return qr_tp(c, n, k, dR, ldr, d_alpha, dZ, ldz, d_vtop, d_info, true, stream);
+}
+
+// the three applies: Q~' (trans = 0), Q~ (trans = 1) of the append, Theta of the downdate (hyp, trans = 0); the rows are B or Z
 static int apply_append(dhqr_context* c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
-                        int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream, int trans) {
-    TRY(check_append_head(c, n, k));
-    if (n > 0 && k > 0 && !dB) return set_err(-4, "null B");
-    TRY(check_elem_ptr<double>(dB, -4, "B"));
-    if (ldb < std::max<int64_t>(1, k)) return set_err(-5, "ldb < max(1,k)");
+                        int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream, int trans, bool hyp = false) {
+    const char* b = hyp ? "Z" : "B";
+    TRY(check_append_head(c, n, k, hyp ? "deleting" : "appending"));
+    if (n > 0 && k > 0 && !dB) return set_err(-4, "null %s", b);
+    TRY(check_elem_ptr<double>(dB, -4, b));
+    if (ldb < std::max<int64_t>(1, k)) return set_err(-5, hyp ? "ldz < max(1,k)" : "ldb < max(1,k)");
     if (n > 0 && !d_vtop) return set_err(-6, "null vtop");
     TRY(check_elem_ptr<double>(d_vtop, -6, "vtop"));
     const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0, vbytes = (size_t)n * 8;
@@ -2707,17 +2746,17 @@ static int apply_append(dhqr_context* c, int64_t n, int64_t k, const double* dB,
     const size_t ebytes = (k > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * lde + k) * 8 : 0;
     if (n > 0 && nrhs > 0 && !d_c) return set_err(-7, "null c");
     TRY(check_elem_ptr<double>(d_c, -7, "c"));
-    if (spans_overlap(d_c, cbytes, dB, bbytes) || spans_overlap(d_c, cbytes, d_vtop, vbytes)) return set_err(-7, "c overlaps B or vtop");
+    if (spans_overlap(d_c, cbytes, dB, bbytes) || spans_overlap(d_c, cbytes, d_vtop, vbytes)) return set_err(-7, "c overlaps %s or vtop", b);
     if (ldc < std::max<int64_t>(1, n)) return set_err(-8, "ldc < max(1,n)");
     if (k > 0 && nrhs > 0 && !d_e) return set_err(-9, "null e");
     TRY(check_elem_ptr<double>(d_e, -9, "e"));
     if (spans_overlap(d_e, ebytes, dB, bbytes) || spans_overlap(d_e, ebytes, d_vtop, vbytes) || spans_overlap(d_e, ebytes, d_c, cbytes))
-        return set_err(-9, "e overlaps B, vtop or c");
+        return set_err(-9, "e overlaps %s, vtop or c", b);
     if (lde < std::max<int64_t>(1, k)) return set_err(-10, "lde < max(1,k)");
     if (nrhs < 0) return set_err(-11, "nrhs < 0");
     if (n == 0 || k == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
-    return apply_append_local(c, (cudaStream_t)stream, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, trans);
+    return apply_append_local(c, (cudaStream_t)stream, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, trans, hyp);
 }
 
 int dhqr_apply_qt_append_f64(dhqr_handle c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
@@ -2728,6 +2767,11 @@ int dhqr_apply_qt_append_f64(dhqr_handle c, int64_t n, int64_t k, const double* 
 int dhqr_apply_q_append_f64(dhqr_handle c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
                             int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream) {
     return apply_append(c, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, stream, 1);
+}
+
+int dhqr_apply_downdate_f64(dhqr_handle c, int64_t n, int64_t k, const double* dZ, int64_t ldz, const double* d_vtop, double* d_c,
+                            int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream) {
+    return apply_append(c, n, k, dZ, ldz, d_vtop, d_c, ldc, d_e, lde, nrhs, stream, 0, true);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

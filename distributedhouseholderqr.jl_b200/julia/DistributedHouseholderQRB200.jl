@@ -196,6 +196,36 @@ function apply_qt!(c::CuVecOrMat{Float64}, e::CuVecOrMat{Float64}, T::AppendedRo
         max(stride(e, 2), k), size(c, 2), stream_ptr()))
     return c, e
 end
+# ---- rows out of a factorisation (LINPACK dchdd; not in the reference), single GPU, DESIGN §2.11 ----
+# Θ [R; Z] = [R'; 0] with R'ᵀR' = RᵀR − ZᵀZ: R' replaces R's strict upper triangle in A and α, Z becomes the hyperbolic reflector
+# tails, vtop their tops; info (on the device) is 0, or the 1-based column at which the removal proved impossible.
+struct DowndatedRows
+    B::CuMatrix{Float64}
+    vtop::CuVector{Float64}
+    info::CuVector{Int64}
+end
+function downdate_rows!(H::DistributedHouseholderQRStruct{<:CuMatrix{Float64}}, Z::CuMatrix{Float64})
+    k, n = size(Z)
+    A = H.A
+    vtop = CUDA.zeros(Float64, n)
+    info = CUDA.zeros(Int64, 1)
+    GC.@preserve A Z vtop info check(:dhqr_qr_downdate_f64, ccall((:dhqr_qr_downdate_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Int64},
+         Ptr{Cvoid}),
+        handle().ptr, n, k, pointer(A), stride(A, 2), pointer(H.α), pointer(Z), max(stride(Z, 2), k), pointer(vtop), pointer(info),
+        stream_ptr()))
+    return DowndatedRows(Z, vtop, info)
+end
+# [c; e] <- Θ [c; e]: c = (Qᵀb)[1:n] and e the removed rows' right-hand sides become c' (x' = R' \ c') and e'.
+function apply!(c::CuVecOrMat{Float64}, e::CuVecOrMat{Float64}, T::DowndatedRows)
+    k, n = size(T.B)
+    GC.@preserve T c e check(:dhqr_apply_downdate_f64, ccall((:dhqr_apply_downdate_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Cint,
+         Ptr{Cvoid}),
+        handle().ptr, n, k, pointer(T.B), max(stride(T.B, 2), k), pointer(T.vtop), pointer(c), max(stride(c, 2), n), pointer(e),
+        max(stride(e, 2), k), size(c, 2), stream_ptr()))
+    return c, e
+end
 # min ||A x - b|| for A fed as row blocks (CuMatrix or Matrix; host blocks are uploaded), from R = 0: x and the residual norm.
 function streaming_lstsq(blocks, n::Integer)
     H = DistributedHouseholderQRStruct(CUDA.zeros(Float64, n, n), CUDA.zeros(Float64, n))

@@ -337,6 +337,31 @@ int dhqr_apply_qt_append_f64(dhqr_handle h, int64_t n, int64_t k, const double *
 int dhqr_apply_q_append_f64(dhqr_handle h, int64_t n, int64_t k, const double *dB, int64_t ldb, const double *d_vtop,
                             double *d_c, int64_t ldc, double *d_e, int64_t lde, int nrhs, void *stream);
 
+/* ---- downdate: delete rows from a factorisation (not in the reference; LINPACK dchdd, scipy qr_delete, MATLAB qrdelete) -------
+ * Theta [R; Z] = [R'; 0] with R''R' = R'R - Z'Z (DESIGN §2.11): R as for dhqr_qr_append_f64, Z the k x n block of rows to remove
+ * (ldz >= max(1, k)).  Theta = Theta_n ... Theta_1, Theta_j = I - v~_j v~_j' J with J = diag(I_n, -I_k), v~_j = vtop[j] on row j of the
+ * R block and Z[:, j] on the k rows, v~_j' J v~_j = 2 or 0.  Theta is J-orthogonal (Theta' J Theta = J), not orthogonal.  Column j
+ * with x0 = R[j, j] in its current state and t = ||Z[:, j]||^2: sigma^2 = (|x0| - sqrt(t)) (|x0| + sqrt(t)), alpha_j = -sign(x0) sigma
+ * (a zero x0 counted as positive); a zero column (x0 = 0, t = 0) stores v~ = 0 and alpha = 0.  The same storage contract as the
+ * append: only R's strict upper triangle and alpha are read and written, Z is overwritten with V2 and vtop with the tops.
+ * The caller is responsible for removing only rows that were folded in.  The library detects only the impossible cases: the first
+ * column with sigma^2 <= 0 while t > 0 (R'R - Z'Z is not positive definite: the rows were never in A, or their removal leaves a
+ * rank-deficient matrix), or with a NaN sigma^2.  Its 1-based index goes to *d_info (int64_t, device memory), and that column and
+ * every later one store vtop = 0, V2 = 0 and alpha = NaN (Theta_j = I); rows of R' above it are the exact downdate of those rows.
+ * Otherwise *d_info = 0.  *d_info is zero-filled in stream order before the first panel and written on the device, so reading it
+ * is the caller's synchronisation.  n = 0 or k = 0 is a no-op that writes nothing, d_info included.  Single GPU, stream-ordered,
+ * bitwise deterministic and layout-independent as the append, with the same cap on k ("append_max_rows", -3 above it).
+ * Errors: -1 to -9 as for dhqr_qr_append_f64 with Z in place of B, -10 null (n > 0 and k > 0) or misaligned info, or info
+ * overlapping R, alpha, Z or vtop. */
+int dhqr_qr_downdate_f64(dhqr_handle h, int64_t n, int64_t k, double *dR, int64_t ldr, double *d_alpha, double *dZ, int64_t ldz,
+                         double *d_vtop, int64_t *d_info, void *stream);
+/* [c; e] <- Theta [c; e], Theta = Theta_n ... Theta_1, from (Z, vtop) of dhqr_qr_downdate_f64: with c = (Q'b)[0:n] and e the
+ * right-hand sides of the removed rows, c' = the first n rows of the result gives x' = R'^{-1} c', and the residual sum of squares
+ * drops by ||e'||^2.  No inverse apply is provided: Theta applied in reverse column order is its own inverse.  Operands, stream and
+ * determinism rules and errors as for dhqr_apply_qt_append_f64, with Z in place of B. */
+int dhqr_apply_downdate_f64(dhqr_handle h, int64_t n, int64_t k, const double *dZ, int64_t ldz, const double *d_vtop,
+                            double *d_c, int64_t ldc, double *d_e, int64_t lde, int nrhs, void *stream);
+
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
  * the result is in host memory.  With pinned host memory the call is a pipeline: the matrix goes up in
