@@ -233,6 +233,10 @@ struct dhqr_context {
     double wide_kappa = 1000.0;                                         // guard on ||D R1^{-1}||_F of the first Cholesky factor (option "wide_kappa")
     DevBuf<long long> wstamps;                                          // clock64 stamps of the single-CTA kernels (option "wide_trace")
     int wide_trace = 0;
+    DevBuf<unsigned long long> gtr_rows;                                // option "gemm_trace": [GTR_MAX_CTAS][GTR_WORDS] bulk-GEMM buckets
+    size_t gtr_used = 0;                                                // rows handed to traced launches since the option was set
+    size_t gtr_dropped = 0;                                             // launches left untraced for want of rows
+    int gemm_trace = 0;
     // Q'b / Qb with one right-hand side: T' of every local panel (computed before the sweep), per-CTA partials of V'b, y, ticket
     DevBuf<double> qt_T;
     DevBuf<double> qt_part;
@@ -279,6 +283,7 @@ struct dhqr_context {
 
 static constexpr int NBMAX = 128;
 static constexpr int CWT_MAX = 8192;   // traced launches per factorisation (option chain_wait_trace)
+static constexpr size_t GTR_MAX_CTAS = (size_t)1 << 17;   // traced CTAs of k_gemm_vta / k_gemm_cvy_p (option gemm_trace), 8 MB
 static constexpr int MAXCTAS_FACTOR = 3;
 
 // gemm tile configurations
@@ -295,15 +300,21 @@ static size_t smem_ymake(int nbp) { return ((size_t)nbp * nbp + YCOLS * nbp) * 8
 
 #define K_G1_128 k_gemm_vta<128, G1_BN, 4, 2, G1_NPW>
 #define K_G1_32 k_gemm_vta<32, G1S_BN, 1, 4, G1S_NPW>
+#define K_G1_128T k_gemm_vta_traced<128, G1_BN, 4, 2, G1_NPW>
+#define K_G1_32T k_gemm_vta_traced<32, G1S_BN, 1, 4, G1S_NPW>
 
 static int set_attrs(dhqr_context* c) {
     if (c->attrs_set) return 0;
     CU(cudaFuncSetAttribute(K_G1_128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g1(128, G1_BN)));
     CU(cudaFuncSetAttribute(K_G1_32, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g1(32, G1S_BN)));
+    CU(cudaFuncSetAttribute(K_G1_128T, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g1(128, G1_BN)));
+    CU(cudaFuncSetAttribute(K_G1_32T, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g1(32, G1S_BN)));
     CU(cudaFuncSetAttribute(k_gemm_cvy, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2()));
     CU(cudaFuncSetAttribute(k_gemm_cvy, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2p()));
     CU(cudaFuncSetAttribute(k_gemm_cvy_p, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    CU(cudaFuncSetAttribute(k_gemm_cvy_p_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g2p()));
+    CU(cudaFuncSetAttribute(k_gemm_cvy_p_traced, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU(cudaFuncSetAttribute(k_gram_sym, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_GRAM_SYM));
     CU(cudaFuncSetAttribute(k_pack_gram, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_GRAM_SYM));
     CU(cudaFuncSetAttribute(k_tinv<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tinv(128)));
@@ -374,6 +385,18 @@ static int launch(dhqr_context* c, cudaStream_t st, const char* what, double wor
         if (e != cudaSuccess) return set_err(1000 + (int)e, "%s failed: %s", what, cudaGetErrorString(e));
     }
     return 0;
+}
+
+// gemm_trace: the rows of a launch of `ctas` CTAs of k_gemm_vta or k_gemm_cvy_p (null: the option is off or the rows ran out)
+static unsigned long long* gtr_slot(dhqr_context* c, size_t ctas) {
+    if (!c->gemm_trace) return nullptr;
+    if (c->gtr_used + ctas > GTR_MAX_CTAS) {
+        c->gtr_dropped++;
+        return nullptr;
+    }
+    unsigned long long* p = c->gtr_rows.p + GTR_WORDS * c->gtr_used;
+    c->gtr_used += ctas;
+    return p;
 }
 
 // Every column of `p` starts 16 B aligned (bulk copies legal): `p` itself is, and the leading dimension is even.
@@ -471,8 +494,10 @@ static int launch_vta_partials(dhqr_context* c, cudaStream_t st, const double* v
     *pstride_out = pstride;
     return launch(c, st, what, 2.0 * (double)rows * nbp * ((double)ncols + nv), [&](CwtSlot cwt) {
         g1.cwt = cwt;
-        if (small) K_G1_32<<<dim3(tiles, nsplit), (1 * 4 + G1S_NPW) * 32, smem_g1(32, G1S_BN), st>>>(g1);
-        else K_G1_128<<<dim3(tiles, nsplit), (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
+        g1.gtr = gtr_slot(c, (size_t)tiles * nsplit);
+        const dim3 grid(tiles, nsplit);
+        if (small) (g1.gtr ? K_G1_32T : K_G1_32)<<<grid, (1 * 4 + G1S_NPW) * 32, smem_g1(32, G1S_BN), st>>>(g1);
+        else (g1.gtr ? K_G1_128T : K_G1_128)<<<grid, (4 * 2 + G1_NPW) * 32, smem_g1(128, G1_BN), st>>>(g1);
     });
 }
 
@@ -557,7 +582,8 @@ static int launch_cvy(dhqr_context* c, cudaStream_t st, const double* vpk, int v
     return launch(c, st, small ? "k_gemm_cvy32" : "k_gemm_cvy128", 2.0 * (double)rows * (small ? 32 : nbp) * (double)ncols,
                   [&](CwtSlot cwt) {
                       g2.cwt = cwt;
-                      if (g2.nkq == 4) k_gemm_cvy_p<<<cvy_p_grid(g2), CVYP_THREADS, smem_g2p(), st>>>(g2);
+                      g2.gtr = g2.nkq == 4 ? gtr_slot(c, cvy_p_grid(g2)) : nullptr;
+                      if (g2.nkq == 4) (g2.gtr ? k_gemm_cvy_p_traced : k_gemm_cvy_p)<<<cvy_p_grid(g2), CVYP_THREADS, smem_g2p(), st>>>(g2);
                       else k_gemm_cvy<<<dim3(g2.tiles_m, g2.tiles_n), 9 * 32, smem_g2(), st>>>(g2);
                   });
 }
@@ -606,7 +632,8 @@ static int apply_pair(dhqr_context* c, cudaStream_t st, const double* vpa, const
     g2.nkq = 8; g2.nkq_alloc = 8; g2.nks = 8;
     return launch(c, st, "k_gemm_cvy256", 2.0 * ((double)rows * WP + (double)(rows - WP) * WP) * (double)ncols, [&](CwtSlot cwt) {
         g2.cwt = cwt;
-        k_gemm_cvy_p<<<cvy_p_grid(g2), CVYP_THREADS, smem_g2p(), st>>>(g2);
+        g2.gtr = gtr_slot(c, cvy_p_grid(g2));
+        (g2.gtr ? k_gemm_cvy_p_traced : k_gemm_cvy_p)<<<cvy_p_grid(g2), CVYP_THREADS, smem_g2p(), st>>>(g2);
     });
 }
 
@@ -1795,6 +1822,16 @@ int dhqr_set_option(dhqr_handle c, const char* key, int64_t value) {
         c->wide_kappa = (double)value;
     } else if (!strcmp(key, "wide_trace")) {
         c->wide_trace = value ? 1 : 0;
+    } else if (!strcmp(key, "gemm_trace")) {
+        // 1: start over with zero rows (no stream here: the fill is complete before the call returns); 0: stop tracing, keep the rows
+        if (value) {
+            CU(cudaSetDevice(c->device));
+            if (!c->gtr_rows) TRY(c->gtr_rows.alloc(GTR_MAX_CTAS * GTR_WORDS));
+            CU(cudaMemset(c->gtr_rows.p, 0, GTR_MAX_CTAS * GTR_WORDS * sizeof(unsigned long long)));
+            CU(cudaStreamSynchronize(cudaStreamLegacy));
+            c->gtr_used = c->gtr_dropped = 0;
+        }
+        c->gemm_trace = value ? 1 : 0;
     } else if (!strcmp(key, "epoch_near_wrap")) {
         // test hook: the tag counters two launches short of their reset (never backwards, so no tag a cell holds comes back);
         // a counter whose buffer is allocated later starts over at 0 with it
@@ -3036,6 +3073,15 @@ int dhqr_debug_copy_f64(dhqr_handle c, const char* which, double* d_dst, int64_t
     if (!strcmp(which, "chain_wait")) {   // [0] = launches of the last look-ahead factorisation, then 6 doubles per launch
         std::vector<double> t(1, (double)(c->cwt_rows.size() / 6));
         t.insert(t.end(), c->cwt_rows.begin(), c->cwt_rows.end());
+        if ((size_t)nelems < t.size()) return set_err(-4, "need %zu elements", t.size());
+        CU(cudaMemcpy(d_dst, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice));
+        return 0;
+    }
+    if (!strcmp(which, "gemm_trace")) {   // [0] = rows, [1] = launches left untraced, then GTR_WORDS doubles per CTA
+        std::vector<unsigned long long> rows(c->gtr_used * GTR_WORDS);
+        if (!rows.empty()) CU(cudaMemcpy(rows.data(), c->gtr_rows.p, rows.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        std::vector<double> t = {(double)c->gtr_used, (double)c->gtr_dropped};
+        t.insert(t.end(), rows.begin(), rows.end());
         if ((size_t)nelems < t.size()) return set_err(-4, "need %zu elements", t.size());
         CU(cudaMemcpy(d_dst, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice));
         return 0;

@@ -102,7 +102,12 @@ int dhqr_destroy(dhqr_handle h);
  *                 under the look-ahead schedule, CUDA events around every launch on the chain's streams and %globaltimer
  *                 stamps of its first CTA start and last warp end ("chain_wait": [0] = launches, then per launch unit,
  *                 stream (0 chain, 1 second apply, 2 side kernels), class index for dhqr_profile_get, event span, stamp
- *                 span, their difference, in ms; -1 for a launch without stamps)
+ *                 span, their difference, in ms; -1 for a launch without stamps); "gemm_trace" 1: zero the rows and trace every
+ *                 later k_gemm_vta / k_gemm_cvy_p launch, one row of 8 words per CTA (kind = (1 << 16) | NBP for k_gemm_vta,
+ *                 (2 << 16) | K for k_gemm_cvy_p; then the clock64 cycles its MMA warps spent from entry to the first operand
+ *                 stage, waiting on later stages, in the k-loop body, waiting on the C tile, in the epilogue, after the last
+ *                 DMMA or epilogue, and from entry to exit, each summed over the warps), 0: stop, keep the rows ("gemm_trace":
+ *                 [0] = rows, [1] = launches left untraced once the 2^17 rows are used, then the rows; synchronise first)
  *   "epoch_near_wrap" 1 (test hook, write-only): move the 32-bit launch-tag counters of the panel exchange cells (k_panel,
  *                 k_tp_panel), the wavefront substitutions and the nb = 1 wave to two launches below their resets, so that a short
  *                 test crosses the resets a long-lived handle meets after ~10^8 panel or ~4 x 10^9 wave launches.  Changes no result
