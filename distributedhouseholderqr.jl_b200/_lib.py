@@ -54,6 +54,10 @@ SIGNATURES = {
     "dhqr_apply_q_append_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
     "dhqr_qr_downdate_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp],
     "dhqr_apply_downdate_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _int, _vp],
+    "dhqr_qr_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _vp],
+    "dhqr_apply_qt_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _int, _vp],
+    "dhqr_apply_q_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _int, _vp],
+    "dhqr_solve_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _int, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

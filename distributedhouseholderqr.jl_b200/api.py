@@ -903,3 +903,138 @@ class StreamingLeastSquares:
         """||A x - b|| per right-hand side at the least-squares solution, accumulated as the blocks were folded in (and taken out:
         rounding can then take the accumulated sum of squares slightly below 0 when the residual is about 0, so it is clamped)."""
         return self._ss.clamp(min=0).sqrt()
+
+
+# --------------------------------------------------------------------------------------------
+# batched QR of many small problems (torch.geqrf / torch.linalg.lstsq on a batch; cuBLAS geqrfBatched / gelsBatched)
+# --------------------------------------------------------------------------------------------
+def colmajor_empty_batched(batch: int, m: int, n: int, device="cuda", lda: Optional[int] = None, stride: Optional[int] = None,
+                           dtype=torch.float64) -> torch.Tensor:
+    """(batch, m, n) tensor whose matrices are column-major: strides (stride, 1, lda), lda default m, stride default lda * n."""
+    lda = max(int(lda or m), 1)
+    stride = int(stride if stride is not None else lda * max(n, 1))
+    if stride < lda * n:
+        raise ValueError(f"stride {stride} < lda * n = {lda * n}")
+    base = torch.empty(max(batch * stride, 1), dtype=dtype, device=device)
+    return base.as_strided((batch, m, n), (stride, 1, lda))
+
+
+def _batched_args(A: torch.Tensor):
+    """(batch, m, n, lda, stride_a) of a (batch, m, n) float64 CUDA tensor of column-major matrices; ValueError otherwise."""
+    if not isinstance(A, torch.Tensor) or not A.is_cuda or A.dtype != torch.float64 or A.dim() != 3:
+        raise ValueError("A must be a (batch, m, n) float64 CUDA tensor")
+    batch, m, n = A.shape
+    if m > 1 and A.stride(1) != 1:
+        raise ValueError("the matrices of A must be column-major: stride(-2) == 1 (see colmajor_empty_batched)")
+    lda = A.stride(2) if n > 1 else max(m, 1)
+    if lda < max(m, 1):
+        raise ValueError("stride(-1) of A is smaller than the row count")
+    if batch > 1 and A.stride(0) < lda * n:
+        raise ValueError("stride(0) of A is smaller than stride(-1) * n: the matrices overlap")
+    return batch, m, n, lda, A.stride(0)
+
+
+def _batched_rhs(b: torch.Tensor, batch: int, m: int):
+    """(ldb, stride_b, nrhs) of b: (batch, m) or (batch, m, k) float64 on the device, each block column-major."""
+    if not isinstance(b, torch.Tensor) or not b.is_cuda or b.dtype != torch.float64 or b.dim() not in (2, 3):
+        raise ValueError("b must be a (batch, m) or (batch, m, k) float64 CUDA tensor")
+    if b.shape[0] != batch or b.shape[1] != m:
+        raise ValueError(f"b must have shape ({batch}, {m}) or ({batch}, {m}, k), not {tuple(b.shape)}")
+    nrhs = 1 if b.dim() == 2 else b.shape[2]
+    if m > 1 and b.stride(1) != 1:
+        raise ValueError("the right-hand sides must be column-major: stride(1) == 1")
+    ldb = b.stride(2) if b.dim() == 3 and nrhs > 1 else max(m, 1)
+    if ldb < max(m, 1):
+        raise ValueError("stride(-1) of b is smaller than the row count")
+    if batch > 1 and b.stride(0) < ldb * nrhs:
+        raise ValueError("stride(0) of b is smaller than stride(-1) * k: the blocks overlap")
+    return ldb, b.stride(0), nrhs
+
+
+def _check_batch_limit(h: Handle, m: int, n: int) -> None:
+    lim = h.get_option("batch_max_elems")
+    if n > m:
+        raise ValueError(f"the batched QR takes n <= m, not {m} x {n}")
+    if m * n > lim:
+        raise ValueError(f"{m} x {n} = {m * n} elements exceeds batch_max_elems = {lim}: factor problems this large one at a time with qr_")
+
+
+class BatchedHouseholderQRStruct:
+    """The factorisations of a batch from ``qr_batched_``: ``.A`` (the caller's (batch, m, n) storage, factored in place) and ``.α``
+    (``.alpha``, (batch, n)).  Problem i is ``(A[i], α[i])`` in the library's storage format, so every single-problem entry point
+    takes it as a factorisation."""
+
+    def __init__(self, A: torch.Tensor, alpha: torch.Tensor, handle: Handle):
+        self.A, self.α, self.handle = A, alpha, handle
+
+    @property
+    def alpha(self):
+        return self.α
+
+    def apply_qt_(self, b: torch.Tensor) -> torch.Tensor:
+        return apply_qt_batched_(b, self.A, self.handle)
+
+    def apply_q_(self, b: torch.Tensor) -> torch.Tensor:
+        return apply_q_batched_(b, self.A, self.handle)
+
+    def ldiv(self, b, return_residual: bool = False):
+        """Least squares min ||A_i x - b_i|| for every problem: ``b`` (batch, m) or (batch, m, k) is left untouched; returns x,
+        (batch, n) or (batch, n, k), and with ``return_residual`` also the residual norms ||A_i x - b_i||, (batch,) or (batch, k)."""
+        batch, m, n, _, _ = _batched_args(self.A)
+        b = torch.as_tensor(b)
+        if b.dim() not in (2, 3) or b.shape[0] != batch or b.shape[1] != m:
+            raise ValueError(f"b must have shape ({batch}, {m}) or ({batch}, {m}, k)")
+        k = 1 if b.dim() == 2 else b.shape[2]
+        s = colmajor_empty_batched(batch, m, k, self.A.device)
+        s.copy_(b.to(device=self.A.device, dtype=torch.float64).reshape(batch, m, k))
+        solve_batched_(s, self.A, self.α, self.handle)
+        x = s[:, :n].clone()
+        res = torch.linalg.vector_norm(s[:, n:], dim=1)
+        if b.dim() == 2:
+            x, res = x[..., 0], res[..., 0]
+        return (x, res) if return_residual else x
+
+
+def qr_batched_(A: torch.Tensor, handle: Optional[Handle] = None) -> BatchedHouseholderQRStruct:
+    """Factor every matrix of ``A`` ((batch, m, n) float64, column-major matrices: stride(-2) == 1, stride(-1) >= m,
+    stride(0) >= stride(-1) * n) in place, in one launch.  n <= m and m * n <= batch_max_elems (196 608); a larger problem raises
+    ValueError (qr_ factors it).  Bitwise deterministic per problem, whatever the batch around it."""
+    batch, m, n, lda, sa = _batched_args(A)
+    h = handle or default_handle(A.device.index)
+    _check_batch_limit(h, m, n)
+    alpha = torch.empty(batch, n, dtype=torch.float64, device=A.device)
+    with torch.cuda.device(A.device):
+        _lib.call("dhqr_qr_batched_f64", h.raw, m, n, batch, C.c_void_p(A.data_ptr()), lda, sa, C.c_void_p(alpha.data_ptr()), n,
+                  _stream_ptr(A.device))
+    return BatchedHouseholderQRStruct(A, alpha, h)
+
+
+def _apply_batched(fn: str, b: torch.Tensor, A: torch.Tensor, handle: Optional[Handle], alpha: Optional[torch.Tensor] = None):
+    batch, m, n, lda, sa = _batched_args(A)
+    h = handle or default_handle(A.device.index)
+    _check_batch_limit(h, m, n)
+    ldb, sb, nrhs = _batched_rhs(b, batch, m)
+    args = [h.raw, m, n, batch, C.c_void_p(A.data_ptr()), lda, sa]
+    if alpha is not None:
+        if alpha.dtype != torch.float64 or alpha.dim() != 2 or tuple(alpha.shape) != (batch, n) or (n > 1 and alpha.stride(1) != 1):
+            raise ValueError(f"alpha must be a ({batch}, {n}) float64 tensor with contiguous rows")
+        args += [C.c_void_p(alpha.data_ptr()), alpha.stride(0)]
+    with torch.cuda.device(A.device):
+        _lib.call(fn, *args, C.c_void_p(b.data_ptr()), ldb, sb, nrhs, _stream_ptr(A.device))
+    return b
+
+
+def apply_qt_batched_(b: torch.Tensor, A: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
+    """b_i <- Q_i' b_i for every problem of a batch factored by qr_batched_; ``b`` (batch, m) or (batch, m, k), in place."""
+    return _apply_batched("dhqr_apply_qt_batched_f64", b, A, handle)
+
+
+def apply_q_batched_(b: torch.Tensor, A: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
+    """b_i <- Q_i b_i for every problem of a batch factored by qr_batched_; ``b`` (batch, m) or (batch, m, k), in place."""
+    return _apply_batched("dhqr_apply_q_batched_f64", b, A, handle)
+
+
+def solve_batched_(b: torch.Tensor, A: torch.Tensor, alpha: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
+    """Q'b and the back-substitution in one launch, in place: on return b[:, :n] = x and b[:, n:] = rows n..m-1 of Q'b, whose
+    norm is the residual norm.  Returns b."""
+    return _apply_batched("dhqr_solve_batched_f64", b, A, handle, alpha)

@@ -22,6 +22,7 @@
 #include "dhqr_complex.cuh"
 #include "dhqr_qrcp.cuh"
 #include "dhqr_append.cuh"
+#include "dhqr_batched.cuh"
 
 using namespace dhqr;
 
@@ -1713,6 +1714,12 @@ static int create_context(std::unique_ptr<dhqr_context>& out, int device) {
         CU(c->aux_stream.create(hi));
         for (int i = 0; i < 4; ++i) CU(c->ev_aux[i].create(cudaEventDisableTiming));
     }
+    // the batched kernels size their shared memory per shape; set here so that no batched call does anything but enqueue
+    const int optin = (int)prop.sharedMemPerBlockOptin;
+    CU(cudaFuncSetAttribute(k_qr_batched, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CU(cudaFuncSetAttribute(k_apply_batched<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CU(cudaFuncSetAttribute(k_apply_batched<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CU(cudaFuncSetAttribute(k_apply_batched<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     out = std::move(c);
     return 0;
 }
@@ -1885,6 +1892,7 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
     }
     else if (!strcmp(key, "sms")) *value = c->sms;
     else if (!strcmp(key, "append_max_rows")) *value = narrow_panel_max_rows(c);
+    else if (!strcmp(key, "batch_max_elems")) *value = BQ_MAX_ELEMS;
     else if (!strcmp(key, "rank")) *value = c->rank;
     else if (!strcmp(key, "nranks")) *value = c->nranks;
     else return set_err(-2, "unknown option '%s'", key);
@@ -2809,6 +2817,124 @@ int dhqr_apply_q_append_f64(dhqr_handle c, int64_t n, int64_t k, const double* d
 int dhqr_apply_downdate_f64(dhqr_handle c, int64_t n, int64_t k, const double* dZ, int64_t ldz, const double* d_vtop, double* d_c,
                             int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream) {
     return apply_append(c, n, k, dZ, ldz, d_vtop, d_c, ldc, d_e, lde, nrhs, stream, 0, true);
+}
+
+// ---- batched QR of many small problems (DESIGN §2.12) -----------------------------------------------------------------------
+// Bytes from the first element of a batch of `batch` operands (rows x cols, leading dimension ld, `stride` apart) to one past the
+// last; 0 when there is none.  The stride counts only when batch > 1, a negative one as 0 (the stride check rejects it next), and
+// the span is clamped, so that an absurd stride cannot wrap the interval test.
+static size_t batch_span(int64_t batch, int64_t stride, int64_t rows, int64_t cols, int64_t ld) {
+    if (batch <= 0 || rows <= 0 || cols <= 0) return 0;
+    const __int128 e = (__int128)(batch - 1) * std::max<int64_t>(stride, 0) + (__int128)(cols - 1) * ld + rows;
+    return e > ((__int128)1 << 58) ? (size_t)1 << 61 : (size_t)e * 8;
+}
+
+// Arguments 1-7 of every batched entry point: handle, m, n, batch, A, lda, stride_a
+static int check_batched_head(dhqr_context* c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the batched QR is single-GPU (the handle has %d ranks)", c->nranks);
+    if (m < 0) return set_err(-2, "m < 0");
+    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
+    if (n > 0 && m > BQ_MAX_ELEMS / n)
+        return set_err(-3, "m * n exceeds batch_max_elems (%lld): factor a problem this large with dhqr_qr_f64", (long long)BQ_MAX_ELEMS);
+    if (batch < 0) return set_err(-4, "batch < 0");
+    if (batch * batched_geom(m, n).cs > INT32_MAX) return set_err(-4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
+    if (batch > 0 && n > 0 && !dA) return set_err(-5, "null A");
+    TRY(check_elem_ptr<double>(dA, -5, "A"));
+    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
+    if (batch > 1 && (__int128)stride_a < (__int128)lda * n) return set_err(-7, "stride_a < lda * n");
+    return 0;
+}
+
+extern "C++" {   // as for the pivoted QR above
+template <typename Kernel, typename... Args>
+static int launch_batched(dhqr_context* c, cudaStream_t st, const char* what, double work, Kernel kern, const BatchedGeom& g,
+                          int64_t batch, int ny, size_t smem, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(batch * g.cs), (unsigned)ny);
+    cfg.blockDim = dim3(g.threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = (unsigned)g.cs;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    return launch(c, st, what, work, [&](CwtSlot) { return cudaLaunchKernelEx(&cfg, kern, args...); });
+}
+}   // extern "C++"
+
+int dhqr_qr_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, double* dA, int64_t lda, int64_t stride_a,
+                        double* d_alpha, int64_t stride_alpha, void* stream) {
+    TRY(check_batched_head(c, m, n, batch, dA, lda, stride_a));
+    if (batch > 0 && n > 0 && !d_alpha) return set_err(-8, "null alpha");
+    TRY(check_elem_ptr<double>(d_alpha, -8, "alpha"));
+    if (spans_overlap(d_alpha, batch_span(batch, stride_alpha, n, 1, n), dA, batch_span(batch, stride_a, m, n, lda)))
+        return set_err(-8, "alpha overlaps A");
+    if (batch > 1 && stride_alpha < n) return set_err(-9, "stride_alpha < n");
+    if (batch == 0 || n == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    const BatchedGeom g = batched_geom(m, n);
+    const double flops = (double)batch * (2.0 * m * n * n - 2.0 * n * n * n / 3.0);
+    return launch_batched(c, (cudaStream_t)stream, "k_qr_batched", flops, k_qr_batched, g, batch, 1, smem_qr_batched(g, n), dA, lda,
+                          stride_a, d_alpha, stride_alpha, (int)m, (int)n, g.rpc);
+}
+
+// dhqr_apply_qt_batched_f64 (trans), dhqr_apply_q_batched_f64 and dhqr_solve_batched_f64 (solve: alpha is arguments 8-9, and
+// every later argument index moves up by 2)
+static int apply_batched(dhqr_context* c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a,
+                         const double* d_alpha, int64_t stride_alpha, double* d_b, int64_t ldb, int64_t stride_b, int nrhs, void* stream,
+                         bool trans, bool solve) {
+    TRY(check_batched_head(c, m, n, batch, dA, lda, stride_a));
+    const size_t abytes = batch_span(batch, stride_a, m, n, lda);
+    const size_t albytes = solve ? batch_span(batch, stride_alpha, n, 1, n) : 0;
+    const int o = solve ? 2 : 0;
+    if (solve) {
+        if (batch > 0 && n > 0 && !d_alpha) return set_err(-8, "null alpha");
+        TRY(check_elem_ptr<double>(d_alpha, -8, "alpha"));
+        if (spans_overlap(d_alpha, albytes, dA, abytes)) return set_err(-8, "alpha overlaps A");
+        if (batch > 1 && stride_alpha < n) return set_err(-9, "stride_alpha < n");
+    }
+    if (batch > 0 && n > 0 && nrhs > 0 && !d_b) return set_err(-8 - o, "null b");
+    TRY(check_elem_ptr<double>(d_b, -8 - o, "b"));
+    const size_t bbytes = batch_span(batch, stride_b, m, nrhs, ldb);
+    if (spans_overlap(d_b, bbytes, dA, abytes) || spans_overlap(d_b, bbytes, d_alpha, albytes))
+        return set_err(-8 - o, solve ? "b overlaps A or alpha" : "b overlaps A");
+    if (ldb < std::max<int64_t>(1, m)) return set_err(-9 - o, "ldb < max(1,m)");
+    if (batch > 1 && (__int128)stride_b < (__int128)ldb * nrhs) return set_err(-10 - o, "stride_b < ldb * nrhs");
+    if (nrhs < 0) return set_err(-11 - o, "nrhs < 0");
+    if (batch == 0 || n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    const BatchedGeom g = batched_geom(m, n);
+    const int kc = batched_kc(g, n, nrhs);
+    const int ny = (int)std::min<int64_t>((nrhs + kc - 1) / kc, 65535);
+    const size_t smem = smem_apply_batched(g, n, kc, solve);
+    const double flops = (double)batch * nrhs * (4.0 * m * n - 2.0 * n * n + (solve ? (double)n * n : 0.0));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (solve)
+        return launch_batched(c, st, "k_solve_batched", flops, k_apply_batched<true, true>, g, batch, ny, smem, dA, lda, stride_a, d_alpha,
+                              stride_alpha, d_b, ldb, stride_b, (int)m, (int)n, nrhs, g.rpc, kc);
+    return launch_batched(c, st, trans ? "k_apply_qt_batched" : "k_apply_q_batched", flops,
+                          trans ? k_apply_batched<true, false> : k_apply_batched<false, false>, g, batch, ny, smem, dA, lda, stride_a,
+                          (const double*)nullptr, (int64_t)0, d_b, ldb, stride_b, (int)m, (int)n, nrhs, g.rpc, kc);
+}
+
+int dhqr_apply_qt_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a,
+                              double* d_b, int64_t ldb, int64_t stride_b, int nrhs, void* stream) {
+    return apply_batched(c, m, n, batch, dA, lda, stride_a, nullptr, 0, d_b, ldb, stride_b, nrhs, stream, true, false);
+}
+
+int dhqr_apply_q_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a,
+                             double* d_b, int64_t ldb, int64_t stride_b, int nrhs, void* stream) {
+    return apply_batched(c, m, n, batch, dA, lda, stride_a, nullptr, 0, d_b, ldb, stride_b, nrhs, stream, false, false);
+}
+
+int dhqr_solve_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a,
+                           const double* d_alpha, int64_t stride_alpha, double* d_b, int64_t ldb, int64_t stride_b, int nrhs,
+                           void* stream) {
+    return apply_batched(c, m, n, batch, dA, lda, stride_a, d_alpha, stride_alpha, d_b, ldb, stride_b, nrhs, stream, true, true);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

@@ -226,6 +226,27 @@ function apply!(c::CuVecOrMat{Float64}, e::CuVecOrMat{Float64}, T::DowndatedRows
         max(stride(e, 2), k), size(c, 2), stream_ptr()))
     return c, e
 end
+# ---- many small problems in one launch (cuBLAS geqrfBatched / gelsBatched; not in the reference), single GPU, DESIGN §2.12 ----
+# A[:, :, i] (m x n, n <= m, m n <= batch_max_elems) is factored in place for every i; α[:, i] receives diag(R).
+function qr_batched!(A::CuArray{Float64,3})
+    m, n, batch = size(A)
+    α = CUDA.zeros(Float64, n, batch)
+    GC.@preserve A α check(:dhqr_qr_batched_f64, ccall((:dhqr_qr_batched_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, Ptr{Cvoid}),
+        handle().ptr, m, n, batch, pointer(A), max(stride(A, 2), m), stride(A, 3), pointer(α), n, stream_ptr()))
+    return A, α
+end
+# x[:, :, i] = A_i \ b[:, :, i] (least squares) from qr_batched!'s (A, α); b (m x k x batch) is left untouched.
+function ldiv_batched(A::CuArray{Float64,3}, α::CuMatrix{Float64}, b::CuArray{Float64,3})
+    m, n, batch = size(A)
+    s = copy(b)
+    GC.@preserve A α s check(:dhqr_solve_batched_f64, ccall((:dhqr_solve_batched_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Int64, Cint,
+         Ptr{Cvoid}),
+        handle().ptr, m, n, batch, pointer(A), max(stride(A, 2), m), stride(A, 3), pointer(α), n, pointer(s), max(stride(s, 2), m),
+        stride(s, 3), size(s, 2), stream_ptr()))
+    return s[1:n, :, :]
+end
 # min ||A x - b|| for A fed as row blocks (CuMatrix or Matrix; host blocks are uploaded), from R = 0: x and the residual norm.
 function streaming_lstsq(blocks, n::Integer)
     H = DistributedHouseholderQRStruct(CUDA.zeros(Float64, n, n), CUDA.zeros(Float64, n))

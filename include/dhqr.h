@@ -116,7 +116,8 @@ int dhqr_destroy(dhqr_handle h);
  *                 counters of work the device has finished: read them after synchronising the stream of the calls),
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
  *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64 and dhqr_qrcp_c64; device-side, read after synchronising),
- *                 "append_max_rows" (the largest k one dhqr_qr_append_f64 call takes on this device)
+ *                 "append_max_rows" (the largest k one dhqr_qr_append_f64 call takes on this device), "batch_max_elems" (the
+ *                 largest m * n of one problem of the batched entry points)
  *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
  *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys (not "epoch_near_wrap").
  *   Any other key returns -2 (unknown option). */
@@ -366,6 +367,49 @@ int dhqr_qr_downdate_f64(dhqr_handle h, int64_t n, int64_t k, double *dR, int64_
  * determinism rules and errors as for dhqr_apply_qt_append_f64, with Z in place of B. */
 int dhqr_apply_downdate_f64(dhqr_handle h, int64_t n, int64_t k, const double *dZ, int64_t ldz, const double *d_vtop,
                             double *d_c, int64_t ldc, double *d_e, int64_t lde, int nrhs, void *stream);
+
+/* ---- batched QR of many small problems (not in the reference; cuBLAS geqrfBatched / gelsBatched, torch.geqrf on a batch) --------
+ * Problem i (0-based, i < batch) is the m x n column-major matrix at dA + i * stride_a (leading dimension lda), its alpha is at
+ * d_alpha + i * stride_alpha (n entries) and its right-hand sides at d_b + i * stride_b (m x nrhs, ldb).  Float64, single GPU (a
+ * handle with nranks > 1 returns -1).  One launch factors, applies or solves the whole batch (DESIGN §2.12): each problem is held in
+ * the shared memory of one thread-block cluster of 1, 2, 4 or 8 CTAs, chosen from (m, n) alone.
+ *   - Size limit: n <= m and m * n <= batch_max_elems (read-only option; 196 608 = 8 CTAs x 24 576 doubles, e.g. 8192 x 24,
+ *     4096 x 48, 443 x 443).  A larger problem returns -3: there is no fall-back to dhqr_qr_f64, which takes it.
+ *   - Strides: when batch > 1, stride_a >= lda * n, stride_alpha >= n and stride_b >= ldb * nrhs (ignored when batch <= 1).  The span
+ *     of A over the batch must not intersect the span of alpha or of b (an interval test); batch x (CTAs per problem) <= 2^31 - 1.
+ *   - Stream-ordered on the caller's stream.  No synchronisation and no allocation, ever: the batched entry points use no handle
+ *     workspace, so they capture into a CUDA graph on a fresh handle.  Each call is one kernel launch (dhqr_launch_count; profile
+ *     classes k_qr_batched, k_apply_qt_batched, k_apply_q_batched, k_solve_batched).
+ *   - Bitwise deterministic: a problem's bits depend on its own data and on (m, n, nrhs) only, not on batch, its position in the
+ *     batch, lda, ldb, the strides, 8 B base offsets or the handle's history.  Nothing outside the operands is written: neither
+ *     padding rows nor the gaps between problems.
+ *   - Errors, in argument order, every check before anything is enqueued: -1 null or multi-rank handle, -2 m < 0, -3 n < 0, n > m
+ *     or m * n above batch_max_elems, -4 batch < 0 or too large for the grid, -5 null (batch > 0 and n > 0) or misaligned A, -6 lda
+ *     < max(1, m), -7 stride_a < lda * n with batch > 1; then, at their own indices, null, misaligned (8 B) or overlapping alpha /
+ *     b, stride_alpha < n, ldb < max(1, m), stride_b < ldb * nrhs and nrhs < 0.  batch = 0, n = 0 or nrhs = 0 is a no-op that
+ *     writes nothing.
+ *
+ * dhqr_qr_batched_f64: factors every problem in place into the library's storage format (v scaled to |v|^2 = 2 in the lower
+ * trapezoid including the diagonal, R's strict upper triangle above it, diag(R) in alpha), by the reference's recurrences as
+ * oracle/dhqr_oracle.c and dhqr_qr_f64 with nb = 1 follow them, sign(0) = 0 included: an exact zero column gives the fp64 oracle's
+ * NaN pattern.  So every other entry point reads problem i as a factorisation (dhqr_form_q_f64, dhqr_backsolve_f64,
+ * dhqr_solve_adj_f64, ... on dA + i * stride_a).  The bits need not equal dhqr_qr_f64's: the sums run in another order.
+ * Errors past -7: -8 null, misaligned or overlapping alpha, -9 stride_alpha < n. */
+int dhqr_qr_batched_f64(dhqr_handle h, int64_t m, int64_t n, int64_t batch, double *dA, int64_t lda, int64_t stride_a,
+                        double *d_alpha, int64_t stride_alpha, void *stream);
+/* b <- Q'b (dhqr_apply_qt_batched_f64) or Q b (dhqr_apply_q_batched_f64) of every problem, for any nrhs >= 0.  Errors past -7:
+ * -8 null, misaligned or overlapping b, -9 ldb < max(1, m), -10 stride_b < ldb * nrhs, -11 nrhs < 0. */
+int dhqr_apply_qt_batched_f64(dhqr_handle h, int64_t m, int64_t n, int64_t batch, const double *dA, int64_t lda,
+                              int64_t stride_a, double *d_b, int64_t ldb, int64_t stride_b, int nrhs, void *stream);
+int dhqr_apply_q_batched_f64(dhqr_handle h, int64_t m, int64_t n, int64_t batch, const double *dA, int64_t lda,
+                             int64_t stride_a, double *d_b, int64_t ldb, int64_t stride_b, int nrhs, void *stream);
+/* Least squares, Q'b and the back-substitution fused in one launch: on return b[0:n] = x = R^{-1} (Q'b)[0:n], and rows n..m-1 hold
+ * rows n..m-1 of Q'b, so the residual norm of each right-hand side is ||b[n:m]||.  A zero alpha propagates Inf / NaN, as in
+ * dhqr_backsolve_f64.  Errors past -7: -8 null, misaligned or overlapping alpha, -9 stride_alpha < n, -10 null, misaligned or
+ * overlapping b (A or alpha), -11 ldb < max(1, m), -12 stride_b < ldb * nrhs, -13 nrhs < 0. */
+int dhqr_solve_batched_f64(dhqr_handle h, int64_t m, int64_t n, int64_t batch, const double *dA, int64_t lda, int64_t stride_a,
+                           const double *d_alpha, int64_t stride_alpha, double *d_b, int64_t ldb, int64_t stride_b, int nrhs,
+                           void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
