@@ -58,6 +58,11 @@ SIGNATURES = {
     "dhqr_apply_qt_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _int, _vp],
     "dhqr_apply_q_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _int, _vp],
     "dhqr_solve_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _int, _vp],
+    "dhqr_qr_append_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64,
+                                   _vp, _i64, _i64, _int, _vp],
+    "dhqr_qr_downdate_batched_f64": [_vp, _i64, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64,
+                                     _vp, _i64, _i64, _int, _vp, _vp],
+    "dhqr_backsolve_batched_f64": [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _int, _vp],
     "dhqr_qr_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _int],
     "dhqr_ldiv_host_f64": [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp],
     "dhqr_partialdot_f64": [_vp, _vp, _vp, _i64, _i64, _vp, _vp],

@@ -1038,3 +1038,211 @@ def solve_batched_(b: torch.Tensor, A: torch.Tensor, alpha: torch.Tensor, handle
     """Q'b and the back-substitution in one launch, in place: on return b[:, :n] = x and b[:, n:] = rows n..m-1 of Q'b, whose
     norm is the residual norm.  Returns b."""
     return _apply_batched("dhqr_solve_batched_f64", b, A, handle, alpha)
+
+
+# --------------------------------------------------------------------------------------------
+# rows into and out of many small triangles in one launch, and their back-substitution (DESIGN §2.13)
+# --------------------------------------------------------------------------------------------
+class BatchedAppendedRows:
+    """The reflectors of ``append_rows_batched_``: ``.B`` holds problem i's tails V2 in B[i] (the caller's (batch, k, n) block,
+    overwritten) and ``.vtop`` ((batch, n)) their tops, so ``AppendedRows(B[i], vtop[i], handle)`` applies problem i's Q~."""
+
+    def __init__(self, B, vtop, handle: Handle):
+        self.B, self.vtop, self.handle = B, vtop, handle
+
+
+class BatchedDowndatedRows(BatchedAppendedRows):
+    """The hyperbolic reflectors of ``downdate_rows_batched_`` (``.B``, ``.vtop``) and ``.info``, a (batch,) int64 CUDA tensor: 0, or
+    the 1-based column at which problem i's removal proved impossible.  Reading it synchronises with the device."""
+
+    def __init__(self, B, vtop, info, handle: Handle):
+        super().__init__(B, vtop, handle)
+        self.info = info
+
+
+def _vector_batch(x: torch.Tensor, batch: int, n: int, what: str) -> int:
+    """stride(0) of a (batch, n) float64 CUDA tensor with contiguous rows."""
+    if (not isinstance(x, torch.Tensor) or not x.is_cuda or x.dtype != torch.float64 or tuple(x.shape) != (batch, n)
+            or (n > 1 and x.stride(1) != 1)):
+        raise ValueError(f"{what} must be a ({batch}, {n}) float64 CUDA tensor with contiguous rows")
+    return x.stride(0)
+
+
+def _check_update_limit(h: Handle, n: int, k: int, nrhs: int) -> None:
+    cols, lim = h.get_option("batch_update_max_cols"), h.get_option("batch_max_elems")
+    if n + nrhs > cols:
+        raise ValueError(f"n + nrhs = {n + nrhs} exceeds batch_update_max_cols = {cols}")
+    if k * (n + nrhs) > lim:
+        raise ValueError(f"k * (n + nrhs) = {k * (n + nrhs)} exceeds batch_max_elems = {lim}: split the block "
+                         "(BatchedStreamingLeastSquares does)")
+
+
+def _tp_batched(fn: str, R: torch.Tensor, alpha: torch.Tensor, B: torch.Tensor, c, e, handle: Optional[Handle], hyp: bool):
+    batch, m, n, ldr, sr = _batched_args(R)
+    if m < n:
+        raise ValueError(f"R must hold (batch, m, n) matrices with m >= n, not {tuple(R.shape)}")
+    sal = _vector_batch(alpha, batch, n, "alpha")
+    bb, k, nb, ldb, sb = _batched_args(B)
+    if bb != batch or nb != n:
+        raise ValueError(f"B must have shape ({batch}, k, {n}), not {tuple(B.shape)}")
+    if (c is None) != (e is None):
+        raise ValueError("pass both c and e, or neither")
+    nrhs, rhs = 0, [None, 0, 0, None, 0, 0]
+    if c is not None:
+        ldc, sc, nrhs = _batched_rhs(c, batch, n)
+        lde, se, nrhs_e = _batched_rhs(e, batch, k)
+        if nrhs != nrhs_e:
+            raise ValueError("c and e must have the same number of right-hand sides")
+        rhs = [C.c_void_p(c.data_ptr()), ldc, sc, C.c_void_p(e.data_ptr()), lde, se]
+    h = handle or default_handle(R.device.index)
+    _check_update_limit(h, n, k, nrhs)
+    vtop = torch.zeros(batch, n, dtype=torch.float64, device=R.device)
+    info = torch.zeros(batch, dtype=torch.int64, device=R.device) if hyp else None
+    args = [h.raw, n, k, batch, C.c_void_p(R.data_ptr()), ldr, sr, C.c_void_p(alpha.data_ptr()), sal, C.c_void_p(B.data_ptr()), ldb, sb,
+            C.c_void_p(vtop.data_ptr()), n, *rhs, nrhs]
+    if hyp:
+        args.append(C.c_void_p(info.data_ptr()))
+    with torch.cuda.device(R.device):
+        _lib.call(fn, *args, _stream_ptr(R.device))
+    return (BatchedDowndatedRows(B, vtop, info, h) if hyp else BatchedAppendedRows(B, vtop, h))
+
+
+def append_rows_batched_(R: torch.Tensor, alpha: torch.Tensor, B: torch.Tensor, c: Optional[torch.Tensor] = None,
+                         e: Optional[torch.Tensor] = None, handle: Optional[Handle] = None) -> BatchedAppendedRows:
+    """Fold the k new rows ``B[i]`` into the triangle of every problem i, in one launch: ``R`` (batch, m, n) column-major matrices
+    with m >= n whose strict upper n x n triangles hold R (a qr_batched_ factorisation works; the diagonal and lower part are never
+    touched), ``alpha`` (batch, n) its diagonal, ``B`` (batch, k, n) column-major, overwritten with the reflector tails.  With ``c``
+    ((batch, n) or (batch, n, nrhs)) and ``e`` ((batch, k) or (batch, k, nrhs)), [c; e] <- Q~'[c; e] in the same launch.  n + nrhs <=
+    batch_update_max_cols and k (n + nrhs) <= batch_max_elems.  Stream-ordered, no synchronisation."""
+    return _tp_batched("dhqr_qr_append_batched_f64", R, alpha, B, c, e, handle, False)
+
+
+def downdate_rows_batched_(R: torch.Tensor, alpha: torch.Tensor, Z: torch.Tensor, c: Optional[torch.Tensor] = None,
+                           e: Optional[torch.Tensor] = None, handle: Optional[Handle] = None) -> BatchedDowndatedRows:
+    """Remove the k rows ``Z[i]`` from the triangle of every problem i, in one launch (operands as for append_rows_batched_; with
+    ``c`` and ``e``, [c; e] <- Theta [c; e]).  ``.info[i]`` is 0, or the 1-based column at which problem i's removal proved
+    impossible; from that column on its alpha is NaN.  Stream-ordered, no synchronisation."""
+    return _tp_batched("dhqr_qr_downdate_batched_f64", R, alpha, Z, c, e, handle, True)
+
+
+def backsolve_batched_(b: torch.Tensor, R: torch.Tensor, alpha: torch.Tensor, handle: Optional[Handle] = None) -> torch.Tensor:
+    """b_i[0:n] <- R_i^{-1} b_i[0:n] for every problem, in place, in one launch: ``R`` and ``alpha`` as for append_rows_batched_
+    (only R's strict upper triangle and alpha are read), ``b`` (batch, m) or (batch, m, k) with m >= n, column-major blocks; rows
+    n..m-1 are left alone.  n <= batch_update_max_cols.  Returns b."""
+    batch, m, n, ldr, sr = _batched_args(R)
+    if m < n:
+        raise ValueError(f"R must hold (batch, m, n) matrices with m >= n, not {tuple(R.shape)}")
+    sal = _vector_batch(alpha, batch, n, "alpha")
+    if not isinstance(b, torch.Tensor) or b.dim() not in (2, 3) or b.shape[0] != batch or b.shape[1] < n:
+        raise ValueError(f"b must be a ({batch}, m) or ({batch}, m, k) tensor with m >= {n}")
+    ldb, sb, nrhs = _batched_rhs(b, batch, b.shape[1])
+    h = handle or default_handle(R.device.index)
+    if n > h.get_option("batch_update_max_cols"):
+        raise ValueError(f"n = {n} exceeds batch_update_max_cols = {h.get_option('batch_update_max_cols')}")
+    with torch.cuda.device(R.device):
+        _lib.call("dhqr_backsolve_batched_f64", h.raw, n, batch, C.c_void_p(R.data_ptr()), ldr, sr, C.c_void_p(alpha.data_ptr()), sal,
+                  C.c_void_p(b.data_ptr()), ldb, sb, nrhs, _stream_ptr(R.device))
+    return b
+
+
+class BatchedStreamingLeastSquares:
+    """min ||A_i x_i - b_i|| for ``batch`` independent problems of n unknowns, fed block by block: ``add`` folds the rows of a
+    (batch, k, n) block into every triangle (from R = 0) and their right-hand sides into c = (Q'b)[0:n]; ``remove`` takes rows out
+    again, so add-newest / remove-oldest / solve keeps a rolling window per problem at O(k n^2) per slide::
+
+        ls = BatchedStreamingLeastSquares(batch, n)
+        for A_blk, b_blk in blocks:            # (batch, k, n), (batch, k)
+            ls.add(A_blk, b_blk)
+            window.append((A_blk, b_blk))
+            if len(window) > w:
+                ls.remove(*window.pop(0))
+            x = ls.solve()                     # (batch, n)
+
+    Each of ``add``, ``remove`` and ``solve`` is one library launch (plus torch copies) while k (n + nrhs) <= batch_max_elems;
+    larger blocks are split.  Nothing synchronises: ``remove`` returns the (batch,) int64 device tensor of its downdates' status,
+    0 where the rows came out, and a problem whose removal failed (the rows were never added, or the remaining rows are
+    rank-deficient) keeps its previous R, alpha, c, sum of squares and row count."""
+
+    def __init__(self, batch: int, n: int, nrhs: int = 1, device=0, handle: Optional[Handle] = None):
+        self.batch, self.n, self.nrhs = int(batch), int(n), int(nrhs)
+        self.device = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
+        self.handle = handle or default_handle(self.device.index)
+        cols = self.handle.get_option("batch_update_max_cols")
+        if self.n < 1 or self.nrhs < 1 or self.n + self.nrhs > cols:
+            raise ValueError(f"need n >= 1, nrhs >= 1 and n + nrhs <= batch_update_max_cols = {cols}")
+        self._cap = self.handle.get_option("batch_max_elems") // (self.n + self.nrhs)
+        self.A = colmajor_empty_batched(self.batch, self.n, self.n, self.device)
+        self.A.zero_()
+        self.α = torch.zeros(self.batch, self.n, dtype=torch.float64, device=self.device)
+        self.c = colmajor_empty_batched(self.batch, self.n, self.nrhs, self.device)
+        self.c.zero_()
+        self._ss = torch.zeros(self.batch, self.nrhs, dtype=torch.float64, device=self.device)
+        self.rows = torch.zeros(self.batch, dtype=torch.int64, device=self.device)
+
+    def _copy(self, x: torch.Tensor) -> torch.Tensor:
+        y = colmajor_empty_batched(x.shape[0], x.shape[1], x.shape[2], self.device)
+        return y.copy_(x)
+
+    def _blocks(self, A_blk, b_blk):
+        """(k, [(B, e), ...]): column-major copies of the block in pieces of at most k (n + nrhs) <= batch_max_elems rows."""
+        A_blk = torch.as_tensor(A_blk, device=self.device, dtype=torch.float64)
+        b_blk = torch.as_tensor(b_blk, device=self.device, dtype=torch.float64)
+        if b_blk.dim() == 2:
+            b_blk = b_blk[..., None]
+        if A_blk.dim() != 3 or A_blk.shape[0] != self.batch or A_blk.shape[2] != self.n:
+            raise ValueError(f"need a ({self.batch}, k, {self.n}) block, not {tuple(A_blk.shape)}")
+        k = A_blk.shape[1]
+        if tuple(b_blk.shape) != (self.batch, k, self.nrhs):
+            raise ValueError(f"need ({self.batch}, {k}) or ({self.batch}, {k}, {self.nrhs}) right-hand sides")
+        return k, [(self._copy(A_blk[:, r0:r0 + self._cap]), self._copy(b_blk[:, r0:r0 + self._cap])) for r0 in range(0, k, self._cap)]
+
+    def add(self, A_blk, b_blk) -> "BatchedStreamingLeastSquares":
+        """Fold rows ``A_blk`` (batch, k, n) with right-hand sides ``b_blk`` ((batch, k) or (batch, k, nrhs)) into every problem."""
+        k, blocks = self._blocks(A_blk, b_blk)
+        for B, e in blocks:
+            append_rows_batched_(self.A, self.α, B, self.c, e, self.handle)
+            self._ss += (e * e).sum(1)
+        self.rows += k
+        return self
+
+    def remove(self, A_blk, b_blk) -> torch.Tensor:
+        """Take rows ``A_blk`` (batch, k, n) with right-hand sides ``b_blk`` out of every problem again: they must be rows that were
+        added.  R, alpha and c are downdated as copies, and each problem takes its copy only where every block's removal succeeded.
+        Returns the (batch,) int64 status on the device (0, or the 1-based column at which the first failing block showed the
+        removal impossible); nothing synchronises."""
+        k, blocks = self._blocks(A_blk, b_blk)
+        A, α, c = self._copy(self.A), self.α.clone(), self._copy(self.c)
+        drop = torch.zeros_like(self._ss)
+        info = torch.zeros(self.batch, dtype=torch.int64, device=self.device)
+        for Z, e in blocks:
+            d = downdate_rows_batched_(A, α, Z, c, e, self.handle)
+            drop += (e * e).sum(1)
+            info = torch.where(info != 0, info, d.info)
+        ok = info == 0
+        self.A.copy_(torch.where(ok[:, None, None], A, self.A))
+        self.α.copy_(torch.where(ok[:, None], α, self.α))
+        self.c.copy_(torch.where(ok[:, None, None], c, self.c))
+        self._ss -= torch.where(ok[:, None], drop, torch.zeros_like(drop))
+        self.rows -= torch.where(ok, k, 0)
+        return info
+
+    @property
+    def alpha(self):
+        return self.α
+
+    @property
+    def R(self) -> torch.Tensor:
+        """(batch, n, n): the triangle R' of every problem's rows."""
+        return torch.triu(self.A, 1) + torch.diag_embed(self.α)
+
+    def solve(self) -> torch.Tensor:
+        """x_i = R_i'^{-1} c_i for every problem through backsolve_batched_: (batch, n), or (batch, n, nrhs); R and c are kept."""
+        x = self._copy(self.c)
+        backsolve_batched_(x, self.A, self.α, self.handle)
+        return x[..., 0] if self.nrhs == 1 else x
+
+    def residual_norm(self) -> torch.Tensor:
+        """||A_i x_i - b_i|| per problem (and right-hand side) at the least-squares solution, accumulated as blocks were added and
+        removed, the sum of squares clamped at 0 against rounding: (batch,), or (batch, nrhs)."""
+        r = self._ss.clamp(min=0).sqrt()
+        return r[:, 0] if self.nrhs == 1 else r

@@ -1720,6 +1720,9 @@ static int create_context(std::unique_ptr<dhqr_context>& out, int device) {
     CU(cudaFuncSetAttribute(k_apply_batched<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     CU(cudaFuncSetAttribute(k_apply_batched<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     CU(cudaFuncSetAttribute(k_apply_batched<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CU(cudaFuncSetAttribute(k_tp_batched<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CU(cudaFuncSetAttribute(k_tp_batched<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CU(cudaFuncSetAttribute(k_backsolve_batched, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     out = std::move(c);
     return 0;
 }
@@ -1893,6 +1896,7 @@ int dhqr_get_option(dhqr_handle c, const char* key, int64_t* value) {
     else if (!strcmp(key, "sms")) *value = c->sms;
     else if (!strcmp(key, "append_max_rows")) *value = narrow_panel_max_rows(c);
     else if (!strcmp(key, "batch_max_elems")) *value = BQ_MAX_ELEMS;
+    else if (!strcmp(key, "batch_update_max_cols")) *value = BQ_UPD_MAX_COLS;
     else if (!strcmp(key, "rank")) *value = c->rank;
     else if (!strcmp(key, "nranks")) *value = c->nranks;
     else return set_err(-2, "unknown option '%s'", key);
@@ -2935,6 +2939,137 @@ int dhqr_solve_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, c
                            const double* d_alpha, int64_t stride_alpha, double* d_b, int64_t ldb, int64_t stride_b, int nrhs,
                            void* stream) {
     return apply_batched(c, m, n, batch, dA, lda, stride_a, d_alpha, stride_alpha, d_b, ldb, stride_b, nrhs, stream, true, true);
+}
+
+// ---- batched append and downdate, batched back-substitution (DESIGN §2.13) ----------------------------------------------------
+// dhqr_qr_append_batched_f64 (hyp = false, the rows are B) and dhqr_qr_downdate_batched_f64 (the rows are Z, d_info is argument 22)
+static int tp_batched(dhqr_context* c, int64_t n, int64_t k, int64_t batch, double* dR, int64_t ldr, int64_t stride_r, double* d_alpha,
+                      int64_t stride_alpha, double* dB, int64_t ldb, int64_t stride_b, double* d_vtop, int64_t stride_vtop, double* d_c,
+                      int64_t ldc, int64_t stride_c, double* d_e, int64_t lde, int64_t stride_e, int nrhs, int64_t* d_info, bool hyp,
+                      void* stream) {
+    const char* b = hyp ? "Z" : "B";
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the batched %s is single-GPU (the handle has %d ranks)", hyp ? "downdate" : "append", c->nranks);
+    if (n < 0) return set_err(-2, "n < 0");
+    if (k < 0) return set_err(-3, "k < 0");
+    const int64_t ncol = n + std::max(nrhs, 0);
+    if (ncol > BQ_UPD_MAX_COLS)
+        return set_err(-3, "n + nrhs = %lld exceeds batch_update_max_cols (%d)", (long long)ncol, BQ_UPD_MAX_COLS);
+    if (ncol > 0 && k > BQ_MAX_ELEMS / ncol)
+        return set_err(-3, "k * (n + nrhs) exceeds batch_max_elems (%lld): split the block", (long long)BQ_MAX_ELEMS);
+    if (batch < 0) return set_err(-4, "batch < 0");
+    if (batch * batched_geom(k, ncol).cs > INT32_MAX) return set_err(-4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
+    const bool work = batch > 0 && n > 0 && k > 0, rhs = work && nrhs > 0;
+    if (batch > 0 && n > 0 && !dR) return set_err(-5, "null R");
+    TRY(check_elem_ptr<double>(dR, -5, "R"));
+    if (ldr < std::max<int64_t>(1, n)) return set_err(-6, "ldr < max(1,n)");
+    if (batch > 1 && (__int128)stride_r < (__int128)ldr * n) return set_err(-7, "stride_r < ldr * n");
+    const size_t rbytes = batch_span(batch, stride_r, n, n, ldr), abytes = batch_span(batch, stride_alpha, n, 1, n);
+    if (batch > 0 && n > 0 && !d_alpha) return set_err(-8, "null alpha");
+    TRY(check_elem_ptr<double>(d_alpha, -8, "alpha"));
+    if (spans_overlap(d_alpha, abytes, dR, rbytes)) return set_err(-8, "alpha overlaps R");
+    if (batch > 1 && stride_alpha < n) return set_err(-9, "stride_alpha < n");
+    const size_t bbytes = work ? batch_span(batch, stride_b, k, n, ldb) : 0;
+    if (work && !dB) return set_err(-10, "null %s", b);
+    TRY(check_elem_ptr<double>(dB, -10, b));
+    if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-10, "%s overlaps R or alpha", b);
+    if (ldb < std::max<int64_t>(1, k)) return set_err(-11, hyp ? "ldz < max(1,k)" : "ldb < max(1,k)");
+    if (batch > 1 && (__int128)stride_b < (__int128)ldb * n) return set_err(-12, hyp ? "stride_z < ldz * n" : "stride_b < ldb * n");
+    const size_t vbytes = work ? batch_span(batch, stride_vtop, n, 1, n) : 0;
+    if (work && !d_vtop) return set_err(-13, "null vtop");
+    TRY(check_elem_ptr<double>(d_vtop, -13, "vtop"));
+    if (spans_overlap(d_vtop, vbytes, dR, rbytes) || spans_overlap(d_vtop, vbytes, d_alpha, abytes) || spans_overlap(d_vtop, vbytes, dB, bbytes))
+        return set_err(-13, "vtop overlaps R, alpha or %s", b);
+    if (batch > 1 && stride_vtop < n) return set_err(-14, "stride_vtop < n");
+    size_t cbytes = 0, ebytes = 0;
+    if (nrhs > 0) {
+        cbytes = rhs ? batch_span(batch, stride_c, n, nrhs, ldc) : 0;
+        if (rhs && !d_c) return set_err(-15, "null c");
+        TRY(check_elem_ptr<double>(d_c, -15, "c"));
+        if (spans_overlap(d_c, cbytes, dR, rbytes) || spans_overlap(d_c, cbytes, d_alpha, abytes) || spans_overlap(d_c, cbytes, dB, bbytes) ||
+            spans_overlap(d_c, cbytes, d_vtop, vbytes))
+            return set_err(-15, "c overlaps R, alpha, %s or vtop", b);
+        if (ldc < std::max<int64_t>(1, n)) return set_err(-16, "ldc < max(1,n)");
+        if (batch > 1 && (__int128)stride_c < (__int128)ldc * nrhs) return set_err(-17, "stride_c < ldc * nrhs");
+        ebytes = rhs ? batch_span(batch, stride_e, k, nrhs, lde) : 0;
+        if (rhs && !d_e) return set_err(-18, "null e");
+        TRY(check_elem_ptr<double>(d_e, -18, "e"));
+        if (spans_overlap(d_e, ebytes, dR, rbytes) || spans_overlap(d_e, ebytes, d_alpha, abytes) || spans_overlap(d_e, ebytes, dB, bbytes) ||
+            spans_overlap(d_e, ebytes, d_vtop, vbytes) || spans_overlap(d_e, ebytes, d_c, cbytes))
+            return set_err(-18, "e overlaps R, alpha, %s, vtop or c", b);
+        if (lde < std::max<int64_t>(1, k)) return set_err(-19, "lde < max(1,k)");
+        if (batch > 1 && (__int128)stride_e < (__int128)lde * nrhs) return set_err(-20, "stride_e < lde * nrhs");
+    }
+    if (nrhs < 0) return set_err(-21, "nrhs < 0");
+    if (hyp) {
+        const size_t ibytes = work ? (size_t)batch * 8 : 0;
+        if (work && !d_info) return set_err(-22, "null info");
+        TRY(check_elem_ptr<int64_t>(d_info, -22, "info"));
+        if (spans_overlap(d_info, ibytes, dR, rbytes) || spans_overlap(d_info, ibytes, d_alpha, abytes) ||
+            spans_overlap(d_info, ibytes, dB, bbytes) || spans_overlap(d_info, ibytes, d_vtop, vbytes) ||
+            spans_overlap(d_info, ibytes, d_c, cbytes) || spans_overlap(d_info, ibytes, d_e, ebytes))
+            return set_err(-22, "info overlaps R, alpha, Z, vtop, c or e");
+    }
+    if (!work) return 0;
+    CU(cudaSetDevice(c->device));
+    const BatchedGeom g = batched_geom(k, ncol);
+    const double flops = (double)batch * (4.0 * k + 6.0) * n * (ncol - (n + 1) / 2.0);
+    return launch_batched(c, (cudaStream_t)stream, hyp ? "k_downdate_batched" : "k_append_batched", flops,
+                          hyp ? k_tp_batched<true> : k_tp_batched<false>, g, batch, 1, smem_tp_batched(g, ncol), dR, ldr, stride_r,
+                          d_alpha, stride_alpha, dB, ldb, stride_b, d_vtop, stride_vtop, rhs ? d_c : nullptr, ldc, stride_c,
+                          rhs ? d_e : nullptr, lde, stride_e, hyp ? d_info : nullptr, (int)n, (int)k, nrhs, g.rpc);
+}
+
+int dhqr_qr_append_batched_f64(dhqr_handle c, int64_t n, int64_t k, int64_t batch, double* dR, int64_t ldr, int64_t stride_r,
+                               double* d_alpha, int64_t stride_alpha, double* dB, int64_t ldb, int64_t stride_b, double* d_vtop,
+                               int64_t stride_vtop, double* d_c, int64_t ldc, int64_t stride_c, double* d_e, int64_t lde, int64_t stride_e,
+                               int nrhs, void* stream) {
+    return tp_batched(c, n, k, batch, dR, ldr, stride_r, d_alpha, stride_alpha, dB, ldb, stride_b, d_vtop, stride_vtop, d_c, ldc, stride_c,
+                      d_e, lde, stride_e, nrhs, nullptr, false, stream);
+}
+
+int dhqr_qr_downdate_batched_f64(dhqr_handle c, int64_t n, int64_t k, int64_t batch, double* dR, int64_t ldr, int64_t stride_r,
+                                 double* d_alpha, int64_t stride_alpha, double* dZ, int64_t ldz, int64_t stride_z, double* d_vtop,
+                                 int64_t stride_vtop, double* d_c, int64_t ldc, int64_t stride_c, double* d_e, int64_t lde,
+                                 int64_t stride_e, int nrhs, int64_t* d_info, void* stream) {
+    return tp_batched(c, n, k, batch, dR, ldr, stride_r, d_alpha, stride_alpha, dZ, ldz, stride_z, d_vtop, stride_vtop, d_c, ldc, stride_c,
+                      d_e, lde, stride_e, nrhs, d_info, true, stream);
+}
+
+int dhqr_backsolve_batched_f64(dhqr_handle c, int64_t n, int64_t batch, const double* dR, int64_t ldr, int64_t stride_r,
+                               const double* d_alpha, int64_t stride_alpha, double* d_b, int64_t ldb, int64_t stride_b, int nrhs,
+                               void* stream) {
+    if (!c) return set_err(-1, "null handle");
+    if (c->nranks != 1) return set_err(-1, "the batched back-substitution is single-GPU (the handle has %d ranks)", c->nranks);
+    if (n < 0) return set_err(-2, "n < 0");
+    if (n > BQ_UPD_MAX_COLS) return set_err(-2, "n = %lld exceeds batch_update_max_cols (%d)", (long long)n, BQ_UPD_MAX_COLS);
+    if (batch < 0) return set_err(-3, "batch < 0");
+    if (batch > INT32_MAX) return set_err(-3, "batch too large for one grid (> 2^31 - 1)");
+    if (batch > 0 && n > 0 && !dR) return set_err(-4, "null R");
+    TRY(check_elem_ptr<double>(dR, -4, "R"));
+    if (ldr < std::max<int64_t>(1, n)) return set_err(-5, "ldr < max(1,n)");
+    if (batch > 1 && (__int128)stride_r < (__int128)ldr * n) return set_err(-6, "stride_r < ldr * n");
+    const size_t rbytes = batch_span(batch, stride_r, n, n, ldr), abytes = batch_span(batch, stride_alpha, n, 1, n);
+    if (batch > 0 && n > 0 && !d_alpha) return set_err(-7, "null alpha");
+    TRY(check_elem_ptr<double>(d_alpha, -7, "alpha"));
+    if (batch > 1 && stride_alpha < n) return set_err(-8, "stride_alpha < n");
+    if (batch > 0 && n > 0 && nrhs > 0 && !d_b) return set_err(-9, "null b");
+    TRY(check_elem_ptr<double>(d_b, -9, "b"));
+    const size_t bbytes = batch_span(batch, stride_b, n, nrhs, ldb);
+    if (spans_overlap(d_b, bbytes, dR, rbytes) || spans_overlap(d_b, bbytes, d_alpha, abytes)) return set_err(-9, "b overlaps R or alpha");
+    if (ldb < std::max<int64_t>(1, n)) return set_err(-10, "ldb < max(1,n)");
+    if (batch > 1 && (__int128)stride_b < (__int128)ldb * nrhs) return set_err(-11, "stride_b < ldb * nrhs");
+    if (nrhs < 0) return set_err(-12, "nrhs < 0");
+    if (batch == 0 || n == 0 || nrhs == 0) return 0;
+    CU(cudaSetDevice(c->device));
+    const int kc = (int)std::min<int64_t>({(int64_t)BQ_KC, BQ_SLAB / n, (int64_t)nrhs});
+    const int ny = (int)std::min<int64_t>((nrhs + kc - 1) / kc, 65535);
+    BatchedGeom g;
+    g.cs = 1;
+    g.rpc = (int)n;
+    g.threads = 32 * (int)std::min<int64_t>(std::max<int64_t>((n + 31) / 32, 1), 8);
+    return launch_batched(c, (cudaStream_t)stream, "k_backsolve_batched", (double)batch * nrhs * n * n, k_backsolve_batched, g, batch, ny,
+                          (size_t)kc * n * 8, dR, ldr, stride_r, d_alpha, stride_alpha, d_b, ldb, stride_b, (int)n, nrhs, kc);
 }
 
 // ---- host-buffer entry points --------------------------------------------------------------------

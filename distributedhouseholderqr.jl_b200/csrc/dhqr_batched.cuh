@@ -80,6 +80,29 @@ __device__ __forceinline__ double bq_warp_sum(double v) {
 // norm of column j + 1 reads exactly the entries this thread updated in step j.
 __device__ __forceinline__ int bq_first(int lo, int t, int T) { return lo <= t ? t : t + (lo - t + T - 1) / T * T; }
 
+// x = R^{-1} xs for kw right-hand sides xs ([kw][n] in shared memory, overwritten) by the block's threads, then x to b[0:n, 0:kw]
+// (leading dimension ldb).  R = triu(R, 1) + diag(ap): only the strict upper triangle of R and ap are read.  Column i of R at a
+// time, from the last: x_i = xs_i / ap[i], then xs[0:i] -= R[0:i, i] x_i; every entry sees its updates in the order of i, whatever
+// the block size.
+__device__ __forceinline__ void bq_backsolve(double* xs, int n, int kw, const double* __restrict__ R, int64_t ldr,
+                                             const double* __restrict__ ap, double* __restrict__ b, int64_t ldb) {
+    const int tid = threadIdx.x, T = blockDim.x;
+    for (int i = n - 1; i >= 0; --i) {
+        for (int k = tid; k < kw; k += T) xs[(int64_t)k * n + i] /= ap[i];
+        __syncthreads();
+        const double* Ri = R + (int64_t)i * ldr;
+        for (int64_t e = tid; e < (int64_t)i * kw; e += T) {
+            const int k = (int)(e / i), l = (int)(e - (int64_t)k * i);
+            xs[(int64_t)k * n + l] -= Ri[l] * xs[(int64_t)k * n + i];
+        }
+        __syncthreads();
+    }
+    for (int64_t e = tid; e < (int64_t)n * kw; e += T) {
+        const int k = (int)(e / n), i = (int)(e - (int64_t)k * n);
+        b[(int64_t)k * ldb + i] = xs[(int64_t)k * n + i];
+    }
+}
+
 // Factor problem blockIdx.x / cs in place.  Per column j: (1) each CTA's partial of ||A[j:, j]||^2; cluster barrier; every CTA sums
 // the partials in rank order and reads x0 = A[j, j] from the CTA that holds row j; (2) alpha, f and v in place (S:129-135, sign(0)
 // = 0 as in the reference); (3) w_c = v' A[j:, c] for c > j, warps owning columns and lanes rows; cluster barrier; every CTA sums
@@ -242,23 +265,7 @@ __global__ void __launch_bounds__(256) k_apply_batched(const double* __restrict_
                 bp[(int64_t)(k0 + k) * ldb + r0 + i] = Bs[(int64_t)k * rpc + i];
             }
             bq_cluster_sync();                                                  // CTA 0 has read every slab
-            if (rank == 0) {
-                const double* ap = alpha + prob * stride_alpha;
-                for (int i = n - 1; i >= 0; --i) {
-                    for (int k = tid; k < kw; k += T) xs[(int64_t)k * n + i] /= ap[i];
-                    __syncthreads();
-                    const double* Ri = Ap + (int64_t)i * lda;
-                    for (int64_t e = tid; e < (int64_t)i * kw; e += T) {
-                        const int k = (int)(e / i), l = (int)(e - (int64_t)k * i);
-                        xs[(int64_t)k * n + l] -= Ri[l] * xs[(int64_t)k * n + i];
-                    }
-                    __syncthreads();
-                }
-                for (int64_t e = tid; e < (int64_t)n * kw; e += T) {
-                    const int k = (int)(e / n), i = (int)(e - (int64_t)k * n);
-                    bp[(int64_t)(k0 + k) * ldb + i] = xs[(int64_t)k * n + i];
-                }
-            }
+            if (rank == 0) bq_backsolve(xs, n, kw, Ap, lda, alpha + prob * stride_alpha, bp + (int64_t)k0 * ldb, ldb);
         } else {
             __syncthreads();
             for (int64_t e = tid; e < (int64_t)nr * kw; e += T) {
@@ -269,4 +276,151 @@ __global__ void __launch_bounds__(256) k_apply_batched(const double* __restrict_
         __syncthreads();
     }
     bq_cluster_sync();   // no CTA leaves while another may still read its w partials
+}
+
+// ---- batched append and downdate (dhqr_qr_append_batched_f64, dhqr_qr_downdate_batched_f64; DESIGN §2.13) ---------------------
+// Problem i folds its k x n block B (or removes Z) into its n x n triangle R, and transforms [c; e] with the same reflectors: the
+// column steps of k_tp_panel (dhqr_append.cuh) on one problem per cluster.  The slab of CTA r is rows [r * rpc, (r + 1) * rpc) of
+// [B | e], n + nrhs columns, column-major; the geometry is batched_geom(k, n + nrhs).  R is never held: row j of R and of c is read
+// from global memory at step j, and only reflector j touches it.
+constexpr int BQ_UPD_MAX_COLS = 1024;   // n + nrhs at most (read-only option batch_update_max_cols); k (n + nrhs) <= BQ_MAX_ELEMS
+// Shared memory: the slab and three column vectors.  At cs = 8, rpc (n + nrhs) < BQ_SLAB + (n + nrhs), so the worst case is
+// (24 576 + 4 x 1024) x 8 B = 229 376 B, inside the 227 KiB (232 448 B) a CTA may opt in to.
+inline size_t smem_tp_batched(const BatchedGeom& g, int64_t ncol) { return ((size_t)g.rpc * ncol + 3 * (size_t)ncol) * 8; }
+
+// Per column j, with x0 = alpha[j] and R[j, :] as they are on entry (reflectors 0..j-1 never touch row j):
+//   (1) each warp owns columns c >= j of the slab and writes this CTA's partial of B[:, j]' B[:, c] (lanes own rows); cluster
+//       barrier; every CTA sums the partials in rank order: w[j] = t = ||B[:, j]||^2, w[c] = t_jc;
+//   (2) every thread forms, from identical data, the scalars of k_tp_panel: append s = sqrt(t + x0^2), alpha = -sign(x0) s (a zero
+//       x0 counts as positive), f = 1 / sqrt(s (s + |x0|)), vtop = f (x0 - alpha), w_c = f t_jc + vtop R[j, c]; downdate s^2 =
+//       (|x0| - sqrt(t)) (|x0| + sqrt(t)), w_c = vtop R[j, c] - f t_jc, and the failure rule of dhqr_qr_downdate_f64;
+//   (3) B[:, j] <- V2 = f B[:, j], B[:, c] -= V2 w_c on the slab.
+// Columns c >= n are the right-hand sides: R[j, c] is then c[j, c - n], and e is transformed with B.  R's row j, c's row j and
+// alpha[j] are read by every CTA after the barrier of step j, so CTA 0 writes them (R[j, c] - vtop w_c) after the barrier of step
+// j + 1, when no CTA can still read them; the w partials alternate between two buffers for the same reason as in k_apply_batched.
+template <bool HYP>
+__global__ void __launch_bounds__(256) k_tp_batched(double* __restrict__ R, int64_t ldr, int64_t stride_r, double* __restrict__ alpha,
+                                                    int64_t stride_alpha, double* __restrict__ B, int64_t ldb, int64_t stride_b,
+                                                    double* __restrict__ vtop, int64_t stride_vtop, double* __restrict__ cm, int64_t ldc,
+                                                    int64_t stride_c, double* __restrict__ e, int64_t lde, int64_t stride_e,
+                                                    int64_t* __restrict__ info, int n, int k, int nrhs, int rpc) {
+    extern __shared__ double bq_sm[];
+    const int ncol = n + nrhs;
+    double* wpart = bq_sm;               // [2][ncol] this CTA's partials
+    double* w = wpart + 2 * ncol;        // [ncol] t_jc, then w_c
+    double* S = w + ncol;                // [ncol][rpc] the slab of [B | e]
+    const int tid = threadIdx.x, T = blockDim.x, warp = tid >> 5, lane = tid & 31, nw = T >> 5;
+    const uint32_t cs = bq_nrank(), rank = bq_rank();
+    const int64_t prob = blockIdx.x / cs;
+    double* Rp = R + prob * stride_r;
+    double* al = alpha + prob * stride_alpha;
+    double* Bp = B + prob * stride_b;
+    double* cp = cm + prob * stride_c;
+    double* ep = e + prob * stride_e;
+    const int r0 = (int)rank * rpc;
+    const int nr = max(0, min(k - r0, rpc));
+    // column c of [R | c] at row j
+    auto top = [&](int j, int c) -> double* { return c < n ? Rp + (int64_t)c * ldr + j : cp + (int64_t)(c - n) * ldc + j; };
+
+    for (int64_t x = tid; x < (int64_t)nr * ncol; x += T) {
+        const int c = (int)(x / nr), i = (int)(x - (int64_t)c * nr);
+        S[(int64_t)c * rpc + i] = c < n ? Bp[(int64_t)c * ldb + r0 + i] : ep[(int64_t)(c - n) * lde + r0 + i];
+    }
+    __syncthreads();
+
+    double vt_prev = 0.0, a_prev = 0.0;
+    bool dead = false;
+    int first = -1;
+    for (int j = 0; j < n; ++j) {
+        const double* Sj = S + (int64_t)j * rpc;
+        double* wp = wpart + (j & 1) * ncol;
+        for (int c = j + warp; c < ncol; c += nw) {
+            const double* Sc = S + (int64_t)c * rpc;
+            double acc = 0.0;
+            for (int i = lane; i < nr; i += 32) acc += Sj[i] * Sc[i];
+            acc = bq_warp_sum(acc);
+            if (lane == 0) wp[c] = acc;
+        }
+        bq_cluster_sync();
+        for (int c = j + tid; c < ncol; c += T) {
+            if (rank == 0 && j > 0) {                                           // row j - 1, now that no CTA reads it
+                double* p = top(j - 1, c);
+                *p -= vt_prev * w[c];
+            }
+            double s = 0.0;
+            for (uint32_t q = 0; q < cs; ++q) s += bq_ld_cluster(wp + c, q);
+            w[c] = s;
+        }
+        if (rank == 0 && tid == 0 && j > 0) al[j - 1] = a_prev;
+        __syncthreads();
+        const double x0 = al[j], t = w[j];
+        double f, vt, a;
+        if constexpr (!HYP) {
+            const double s = sqrt(t + x0 * x0);
+            a = s == 0.0 ? 0.0 : (x0 >= 0.0 ? -s : s);
+            f = s == 0.0 ? 0.0 : 1.0 / sqrt(s * (s + fabs(x0)));
+            vt = f * (x0 - a);
+        } else {
+            const double ax = fabs(x0), rt = sqrt(t);
+            const double s2 = (ax - rt) * (ax + rt);
+            const bool fails = isnan(s2) || (t > 0.0 && s2 <= 0.0);
+            if (fails && !dead) first = j;
+            dead = dead || fails;
+            const double s = dead ? 0.0 : sqrt(s2);
+            a = dead ? __longlong_as_double(0x7ff8000000000000ll) : (s == 0.0 ? 0.0 : (x0 >= 0.0 ? -s : s));
+            f = (dead || s == 0.0) ? 0.0 : 1.0 / sqrt(s * (s + ax));
+            vt = dead ? 0.0 : f * (x0 - a);
+        }
+        for (int c = j + 1 + tid; c < ncol; c += T) {                          // w[j] = t is not overwritten
+            const double rc = *top(j, c);
+            if constexpr (!HYP) w[c] = f * w[c] + vt * rc;
+            else w[c] = dead ? 0.0 : vt * rc - f * w[c];
+        }
+        if (rank == 0 && tid == 0) vtop[prob * stride_vtop + j] = vt;
+        vt_prev = vt;
+        a_prev = a;
+        __syncthreads();
+        for (int i = tid; i < nr; i += T) {
+            const double v = (HYP && dead) ? 0.0 : f * Sj[i];
+            S[(int64_t)j * rpc + i] = v;
+            for (int c = j + 1; c < ncol; ++c) S[(int64_t)c * rpc + i] -= v * w[c];
+        }
+        __syncthreads();
+    }
+    bq_cluster_sync();   // no CTA reads row n - 1 or another's partials any more
+    if (rank == 0) {
+        for (int c = n + tid; c < ncol; c += T) *top(n - 1, c) -= vt_prev * w[c];
+        if (tid == 0) {
+            al[n - 1] = a_prev;
+            if constexpr (HYP) info[prob] = first + 1;
+        }
+    }
+    for (int64_t x = tid; x < (int64_t)nr * ncol; x += T) {
+        const int c = (int)(x / nr), i = (int)(x - (int64_t)c * nr);
+        const double v = S[(int64_t)c * rpc + i];
+        if (c < n) Bp[(int64_t)c * ldb + r0 + i] = v;
+        else ep[(int64_t)(c - n) * lde + r0 + i] = v;
+    }
+}
+
+// b[0:n] <- R^{-1} b[0:n] of problem blockIdx.x for right-hand-side chunks blockIdx.y, blockIdx.y + gridDim.y, ... of kc columns:
+// the back-substitution of k_apply_batched<true, true> (bq_backsolve) on b's top n rows, loaded into shared memory.
+__global__ void __launch_bounds__(256) k_backsolve_batched(const double* __restrict__ R, int64_t ldr, int64_t stride_r,
+                                                           const double* __restrict__ alpha, int64_t stride_alpha, double* __restrict__ b,
+                                                           int64_t ldb, int64_t stride_b, int n, int nrhs, int kc) {
+    extern __shared__ double bq_sm[];
+    double* xs = bq_sm;                  // [kc][n]
+    const int tid = threadIdx.x, T = blockDim.x;
+    const int64_t prob = blockIdx.x;
+    double* bp = b + prob * stride_b;
+    for (int k0 = blockIdx.y * kc; k0 < nrhs; k0 += gridDim.y * kc) {
+        const int kw = min(kc, nrhs - k0);
+        for (int64_t x = tid; x < (int64_t)n * kw; x += T) {
+            const int k = (int)(x / n), i = (int)(x - (int64_t)k * n);
+            xs[(int64_t)k * n + i] = bp[(int64_t)(k0 + k) * ldb + i];
+        }
+        __syncthreads();
+        bq_backsolve(xs, n, kw, R + prob * stride_r, ldr, alpha + prob * stride_alpha, bp + (int64_t)k0 * ldb, ldb);
+        __syncthreads();
+    }
 }

@@ -247,6 +247,47 @@ function ldiv_batched(A::CuArray{Float64,3}, α::CuMatrix{Float64}, b::CuArray{F
         stride(s, 3), size(s, 2), stream_ptr()))
     return s[1:n, :, :]
 end
+# ---- rows into and out of many small triangles in one launch (not in the reference), single GPU, DESIGN §2.13 ----
+# Problem i: R = triu(R[1:n, 1:n, i], 1) + diag(α[:, i]) (a qr_batched! factorisation works), the k x n block B[:, :, i]
+# (overwritten with the reflector tails), [c; e] = [c[:, :, i]; e[:, :, i]] transformed in the same launch (nothing: pass c and e
+# with size(c, 2) == 0).  n + nrhs <= batch_update_max_cols and k (n + nrhs) <= batch_max_elems.  Returns vtop (n x batch), and
+# for the downdate also info (batch, on the device): 0, or the 1-based column at which problem i's removal proved impossible.
+function _tp_batched!(name::Symbol, R::CuArray{Float64,3}, α::CuMatrix{Float64}, B::CuArray{Float64,3}, c::CuArray{Float64,3},
+                      e::CuArray{Float64,3}, info)
+    m, n, batch = size(R)
+    k = size(B, 1)
+    nrhs = size(c, 2)
+    vtop = CUDA.zeros(Float64, n, batch)
+    ptrs = (handle().ptr, n, k, batch, pointer(R), max(stride(R, 2), m), stride(R, 3), pointer(α), n, pointer(B), max(stride(B, 2), k),
+            stride(B, 3), pointer(vtop), n, pointer(c), max(stride(c, 2), n), stride(c, 3), pointer(e), max(stride(e, 2), k), stride(e, 3),
+            Cint(nrhs))
+    if info === nothing
+        GC.@preserve R α B vtop c e check(name, ccall((:dhqr_qr_append_batched_f64, libdhqr), Cint,
+            (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Int64,
+             CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, Int64, Cint, Ptr{Cvoid}), ptrs..., stream_ptr()))
+    else
+        GC.@preserve R α B vtop c e info check(name, ccall((:dhqr_qr_downdate_batched_f64, libdhqr), Cint,
+            (Ptr{Cvoid}, Int64, Int64, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Int64,
+             CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, Int64, Cint, CuPtr{Int64}, Ptr{Cvoid}),
+            ptrs..., pointer(info), stream_ptr()))
+    end
+    return vtop
+end
+append_rows_batched!(R, α, B, c, e) = _tp_batched!(:dhqr_qr_append_batched_f64, R, α, B, c, e, nothing)
+function downdate_rows_batched!(R, α, Z, c, e)
+    info = CUDA.zeros(Int64, size(R, 3))
+    vtop = _tp_batched!(:dhqr_qr_downdate_batched_f64, R, α, Z, c, e, info)
+    return vtop, info
+end
+# b[1:n, :, i] <- R_i \ b[1:n, :, i] for every problem (only R's strict upper triangle and α are read).
+function backsolve_batched!(b::CuArray{Float64,3}, R::CuArray{Float64,3}, α::CuMatrix{Float64})
+    m, n, batch = size(R)
+    GC.@preserve R α b check(:dhqr_backsolve_batched_f64, ccall((:dhqr_backsolve_batched_f64, libdhqr), Cint,
+        (Ptr{Cvoid}, Int64, Int64, CuPtr{Float64}, Int64, Int64, CuPtr{Float64}, Int64, CuPtr{Float64}, Int64, Int64, Cint, Ptr{Cvoid}),
+        handle().ptr, n, batch, pointer(R), max(stride(R, 2), m), stride(R, 3), pointer(α), n, pointer(b), max(stride(b, 2), size(b, 1)),
+        stride(b, 3), size(b, 2), stream_ptr()))
+    return b
+end
 # min ||A x - b|| for A fed as row blocks (CuMatrix or Matrix; host blocks are uploaded), from R = 0: x and the residual norm.
 function streaming_lstsq(blocks, n::Integer)
     H = DistributedHouseholderQRStruct(CUDA.zeros(Float64, n, n), CUDA.zeros(Float64, n))

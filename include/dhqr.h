@@ -117,7 +117,9 @@ int dhqr_destroy(dhqr_handle h);
  *                 "wide_panels" (outer panels factored by the 128-column chain), "wide_redone" (restarts after a refusal),
  *                 "qrcp_renorms" (exact column renorms of dhqr_qrcp_f64 and dhqr_qrcp_c64; device-side, read after synchronising),
  *                 "append_max_rows" (the largest k one dhqr_qr_append_f64 call takes on this device), "batch_max_elems" (the
- *                 largest m * n of one problem of the batched entry points)
+ *                 largest m * n of one problem of the batched entry points, and the largest k (n + nrhs) of the batched append and
+ *                 downdate), "batch_update_max_cols" (the largest n + nrhs of the batched append and downdate, and the largest n of
+ *                 dhqr_backsolve_batched_f64)
  *   dhqr_get_option reads "nb", "panel_ctas", "sync", "profile", "lookahead", "panel_fast", "wide_panel", "cvy_persist",
  *                 "qt_vec", "bs_wave", "unblocked_wave", "fuse_house", "host_chunk" and the read-only keys (not "epoch_near_wrap").
  *   Any other key returns -2 (unknown option). */
@@ -410,6 +412,56 @@ int dhqr_apply_q_batched_f64(dhqr_handle h, int64_t m, int64_t n, int64_t batch,
 int dhqr_solve_batched_f64(dhqr_handle h, int64_t m, int64_t n, int64_t batch, const double *dA, int64_t lda, int64_t stride_a,
                            const double *d_alpha, int64_t stride_alpha, double *d_b, int64_t ldb, int64_t stride_b, int nrhs,
                            void *stream);
+
+/* ---- batched append and downdate: rows into and out of many small triangles (not in the reference; DESIGN §2.13) -------------
+ * Problem i: R = triu(dR_i[0:n, 0:n], 1) + diag(alpha_i) with dR_i = dR + i * stride_r (leading dimension ldr >= max(1, n); any
+ * factorisation in the library's storage format, e.g. a problem of dhqr_qr_batched_f64), alpha_i = d_alpha + i * stride_alpha, the
+ * k x n block B_i (or Z_i) at dB + i * stride_b (ldb >= max(1, k)), vtop_i = d_vtop + i * stride_vtop (n entries), and, when
+ * nrhs > 0, c_i = d_c + i * stride_c (n x nrhs, ldc >= max(1, n)) and e_i = d_e + i * stride_e (k x nrhs, lde >= max(1, k)).
+ * Per problem, the storage contract is that of dhqr_qr_append_f64 / dhqr_qr_downdate_f64: only R's strict upper triangle and alpha
+ * are read and written, B (Z) is overwritten with the reflector tails V2 and vtop receives their tops, so dhqr_apply_qt_append_f64 /
+ * dhqr_apply_downdate_f64 take (B_i, vtop_i) unchanged.  [c_i; e_i] is transformed in the same launch (Q~'[c; e] for the append,
+ * Theta [c; e] for the downdate); nrhs = 0 transforms nothing, and c and e may then be null.  Each column follows the single-problem
+ * recurrences: alpha_j = -sign(x0) ||x|| with a zero x0 counted as positive (not dhqr_qr_batched_f64's sign(0) = 0), a zero column
+ * stores v~ = 0 and alpha = 0; the downdate's sigma^2 = (|x0| - sqrt(t)) (|x0| + sqrt(t)) and its failure rule: the first column with
+ * sigma^2 <= 0 while t > 0, or a NaN sigma^2, goes 1-based into d_info[i] (int64_t, batch entries, contiguous; 0 when the problem's
+ * removal succeeded), and that column and every later one of problem i store vtop = 0, V2 = 0, alpha = NaN.
+ *   - One cluster of 1, 2, 4 or 8 CTAs per problem, chosen from (n, k, nrhs) alone; the slab of [B | e] stays in shared memory and R
+ *     is read and written row by row.  Size limit: n + nrhs <= batch_update_max_cols (read-only option; 1024) and k (n + nrhs) <=
+ *     batch_max_elems (196 608), so that the slab (at most 24 576 + n + nrhs doubles per CTA) and three vectors of n + nrhs doubles
+ *     fit the 227 KiB of shared memory a CTA can have.  A larger block returns -3 and is split by the caller.
+ *   - Single GPU (a handle with nranks > 1 returns -1), stream-ordered, one kernel launch per call (profile classes
+ *     k_append_batched, k_downdate_batched), no workspace, no allocation, no synchronisation: a call captures into a CUDA graph on a
+ *     fresh handle.  Bitwise deterministic: a problem's bits depend on its own data and on (n, k, nrhs) only, not on batch, its
+ *     position, the leading dimensions, the strides, 8 B base offsets or the handle's history.  Nothing outside the operands is
+ *     written.  batch = 0, n = 0 or k = 0 is a no-op that writes nothing, d_info included.
+ *   - Strides (batch > 1): stride_r >= ldr * n, stride_alpha >= n, stride_b >= ldb * n, stride_vtop >= n, stride_c >= ldc * nrhs,
+ *     stride_e >= lde * nrhs.  The span of every operand over the batch must not intersect the span of an earlier one.
+ *   - Errors, in argument order, every check before anything is enqueued: -1 null or multi-rank handle, -2 n < 0, -3 k < 0 or the
+ *     size limit, -4 batch < 0 or batch x (CTAs per problem) > 2^31 - 1, -5 null (batch > 0, n > 0) or misaligned R, -6 ldr < max(1, n),
+ *     -7 stride_r, -8 null, misaligned or overlapping alpha, -9 stride_alpha, -10 null (batch, n, k > 0), misaligned or overlapping B,
+ *     -11 ldb < max(1, k), -12 stride_b, -13 null, misaligned or overlapping vtop, -14 stride_vtop; with nrhs > 0: -15 null, misaligned
+ *     or overlapping c, -16 ldc < max(1, n), -17 stride_c, -18 null, misaligned or overlapping e, -19 lde < max(1, k), -20 stride_e;
+ *     -21 nrhs < 0; the downdate: -22 null, misaligned or overlapping info. */
+int dhqr_qr_append_batched_f64(dhqr_handle h, int64_t n, int64_t k, int64_t batch, double *dR, int64_t ldr, int64_t stride_r,
+                               double *d_alpha, int64_t stride_alpha, double *dB, int64_t ldb, int64_t stride_b, double *d_vtop,
+                               int64_t stride_vtop, double *d_c, int64_t ldc, int64_t stride_c, double *d_e, int64_t lde, int64_t stride_e,
+                               int nrhs, void *stream);
+int dhqr_qr_downdate_batched_f64(dhqr_handle h, int64_t n, int64_t k, int64_t batch, double *dR, int64_t ldr, int64_t stride_r,
+                                 double *d_alpha, int64_t stride_alpha, double *dZ, int64_t ldz, int64_t stride_z, double *d_vtop,
+                                 int64_t stride_vtop, double *d_c, int64_t ldc, int64_t stride_c, double *d_e, int64_t lde,
+                                 int64_t stride_e, int nrhs, int64_t *d_info, void *stream);
+/* b_i[0:n] <- R_i^{-1} b_i[0:n] for every problem: R_i = triu(dR_i, 1) + diag(alpha_i) as above (only the strict upper triangle and
+ * alpha are read; the diagonal and lower part of dR_i may hold anything), b_i = d_b + i * stride_b (n x nrhs, ldb >= max(1, n); rows
+ * below n are neither read nor written).  The back-substitution of dhqr_solve_batched_f64, one CTA per problem and chunk of up to
+ * 32 right-hand sides; n <= batch_update_max_cols.  A zero alpha propagates Inf / NaN.  Same stream, graph, determinism and no-op
+ * rules (profile class k_backsolve_batched).  Errors: -1 null or multi-rank handle, -2 n < 0 or n > batch_update_max_cols, -3
+ * batch < 0 or > 2^31 - 1, -4 null (batch > 0, n > 0) or misaligned R, -5 ldr < max(1, n), -6 stride_r < ldr * n, -7 null or
+ * misaligned alpha, -8 stride_alpha < n, -9 null, misaligned or overlapping (R, alpha) b, -10 ldb < max(1, n), -11 stride_b < ldb *
+ * nrhs, -12 nrhs < 0.  batch = 0, n = 0 or nrhs = 0 is a no-op. */
+int dhqr_backsolve_batched_f64(dhqr_handle h, int64_t n, int64_t batch, const double *dR, int64_t ldr, int64_t stride_r,
+                               const double *d_alpha, int64_t stride_alpha, double *d_b, int64_t ldb, int64_t stride_b, int nrhs,
+                               void *stream);
 
 /* ---- host-buffer entry points (single GPU): the call a CPU-side user of qr! / \ makes -------
  * hA (m x n, lda) is copied to the device, factored, and copied back with alpha; blocks until
