@@ -728,25 +728,99 @@ static void build_panels(const std::vector<int64_t>& col0s, const std::vector<in
         for (int64_t o = 0; o < nls[r]; o += nb) out.push_back({(int)r, col0s[r] + o, (int)std::min<int64_t>(nb, nls[r] - o)});
 }
 
-static int check_common(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* A, int64_t lda) {
-    if (!c) return set_err(-1, "null handle");
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n_global < 0 || n_global > m) return set_err(-3, "need 0 <= n_global <= m (reference asserts full column rank shapes)");
-    if (col0 < 0 || col0 > n_global) return set_err(-4, "col0 out of range");
-    if (n_local < 0 || col0 + n_local > n_global) return set_err(-5, "n_local out of range");
-    if (n_local > 0 && !A) return set_err(-6, "null matrix pointer");
-    if (lda < std::max<int64_t>(1, m)) return set_err(-7, "lda < max(1,m)");
-    return 0;
-}
+// ------------------------------------------------------------------------------------------------
+// argument checks: the storage contract of include/dhqr.h
+// ------------------------------------------------------------------------------------------------
+// An entry point lists its arguments in order: require() for a scalar rule, operand() for a pointer with its extent.  The first
+// failing check sets the error, minus the argument's 1-based position, and turns every later check into a no-op; the entry point
+// returns that code (a Check converts to it) before anything is enqueued.  The success path neither allocates nor formats.
+enum : unsigned {
+    NEED = 1,       // a null pointer is an error (the entry point passes it when the operand is not empty)
+    ALIGN = 2,      // the pointer must be aligned for its element type, even when the operand is empty
+    DISJOINT = 4,   // the operand must not overlap any operand listed before it
+    OR_SAME = 8,    // ... unless it is that operand itself, with the same leading dimension (form_q's Q == A)
+};
+static unsigned when(bool cond, unsigned rules) { return cond ? rules : 0u; }
 
-// The alignment check of a pointer to T, before anything is enqueued instead of a fault on the device.  The complex kernels load
-// and store whole double2 elements, so a ComplexF64 pointer must be 16 B aligned.  The C-ABI takes void* and an 8 B aligned one is
-// legal C (double _Complex, Julia's ComplexF64, a reinterpreted view of a Float64 vector).
-template <typename T>
-static int check_elem_ptr(const void* p, int arg, const char* name) {
-    if ((uintptr_t)p % alignof(T) == 0) return 0;
-    if (std::is_same<T, double2>::value) return set_err(arg, "%s is not 16-byte aligned (ComplexF64 data needs the alignment of double2)", name);
-    return set_err(arg, "%s must be 8 B aligned", name);
+// rows x cols elements, leading dimension ld; `batch` of them `stride` elements apart (the stride counts when batch > 1)
+struct Extent { int64_t rows, cols, ld; bool has_ld; int64_t batch, stride; };
+static Extent mat(int64_t rows, int64_t cols, int64_t ld, int64_t batch = 1, int64_t stride = 0) {
+    return {rows, cols, ld, true, batch, stride};
+}
+static Extent vec(int64_t n, int64_t batch = 1, int64_t stride = 0) { return {n, 1, n, false, batch, stride}; }
+
+class Check {
+  public:
+    // argument 1: a null handle, or one of several ranks when the entry point is single-GPU (`single_gpu` names what it serves)
+    explicit Check(const dhqr_context* c, const char* single_gpu = nullptr) {
+        if (!c) fail(1, "null handle");
+        else if (single_gpu && c->nranks != 1) fail(1, "%s is single-GPU (the handle has %d ranks)", single_gpu, c->nranks);
+    }
+    operator int() const { return rc_; }
+
+    template <typename... A>
+    Check& require(bool ok, int pos, const char* fmt, A... args) {
+        if (!rc_ && !ok) fail(pos, fmt, args...);
+        return *this;
+    }
+
+    // Pointer argument `pos` to elements of type T; a matrix's leading dimension is argument pos + 1, and the stride (batch > 1)
+    // the argument after the last of these.  Checks null, alignment, ld, stride, then overlap with the operands listed before.
+    template <typename T>
+    Check& operand(int pos, const char* name, const void* p, const Extent& e, unsigned rules) {
+        if (rc_) return *this;
+        if ((rules & NEED) && !p) return fail(pos, "null %s", name);
+        // The complex kernels move whole double2 elements.  The C-ABI takes void*, and an 8 B aligned ComplexF64 pointer is legal C
+        // (double _Complex, Julia's ComplexF64, a reinterpreted view of a Float64 vector): refuse it here instead of faulting.
+        if ((rules & ALIGN) && (uintptr_t)p % alignof(T)) {
+            if (std::is_same<T, double2>::value)
+                return fail(pos, "%s is not 16-byte aligned (ComplexF64 data needs the alignment of double2)", name);
+            return fail(pos, "%s must be %d B aligned", name, (int)alignof(T));
+        }
+        if (e.has_ld && e.ld < std::max<int64_t>(1, e.rows))
+            return fail(pos + 1, "the leading dimension of %s is %lld < max(1, rows = %lld)", name, (long long)e.ld, (long long)e.rows);
+        if (e.batch > 1 && (__int128)e.stride < (__int128)e.ld * e.cols)
+            return fail(pos + (e.has_ld ? 2 : 1), "the stride of %s is %lld < %lld (%s)", name, (long long)e.stride,
+                        (long long)(e.ld * e.cols), e.has_ld ? "leading dimension x columns" : "its length");
+        const Span s = {name, (uintptr_t)p, span(e, sizeof(T)), e.ld};
+        for (int i = 0; i < nseen_ && (rules & DISJOINT); ++i) {
+            const Span& q = seen_[i];
+            if (s.bytes && q.bytes && s.p < q.p + q.bytes && q.p < s.p + s.bytes && !((rules & OR_SAME) && s.p == q.p && s.ld == q.ld))
+                return fail(pos, (rules & OR_SAME) ? "%s overlaps %s without being it (with the same leading dimension)" : "%s overlaps %s",
+                            name, q.name);
+        }
+        if (nseen_ < MAXOPS) seen_[nseen_++] = s;
+        return *this;
+    }
+
+  private:
+    static constexpr int MAXOPS = 8;   // the batched downdate has seven
+    struct Span { const char* name; uintptr_t p; size_t bytes; int64_t ld; };
+    int rc_ = 0;
+    int nseen_ = 0;
+    Span seen_[MAXOPS];
+
+    template <typename... A>
+    Check& fail(int pos, const char* fmt, A... args) {
+        rc_ = set_err(-pos, fmt, args...);
+        return *this;
+    }
+    // Bytes from the first element to one past the last; 0 when the operand is empty.  A negative stride counts as 0, and the span
+    // is clamped, so that an absurd stride or leading dimension cannot wrap the interval test.
+    static size_t span(const Extent& e, size_t esz) {
+        if (e.batch <= 0 || e.rows <= 0 || e.cols <= 0) return 0;
+        const __int128 n = (__int128)(e.batch - 1) * std::max<int64_t>(e.stride, 0) + (__int128)(e.cols - 1) * e.ld + e.rows;
+        const __int128 bytes = n * (__int128)esz, cap = (__int128)1 << 61;
+        return (size_t)(bytes > cap ? cap : bytes);
+    }
+};
+
+// arguments 2-5 of the column-block entry points: the m x n_global matrix and this rank's columns [col0, col0 + n_local)
+static void column_block(Check& a, int64_t m, int64_t n_global, int64_t col0, int64_t n_local) {
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n_global >= 0 && n_global <= m, 3, "need 0 <= n_global <= m (reference asserts full column rank shapes)");
+    a.require(col0 >= 0 && col0 <= n_global, 4, "col0 out of range");
+    a.require(n_local >= 0 && col0 + n_local <= n_global, 5, "n_local out of range");
 }
 
 // the profile class of a launch: the Float64 kernel's name or the ComplexF64 one's
@@ -1943,10 +2017,13 @@ int dhqr_profile_get(dhqr_handle c, int index, char* name, int name_len, double*
 
 int dhqr_qr_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, double* dA, int64_t lda,
                 double* d_alpha, int nb, void* stream) {
-    TRY(check_common(c, m, n_global, col0, n_local, dA, lda));
-    if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
+    Check a(c);
+    column_block(a, m, n_global, col0, n_local);
+    a.operand<double>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED));
+    a.operand<double>(8, "alpha", d_alpha, vec(n_global), when(n_global > 0, NEED));
+    a.require(nb == 0 || nb == 1 || (nb >= 32 && nb <= 128 && nb % 32 == 0), 9, "nb must be 0, 1 or a multiple of 32 in [32,128]");
+    TRY(a);
     if (nb == 0) nb = c->nb;
-    if (nb != 1 && (nb < 32 || nb > 128 || nb % 32)) return set_err(-9, "nb must be 0, 1 or a multiple of 32 in [32,128]");
     if (n_global == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -1974,10 +2051,12 @@ static int rhs_copy(cudaStream_t st, double* dst, int64_t lddst, const double* s
 // order for Q^H b (C3, S:227-229), in reverse rank order for Q b = H_1 ... H_n b.  The last owner to act broadcasts the result.
 static int apply_q_dist(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA, int64_t lda,
                         double* d_b, int64_t ldb, int nrhs, void* stream, int notrans) {
-    TRY(check_common(c, m, n_global, col0, n_local, dA, lda));
-    if (nrhs < 0) return set_err(-10, "nrhs < 0");
-    if (nrhs > 0 && !d_b) return set_err(-8, "null b");
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-9, "ldb < max(1,m)");
+    Check a(c);
+    column_block(a, m, n_global, col0, n_local);
+    a.operand<double>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED));
+    a.operand<double>(8, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED));
+    a.require(nrhs >= 0, 10, "nrhs < 0");
+    TRY(a);
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2018,11 +2097,13 @@ int dhqr_apply_q_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, i
 
 int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
                        int64_t lda, const double* d_alpha, double* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_common(c, m, n_global, col0, n_local, dA, lda));
-    if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
-    if (nrhs < 0) return set_err(-11, "nrhs < 0");
-    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
+    Check a(c);
+    column_block(a, m, n_global, col0, n_local);
+    a.operand<double>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED));
+    a.operand<double>(8, "alpha", d_alpha, vec(n_global), when(n_global > 0, NEED));
+    a.operand<double>(9, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED));
+    a.require(nrhs >= 0, 11, "nrhs < 0");
+    TRY(a);
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2057,6 +2138,14 @@ int dhqr_backsolve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
 
 int dhqr_solve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const double* dA,
                    int64_t lda, const double* d_alpha, double* d_b, int64_t ldb, int nrhs, void* stream) {
+    // Every argument before Q'b runs.  b, ldb and nrhs keep the codes of dhqr_apply_qt_f64, which reports them in its numbering.
+    Check a(c);
+    column_block(a, m, n_global, col0, n_local);
+    a.operand<double>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED));
+    a.operand<double>(8, "alpha", d_alpha, vec(n_global), when(n_global > 0, NEED));
+    a.operand<double>(8, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED));
+    a.require(nrhs >= 0, 10, "nrhs < 0");
+    TRY(a);
     TRY(dhqr_apply_qt_f64(c, m, n_global, col0, n_local, dA, lda, d_b, ldb, nrhs, stream));   // S:288
     return dhqr_backsolve_f64(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs, stream);   // S:291
 }
@@ -2064,34 +2153,19 @@ int dhqr_solve_f64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int
 // ---- ComplexF64 (S:9, S:51-59, S:162-196; test/runtests.jl:43) -------------------------------------------------------
 // Panels of 64 complex columns: complex column-by-column panel, then the trailing update as the REAL block reflector of the
 // 128 vectors [v_r, v_i] on the real view of the matrix (dhqr_complex.cuh).  Single GPU.
-static int check_complex(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* A, int64_t lda) {
-    TRY(check_common(c, m, n_global, col0, n_local, A, lda));
-    if (c->nranks != 1 || col0 != 0 || n_local != n_global) return set_err(-1, "the ComplexF64 path is single-GPU (col0 = 0, n_local = n_global)");
-    return 0;
-}
-
-// arguments of dhqr_backsolve_c64 and dhqr_solve_c64 (same signature)
-static int check_c64_args(dhqr_context* c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
-                          const void* d_alpha, const void* d_b, int64_t ldb, int nrhs) {
-    TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    TRY(check_elem_ptr<double2>(dA, -6, "A"));
-    if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
-    TRY(check_elem_ptr<double2>(d_alpha, -8, "alpha"));
-    if (nrhs < 0) return set_err(-11, "nrhs < 0");
-    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    TRY(check_elem_ptr<double2>(d_b, -9, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
-    return 0;
-}
+static const char* const C64_PATH = "the ComplexF64 path";
+static const char* const C64_BLOCK = "the ComplexF64 path is single-GPU (col0 = 0, n_local = n_global)";
 
 static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, double2* A, int64_t lda, double2* alpha);
 
 int dhqr_qr_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, void* dA, int64_t lda, void* d_alpha,
                 void* stream) {
-    TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    TRY(check_elem_ptr<double2>(dA, -6, "A"));
-    if (n_global > 0 && !d_alpha) return set_err(-8, "null alpha");
-    TRY(check_elem_ptr<double2>(d_alpha, -8, "alpha"));
+    Check a(c, C64_PATH);
+    column_block(a, m, n_global, col0, n_local);
+    a.require(col0 == 0 && n_local == n_global, 1, C64_BLOCK);
+    a.operand<double2>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED) | ALIGN);
+    a.operand<double2>(8, "alpha", d_alpha, vec(n_global), when(n_global > 0, NEED) | ALIGN);
+    TRY(a);
     if (n_global == 0) return 0;
     CU(cudaSetDevice(c->device));
     return qr_c64_local(c, (cudaStream_t)stream, m, n_global, (double2*)dA, lda, (double2*)d_alpha);
@@ -2125,12 +2199,13 @@ static int qr_c64_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, 
 
 int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                       void* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_complex(c, m, n_global, col0, n_local, dA, lda));
-    TRY(check_elem_ptr<double2>(dA, -6, "A"));
-    if (nrhs < 0) return set_err(-10, "nrhs < 0");
-    if (nrhs > 0 && !d_b) return set_err(-8, "null b");
-    TRY(check_elem_ptr<double2>(d_b, -8, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-9, "ldb < max(1,m)");
+    Check a(c, C64_PATH);
+    column_block(a, m, n_global, col0, n_local);
+    a.require(col0 == 0 && n_local == n_global, 1, C64_BLOCK);
+    a.operand<double2>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED) | ALIGN);
+    a.operand<double2>(8, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED) | ALIGN);
+    a.require(nrhs >= 0, 10, "nrhs < 0");
+    TRY(a);
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     return apply_q_local(c, (cudaStream_t)stream, m, n_global, (const double2*)dA, lda, (double2*)d_b, ldb, nrhs, 0);
@@ -2138,7 +2213,14 @@ int dhqr_apply_qt_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, 
 
 int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                        const void* d_alpha, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_c64_args(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs));
+    Check a(c, C64_PATH);
+    column_block(a, m, n_global, col0, n_local);
+    a.require(col0 == 0 && n_local == n_global, 1, C64_BLOCK);
+    a.operand<double2>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED) | ALIGN);
+    a.operand<double2>(8, "alpha", d_alpha, vec(n_global), when(n_global > 0, NEED) | ALIGN);
+    a.operand<double2>(9, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED) | ALIGN);
+    a.require(nrhs >= 0, 11, "nrhs < 0");
+    TRY(a);
     if (n_global == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2152,7 +2234,14 @@ int dhqr_backsolve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0,
 
 int dhqr_solve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int64_t n_local, const void* dA, int64_t lda,
                    const void* d_alpha, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_c64_args(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs));   // every argument, before Q'b runs
+    Check a(c, C64_PATH);                                                                       // every argument, before Q'b runs
+    column_block(a, m, n_global, col0, n_local);
+    a.require(col0 == 0 && n_local == n_global, 1, C64_BLOCK);
+    a.operand<double2>(6, "A", dA, mat(m, n_local, lda), when(n_local > 0, NEED) | ALIGN);
+    a.operand<double2>(8, "alpha", d_alpha, vec(n_global), when(n_global > 0, NEED) | ALIGN);
+    a.operand<double2>(9, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED) | ALIGN);
+    a.require(nrhs >= 0, 11, "nrhs < 0");
+    TRY(a);
     TRY(dhqr_apply_qt_c64(c, m, n_global, col0, n_local, dA, lda, d_b, ldb, nrhs, stream));                   // S:288
     return dhqr_backsolve_c64(c, m, n_global, col0, n_local, dA, lda, d_alpha, d_b, ldb, nrhs, stream);       // S:291
 }
@@ -2163,36 +2252,6 @@ int dhqr_solve_c64(dhqr_handle c, int64_t m, int64_t n_global, int64_t col0, int
 // (T, not T') to rows >= cs, columns [cs, n) of Q.  Columns left of cs are still unit vectors with zeros in rows >= cs, so the
 // panel leaves them alone: 2mn^2 - 2n^3/3 flops instead of the 4mn^2 - 2n^3 of Q applied to [I; 0].  V_p is packed before its
 // columns are overwritten, so in place and out of place are the same sweep.
-// Templates and overloads over the element type, which C linkage does not allow, sit in extern "C++" blocks; the dhqr_* functions
-// keep the C linkage of their declarations in dhqr.h.
-extern "C++" {
-
-template <typename T>
-static int check_form_q(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* Q, int64_t ldq) {
-    const size_t esz = sizeof(T);
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "form_q is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (n > 0 && !A) return set_err(-4, "null matrix pointer");
-    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
-    if (n > 0 && !Q) return set_err(-6, "null Q");
-    if (ldq < std::max<int64_t>(1, m)) return set_err(-7, "ldq < max(1,m)");
-    if (n > 0) {
-        const uintptr_t a0 = (uintptr_t)A, a1 = a0 + ((size_t)(n - 1) * lda + m) * esz;
-        const uintptr_t q0 = (uintptr_t)Q, q1 = q0 + ((size_t)(n - 1) * ldq + m) * esz;
-        if (q0 < a1 && a0 < q1 && !(Q == A && ldq == lda))
-            return set_err(-6, "Q overlaps A without being A itself (Q == A needs ldq == lda)");
-    }
-    if (std::is_same<T, double2>::value) {                  // Float64 pointers are not checked for alignment here
-        TRY(check_elem_ptr<T>(A, -4, "A"));
-        TRY(check_elem_ptr<T>(Q, -6, "Q"));
-    }
-    return 0;
-}
-
-}  // extern "C++"
-
 static int eye_cols(dhqr_context* c, cudaStream_t st, void* Q, bool cplx, int64_t ldq, int64_t m, int64_t c0, int kb) {
     const dim3 grid((unsigned)std::min<int64_t>((m + 255) / 256, 64), kb);
     return launch(c, st, cplx ? "k_eye_cols_c" : "k_eye_cols", 0.0, [&](CwtSlot) {
@@ -2202,7 +2261,12 @@ static int eye_cols(dhqr_context* c, cudaStream_t st, void* Q, bool cplx, int64_
 }
 
 int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, double* dQ, int64_t ldq, void* stream) {
-    TRY(check_form_q<double>(c, m, n, dA, lda, dQ, ldq));
+    Check a(c, "form_q");                                        // Float64 pointers are not checked for alignment here
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.operand<double>(4, "A", dA, mat(m, n, lda), when(n > 0, NEED));
+    a.operand<double>(6, "Q", dQ, mat(m, n, ldq), when(n > 0, NEED) | DISJOINT | OR_SAME);
+    TRY(a);
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2222,7 +2286,12 @@ int dhqr_form_q_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64
 // ComplexF64: the same sweep over 64-column complex panels on the real view of Q (2m x n, leading dimension 2 ldq), each panel the
 // real block reflector of its 128 vectors [v_r, v_i] (dhqr_complex.cuh); T from the Gram block of the update itself.
 int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, void* dQ, int64_t ldq, void* stream) {
-    TRY(check_form_q<double2>(c, m, n, dA, lda, dQ, ldq));
+    Check a(c, "form_q");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.operand<double2>(4, "A", dA, mat(m, n, lda), when(n > 0, NEED) | ALIGN);
+    a.operand<double2>(6, "Q", dQ, mat(m, n, ldq), when(n > 0, NEED) | ALIGN | DISJOINT | OR_SAME);
+    TRY(a);
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2242,43 +2311,26 @@ int dhqr_form_q_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t
 
 // ---- solves with the adjoint (LAPACK ?gels, TRANS = 'C') ------------------------------------------------------------------
 // forwardsolve: b[0:n] <- R^{-H} b[0:n].  solve_adj: the minimum-norm solution of A^H y = c (solve_adj_local).  Single GPU.
-extern "C++" {   // as for form_q above
+// Templates and overloads over the element type, which C linkage does not allow, sit in extern "C++" blocks; the dhqr_* functions
+// keep the C linkage of their declarations in dhqr.h.
+extern "C++" {
 
+// dhqr_forwardsolve_* (forward) and dhqr_solve_adj_*: the same arguments
 template <typename T>
-static int check_adj(dhqr_context* c, int64_t m, int64_t n, const void* A, int64_t lda, const void* alpha, const void* b, int64_t ldb,
-                     int nrhs) {
-    constexpr bool cplx = std::is_same<T, double2>::value;       // Float64 pointers are not checked for alignment here
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the adjoint solves are single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (n > 0 && !A) return set_err(-4, "null A");
-    if (cplx) TRY(check_elem_ptr<T>(A, -4, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
-    if (n > 0 && !alpha) return set_err(-6, "null alpha");
-    if (cplx) TRY(check_elem_ptr<T>(alpha, -6, "alpha"));
-    if (nrhs > 0 && !b) return set_err(-7, "null b");
-    if (cplx) TRY(check_elem_ptr<T>(b, -7, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-8, "ldb < max(1,m)");
-    if (nrhs < 0) return set_err(-9, "nrhs < 0");
-    return 0;
-}
-
-template <typename T>
-static int forwardsolve(dhqr_context* c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
-                        int nrhs, void* stream) {
-    TRY(check_adj<T>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs));
-    if (n == 0 || nrhs == 0) return 0;
+static int adjoint_solve(dhqr_context* c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
+                         int nrhs, void* stream, bool forward) {
+    const unsigned align = when(std::is_same<T, double2>::value, ALIGN);   // Float64 pointers are not checked for alignment here
+    Check a(c, "the adjoint solve");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.operand<T>(4, "A", dA, mat(m, n, lda), when(n > 0, NEED) | align);
+    a.operand<T>(6, "alpha", d_alpha, vec(n), when(n > 0, NEED) | align);
+    a.operand<T>(7, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED) | align);
+    a.require(nrhs >= 0, 9, "nrhs < 0");
+    TRY(a);
+    if ((forward ? n : m) == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
-    return forwardsolve_local(c, (cudaStream_t)stream, n, (const T*)dA, lda, (const T*)d_alpha, (T*)d_b, ldb, nrhs);
-}
-
-template <typename T>
-static int solve_adj(dhqr_context* c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
-                     int nrhs, void* stream) {
-    TRY(check_adj<T>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs));
-    if (m == 0 || nrhs == 0) return 0;
-    CU(cudaSetDevice(c->device));
+    if (forward) return forwardsolve_local(c, (cudaStream_t)stream, n, (const T*)dA, lda, (const T*)d_alpha, (T*)d_b, ldb, nrhs);
     return solve_adj_local(c, (cudaStream_t)stream, m, n, (const T*)dA, lda, (const T*)d_alpha, (T*)d_b, ldb, nrhs);
 }
 
@@ -2286,22 +2338,22 @@ static int solve_adj(dhqr_context* c, int64_t m, int64_t n, const void* dA, int6
 
 int dhqr_forwardsolve_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
                           int64_t ldb, int nrhs, void* stream) {
-    return forwardsolve<double>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
+    return adjoint_solve<double>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream, true);
 }
 
 int dhqr_forwardsolve_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b,
                           int64_t ldb, int nrhs, void* stream) {
-    return forwardsolve<double2>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
+    return adjoint_solve<double2>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream, true);
 }
 
 int dhqr_solve_adj_f64(dhqr_handle c, int64_t m, int64_t n, const double* dA, int64_t lda, const double* d_alpha, double* d_b,
                        int64_t ldb, int nrhs, void* stream) {
-    return solve_adj<double>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
+    return adjoint_solve<double>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream, false);
 }
 
 int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int64_t lda, const void* d_alpha, void* d_b, int64_t ldb,
                        int nrhs, void* stream) {
-    return solve_adj<double2>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream);
+    return adjoint_solve<double2>(c, m, n, dA, lda, d_alpha, d_b, ldb, nrhs, stream, false);
 }
 
 // ---- QR with column pivoting (LAPACK ?geqp3 / ?laqps, dhqr_qrcp.cuh), Float64 and ComplexF64 ---------------------------------
@@ -2310,7 +2362,7 @@ int dhqr_solve_adj_c64(dhqr_handle c, int64_t m, int64_t n, const void* dA, int6
 // ending the panel early: every panel has its static width and the host never needs a device value, so the driver is one static
 // loop and the call does not synchronise.  Single GPU, n <= m, no row limit.  T = double or double2; the workspace is sized in
 // doubles, and every section of it that holds T is aligned for T.
-extern "C++" {   // as for form_q above
+extern "C++" {   // as for the adjoint solves above
 
 // A[c1:, c1:] -= V F' on the window starting at row k0 (a multiple of 32), rows >= c1 only: the 32-wide C += V Y with Y = -F'
 static int qrcp_update(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, int64_t k0, int kb, double* A, int64_t lda,
@@ -2394,17 +2446,13 @@ static int qrcp_local(dhqr_context* c, cudaStream_t st, int64_t m, int64_t n, T*
 
 template <typename T>
 static int qrcp_factor(dhqr_context* c, int64_t m, int64_t n, void* dA, int64_t lda, void* d_alpha, int64_t* d_jpvt, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the pivoted factorisation is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (n > 0 && !dA) return set_err(-4, "null A");
-    TRY(check_elem_ptr<T>(dA, -4, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-5, "lda < max(1,m)");
-    if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
-    TRY(check_elem_ptr<T>(d_alpha, -6, "alpha"));
-    if (n > 0 && !d_jpvt) return set_err(-7, "null jpvt");
-    TRY(check_elem_ptr<int64_t>(d_jpvt, -7, "jpvt"));
+    Check a(c, "the pivoted factorisation");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.operand<T>(4, "A", dA, mat(m, n, lda), when(n > 0, NEED) | ALIGN);
+    a.operand<T>(6, "alpha", d_alpha, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<int64_t>(7, "jpvt", d_jpvt, vec(n), when(n > 0, NEED) | ALIGN);
+    TRY(a);
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     return qrcp_local(c, (cudaStream_t)stream, m, n, (T*)dA, lda, (T*)d_alpha, d_jpvt);
@@ -2427,22 +2475,16 @@ static int qrcp_scatter(dhqr_context* c, cudaStream_t st, int64_t n, int64_t ran
 template <typename T>
 static int qrcp_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha,
                       const int64_t* d_jpvt, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the pivoted solve is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
-    if (n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_elem_ptr<T>(dA, -5, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
-    if (n > 0 && !d_alpha) return set_err(-7, "null alpha");
-    TRY(check_elem_ptr<T>(d_alpha, -7, "alpha"));
-    if (n > 0 && !d_jpvt) return set_err(-8, "null jpvt");
-    TRY(check_elem_ptr<int64_t>(d_jpvt, -8, "jpvt"));
-    if (nrhs > 0 && !d_b) return set_err(-9, "null b");
-    TRY(check_elem_ptr<T>(d_b, -9, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-10, "ldb < max(1,m)");
-    if (nrhs < 0) return set_err(-11, "nrhs < 0");
+    Check a(c, "the pivoted solve");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.require(rank >= 0 && rank <= n, 4, "need 0 <= rank <= n");
+    a.operand<T>(5, "A", dA, mat(m, n, lda), when(n > 0, NEED) | ALIGN);
+    a.operand<T>(7, "alpha", d_alpha, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<int64_t>(8, "jpvt", d_jpvt, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<T>(9, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED) | ALIGN);
+    a.require(nrhs >= 0, 11, "nrhs < 0");
+    TRY(a);
     if (n == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2484,49 +2526,7 @@ int dhqr_solve_qrcp_c64(dhqr_handle c, int64_t m, int64_t n, int64_t rank, const
 // gives A P ~ Q1 [U^H 0] Z^H.  The minimum-norm solution of the rank-r problem is x = P Z [U^{-H} (Q^H b)[0:r]; 0], and the step
 // after Q^H b is exactly the minimum-norm solution of R_r y = c that dhqr_solve_adj_* computes from the factorisation (F, gamma) of
 // R_r^H.
-static bool spans_overlap(const void* p, size_t pbytes, const void* q, size_t qbytes) {
-    const uintptr_t p0 = (uintptr_t)p, q0 = (uintptr_t)q;
-    return pbytes > 0 && qbytes > 0 && p0 < q0 + qbytes && q0 < p0 + pbytes;
-}
-
 extern "C++" {   // as for the pivoted QR above
-
-// Arguments 1-10, which both entry points share but for the 7th: alpha (dhqr_cod_*, factor = true) or jpvt (dhqr_solve_cod_*).
-// Only the Float64 factorisation has a row limit: the ComplexF64 unpivoted path has none.
-template <typename T>
-static int check_cod(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* seventh,
-                     const void* dF, int64_t ldf, const void* d_gamma, bool factor) {
-    const size_t esz = sizeof(T);
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the complete orthogonal decomposition is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (factor && std::is_same<T, double>::value && n > narrow_panel_max_rows(c))   // R_r' has n rows and goes through the unpivoted path
-        return set_err(-3, "n = %lld exceeds the row limit of the unpivoted factorisation (%lld)", (long long)n,
-                       (long long)narrow_panel_max_rows(c));
-    if (rank < 0 || rank > n) return set_err(-4, "need 0 <= rank <= n");
-    if (n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_elem_ptr<T>(dA, -5, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
-    const char* name7 = factor ? "alpha" : "jpvt";
-    if (n > 0 && !seventh) return set_err(-7, "null %s", name7);
-    TRY(factor ? check_elem_ptr<T>(seventh, -7, name7) : check_elem_ptr<int64_t>(seventh, -7, name7));
-    if (rank > 0 && !dF) return set_err(-8, "null F");
-    TRY(check_elem_ptr<T>(dF, -8, "F"));
-    if (ldf < std::max<int64_t>(1, n)) return set_err(-9, "ldf < max(1,n)");
-    if (rank > 0 && !d_gamma) return set_err(-10, "null gamma");
-    TRY(check_elem_ptr<T>(d_gamma, -10, "gamma"));
-    if (factor && rank > 0) {                                          // F and gamma are written: neither may overlap an input
-        const size_t abytes = ((size_t)(n - 1) * lda + m) * esz, alphabytes = (size_t)n * esz;
-        const size_t fbytes = ((size_t)(rank - 1) * ldf + n) * esz, gbytes = (size_t)rank * esz;
-        if (spans_overlap(dF, fbytes, dA, abytes) || spans_overlap(dF, fbytes, seventh, alphabytes))
-            return set_err(-8, "F overlaps A or alpha");
-        if (spans_overlap(d_gamma, gbytes, dA, abytes) || spans_overlap(d_gamma, gbytes, seventh, alphabytes) ||
-            spans_overlap(d_gamma, gbytes, dF, fbytes))
-            return set_err(-10, "gamma overlaps A, alpha or F");
-    }
-    return 0;
-}
 
 // (F, gamma) <- the unpivoted factorisation of R_r^H (n x rank) in place
 static int qr_rrh(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, double* F, int64_t ldf, double* gamma) {
@@ -2540,7 +2540,19 @@ static int qr_rrh(dhqr_context* c, cudaStream_t st, int64_t n, int64_t rank, dou
 template <typename T>
 static int cod_factor(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const void* d_alpha, void* dF,
                       int64_t ldf, void* d_gamma, void* stream) {
-    TRY(check_cod<T>(c, m, n, rank, dA, lda, d_alpha, dF, ldf, d_gamma, true));
+    Check a(c, "the complete orthogonal decomposition");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    TRY(a);
+    if (std::is_same<T, double>::value)   // R_r' has n rows and goes through the unpivoted path; the ComplexF64 one has no row limit
+        a.require(n <= narrow_panel_max_rows(c), 3, "n = %lld exceeds the row limit of the unpivoted factorisation (%lld)", (long long)n,
+                  (long long)narrow_panel_max_rows(c));
+    a.require(rank >= 0 && rank <= n, 4, "need 0 <= rank <= n");
+    a.operand<T>(5, "A", dA, mat(m, n, lda), when(n > 0, NEED) | ALIGN);
+    a.operand<T>(7, "alpha", d_alpha, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<T>(8, "F", dF, mat(n, rank, ldf), when(rank > 0, NEED) | ALIGN | DISJOINT);     // F and gamma are written
+    a.operand<T>(10, "gamma", d_gamma, vec(rank), when(rank > 0, NEED) | ALIGN | DISJOINT);
+    TRY(a);
     if (n == 0 || rank == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2554,11 +2566,17 @@ static int cod_factor(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const
 template <typename T>
 static int cod_solve(dhqr_context* c, int64_t m, int64_t n, int64_t rank, const void* dA, int64_t lda, const int64_t* d_jpvt,
                      const void* dF, int64_t ldf, const void* d_gamma, void* d_b, int64_t ldb, int nrhs, void* stream) {
-    TRY(check_cod<T>(c, m, n, rank, dA, lda, d_jpvt, dF, ldf, d_gamma, false));
-    if (nrhs > 0 && !d_b) return set_err(-11, "null b");
-    TRY(check_elem_ptr<T>(d_b, -11, "b"));
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-12, "ldb < max(1,m)");
-    if (nrhs < 0) return set_err(-13, "nrhs < 0");
+    Check a(c, "the complete orthogonal decomposition");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.require(rank >= 0 && rank <= n, 4, "need 0 <= rank <= n");
+    a.operand<T>(5, "A", dA, mat(m, n, lda), when(n > 0, NEED) | ALIGN);
+    a.operand<int64_t>(7, "jpvt", d_jpvt, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<T>(8, "F", dF, mat(n, rank, ldf), when(rank > 0, NEED) | ALIGN);
+    a.operand<T>(10, "gamma", d_gamma, vec(rank), when(rank > 0, NEED) | ALIGN);
+    a.operand<T>(11, "b", d_b, mat(m, nrhs, ldb), when(nrhs > 0, NEED) | ALIGN);
+    a.require(nrhs >= 0, 13, "nrhs < 0");
+    TRY(a);
     if (n == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2725,47 +2743,25 @@ static int apply_append_local(dhqr_context* c, cudaStream_t st, int64_t n, int64
     return 0;
 }
 
-// Arguments 1-3 of every append and downdate call: handle, n, k (k capped by the panel kernel's slab capacity)
-static int check_append_head(dhqr_context* c, int64_t n, int64_t k, const char* what = "appending") {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "%s rows is single-GPU (the handle has %d ranks)", what, c->nranks);
-    if (n < 0) return set_err(-2, "n < 0");
-    if (k < 0) return set_err(-3, "k < 0");
-    if (k > narrow_panel_max_rows(c))
-        return set_err(-3, "k = %lld exceeds the rows one %s can take on this device (%lld): split the block", (long long)k,
-                       what[0] == 'a' ? "append" : "downdate", (long long)narrow_panel_max_rows(c));
-    return 0;
-}
+// k is capped by the panel kernel's slab capacity
+static const char* const TP_ROWS = "k = %lld exceeds the rows one %s can take on this device (%lld): split the block";
 
 // dhqr_qr_append_f64 (d_info == nullptr, the rows are B) and dhqr_qr_downdate_f64 (the rows are Z): the same checks and driver
 static int qr_tp(dhqr_context* c, int64_t n, int64_t k, double* dR, int64_t ldr, double* d_alpha, double* dB, int64_t ldb, double* d_vtop,
                  int64_t* d_info, bool hyp, void* stream) {
-    const char* b = hyp ? "Z" : "B";
-    TRY(check_append_head(c, n, k, hyp ? "deleting" : "appending"));
-    if (n > 0 && !dR) return set_err(-4, "null R");
-    TRY(check_elem_ptr<double>(dR, -4, "R"));
-    if (ldr < std::max<int64_t>(1, n)) return set_err(-5, "ldr < max(1,n)");
-    if (n > 0 && !d_alpha) return set_err(-6, "null alpha");
-    TRY(check_elem_ptr<double>(d_alpha, -6, "alpha"));
-    const size_t rbytes = n > 0 ? ((size_t)(n - 1) * ldr + n) * 8 : 0, abytes = (size_t)n * 8;
-    if (n > 0 && k > 0 && !dB) return set_err(-7, "null %s", b);
-    TRY(check_elem_ptr<double>(dB, -7, b));
-    const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0;
-    if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-7, "%s overlaps R or alpha", b);
-    if (ldb < std::max<int64_t>(1, k)) return set_err(-8, hyp ? "ldz < max(1,k)" : "ldb < max(1,k)");
-    if (n > 0 && !d_vtop) return set_err(-9, "null vtop");
-    TRY(check_elem_ptr<double>(d_vtop, -9, "vtop"));
-    if (k > 0 && (spans_overlap(d_vtop, abytes, dR, rbytes) || spans_overlap(d_vtop, abytes, d_alpha, abytes) ||
-                  spans_overlap(d_vtop, abytes, dB, bbytes)))
-        return set_err(-9, "vtop overlaps R, alpha or %s", b);
-    if (hyp) {
-        if (n > 0 && k > 0 && !d_info) return set_err(-10, "null info");
-        TRY(check_elem_ptr<int64_t>(d_info, -10, "info"));
-        if (n > 0 && k > 0 && (spans_overlap(d_info, 8, dR, rbytes) || spans_overlap(d_info, 8, d_alpha, abytes) ||
-                               spans_overlap(d_info, 8, dB, bbytes) || spans_overlap(d_info, 8, d_vtop, abytes)))
-            return set_err(-10, "info overlaps R, alpha, Z or vtop");
-    }
-    if (n == 0 || k == 0) return 0;
+    const bool work = n > 0 && k > 0;
+    Check a(c, hyp ? "deleting rows" : "appending rows");
+    a.require(n >= 0, 2, "n < 0");
+    a.require(k >= 0, 3, "k < 0");
+    TRY(a);
+    a.require(k <= narrow_panel_max_rows(c), 3, TP_ROWS, (long long)k, hyp ? "downdate" : "append", (long long)narrow_panel_max_rows(c));
+    a.operand<double>(4, "R", dR, mat(n, n, ldr), when(n > 0, NEED) | ALIGN);
+    a.operand<double>(6, "alpha", d_alpha, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<double>(7, hyp ? "Z" : "B", dB, mat(k, n, ldb), when(work, NEED) | ALIGN | DISJOINT);
+    a.operand<double>(9, "vtop", d_vtop, vec(n), when(n > 0, NEED) | ALIGN | when(k > 0, DISJOINT));
+    if (hyp) a.operand<int64_t>(10, "info", d_info, vec(1), when(work, NEED | DISJOINT) | ALIGN);
+    TRY(a);
+    if (!work) return 0;
     CU(cudaSetDevice(c->device));
     return qr_append_local(c, (cudaStream_t)stream, n, k, dR, ldr, d_alpha, dB, ldb, d_vtop, hyp ? d_info : nullptr);
 }
@@ -2783,26 +2779,17 @@ int dhqr_qr_downdate_f64(dhqr_handle c, int64_t n, int64_t k, double* dR, int64_
 // the three applies: Q~' (trans = 0), Q~ (trans = 1) of the append, Theta of the downdate (hyp, trans = 0); the rows are B or Z
 static int apply_append(dhqr_context* c, int64_t n, int64_t k, const double* dB, int64_t ldb, const double* d_vtop, double* d_c,
                         int64_t ldc, double* d_e, int64_t lde, int nrhs, void* stream, int trans, bool hyp = false) {
-    const char* b = hyp ? "Z" : "B";
-    TRY(check_append_head(c, n, k, hyp ? "deleting" : "appending"));
-    if (n > 0 && k > 0 && !dB) return set_err(-4, "null %s", b);
-    TRY(check_elem_ptr<double>(dB, -4, b));
-    if (ldb < std::max<int64_t>(1, k)) return set_err(-5, hyp ? "ldz < max(1,k)" : "ldb < max(1,k)");
-    if (n > 0 && !d_vtop) return set_err(-6, "null vtop");
-    TRY(check_elem_ptr<double>(d_vtop, -6, "vtop"));
-    const size_t bbytes = (n > 0 && k > 0) ? ((size_t)(n - 1) * ldb + k) * 8 : 0, vbytes = (size_t)n * 8;
-    const size_t cbytes = (n > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * ldc + n) * 8 : 0;
-    const size_t ebytes = (k > 0 && nrhs > 0) ? ((size_t)(nrhs - 1) * lde + k) * 8 : 0;
-    if (n > 0 && nrhs > 0 && !d_c) return set_err(-7, "null c");
-    TRY(check_elem_ptr<double>(d_c, -7, "c"));
-    if (spans_overlap(d_c, cbytes, dB, bbytes) || spans_overlap(d_c, cbytes, d_vtop, vbytes)) return set_err(-7, "c overlaps %s or vtop", b);
-    if (ldc < std::max<int64_t>(1, n)) return set_err(-8, "ldc < max(1,n)");
-    if (k > 0 && nrhs > 0 && !d_e) return set_err(-9, "null e");
-    TRY(check_elem_ptr<double>(d_e, -9, "e"));
-    if (spans_overlap(d_e, ebytes, dB, bbytes) || spans_overlap(d_e, ebytes, d_vtop, vbytes) || spans_overlap(d_e, ebytes, d_c, cbytes))
-        return set_err(-9, "e overlaps %s, vtop or c", b);
-    if (lde < std::max<int64_t>(1, k)) return set_err(-10, "lde < max(1,k)");
-    if (nrhs < 0) return set_err(-11, "nrhs < 0");
+    Check a(c, hyp ? "deleting rows" : "appending rows");
+    a.require(n >= 0, 2, "n < 0");
+    a.require(k >= 0, 3, "k < 0");
+    TRY(a);
+    a.require(k <= narrow_panel_max_rows(c), 3, TP_ROWS, (long long)k, hyp ? "downdate" : "append", (long long)narrow_panel_max_rows(c));
+    a.operand<double>(4, hyp ? "Z" : "B", dB, mat(k, n, ldb), when(n > 0 && k > 0, NEED) | ALIGN);
+    a.operand<double>(6, "vtop", d_vtop, vec(n), when(n > 0, NEED) | ALIGN);
+    a.operand<double>(7, "c", d_c, mat(n, nrhs, ldc), when(n > 0 && nrhs > 0, NEED) | ALIGN | DISJOINT);
+    a.operand<double>(9, "e", d_e, mat(k, nrhs, lde), when(k > 0 && nrhs > 0, NEED) | ALIGN | DISJOINT);
+    a.require(nrhs >= 0, 11, "nrhs < 0");
+    TRY(a);
     if (n == 0 || k == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     return apply_append_local(c, (cudaStream_t)stream, n, k, dB, ldb, d_vtop, d_c, ldc, d_e, lde, nrhs, trans, hyp);
@@ -2824,32 +2811,6 @@ int dhqr_apply_downdate_f64(dhqr_handle c, int64_t n, int64_t k, const double* d
 }
 
 // ---- batched QR of many small problems (DESIGN §2.12) -----------------------------------------------------------------------
-// Bytes from the first element of a batch of `batch` operands (rows x cols, leading dimension ld, `stride` apart) to one past the
-// last; 0 when there is none.  The stride counts only when batch > 1, a negative one as 0 (the stride check rejects it next), and
-// the span is clamped, so that an absurd stride cannot wrap the interval test.
-static size_t batch_span(int64_t batch, int64_t stride, int64_t rows, int64_t cols, int64_t ld) {
-    if (batch <= 0 || rows <= 0 || cols <= 0) return 0;
-    const __int128 e = (__int128)(batch - 1) * std::max<int64_t>(stride, 0) + (__int128)(cols - 1) * ld + rows;
-    return e > ((__int128)1 << 58) ? (size_t)1 << 61 : (size_t)e * 8;
-}
-
-// Arguments 1-7 of every batched entry point: handle, m, n, batch, A, lda, stride_a
-static int check_batched_head(dhqr_context* c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a) {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the batched QR is single-GPU (the handle has %d ranks)", c->nranks);
-    if (m < 0) return set_err(-2, "m < 0");
-    if (n < 0 || n > m) return set_err(-3, "need 0 <= n <= m");
-    if (n > 0 && m > BQ_MAX_ELEMS / n)
-        return set_err(-3, "m * n exceeds batch_max_elems (%lld): factor a problem this large with dhqr_qr_f64", (long long)BQ_MAX_ELEMS);
-    if (batch < 0) return set_err(-4, "batch < 0");
-    if (batch * batched_geom(m, n).cs > INT32_MAX) return set_err(-4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
-    if (batch > 0 && n > 0 && !dA) return set_err(-5, "null A");
-    TRY(check_elem_ptr<double>(dA, -5, "A"));
-    if (lda < std::max<int64_t>(1, m)) return set_err(-6, "lda < max(1,m)");
-    if (batch > 1 && (__int128)stride_a < (__int128)lda * n) return set_err(-7, "stride_a < lda * n");
-    return 0;
-}
-
 extern "C++" {   // as for the pivoted QR above
 template <typename Kernel, typename... Args>
 static int launch_batched(dhqr_context* c, cudaStream_t st, const char* what, double work, Kernel kern, const BatchedGeom& g,
@@ -2872,12 +2833,17 @@ static int launch_batched(dhqr_context* c, cudaStream_t st, const char* what, do
 
 int dhqr_qr_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, double* dA, int64_t lda, int64_t stride_a,
                         double* d_alpha, int64_t stride_alpha, void* stream) {
-    TRY(check_batched_head(c, m, n, batch, dA, lda, stride_a));
-    if (batch > 0 && n > 0 && !d_alpha) return set_err(-8, "null alpha");
-    TRY(check_elem_ptr<double>(d_alpha, -8, "alpha"));
-    if (spans_overlap(d_alpha, batch_span(batch, stride_alpha, n, 1, n), dA, batch_span(batch, stride_a, m, n, lda)))
-        return set_err(-8, "alpha overlaps A");
-    if (batch > 1 && stride_alpha < n) return set_err(-9, "stride_alpha < n");
+    Check a(c, "the batched QR");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.require(n == 0 || m <= BQ_MAX_ELEMS / n, 3, "m * n exceeds batch_max_elems (%lld): factor a problem this large with dhqr_qr_f64",
+              (long long)BQ_MAX_ELEMS);
+    a.require(batch >= 0, 4, "batch < 0");
+    TRY(a);
+    a.require(batch * batched_geom(m, n).cs <= INT32_MAX, 4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
+    a.operand<double>(5, "A", dA, mat(m, n, lda, batch, stride_a), when(batch > 0 && n > 0, NEED) | ALIGN);
+    a.operand<double>(8, "alpha", d_alpha, vec(n, batch, stride_alpha), when(batch > 0 && n > 0, NEED) | ALIGN | DISJOINT);
+    TRY(a);
     if (batch == 0 || n == 0) return 0;
     CU(cudaSetDevice(c->device));
     const BatchedGeom g = batched_geom(m, n);
@@ -2891,24 +2857,20 @@ int dhqr_qr_batched_f64(dhqr_handle c, int64_t m, int64_t n, int64_t batch, doub
 static int apply_batched(dhqr_context* c, int64_t m, int64_t n, int64_t batch, const double* dA, int64_t lda, int64_t stride_a,
                          const double* d_alpha, int64_t stride_alpha, double* d_b, int64_t ldb, int64_t stride_b, int nrhs, void* stream,
                          bool trans, bool solve) {
-    TRY(check_batched_head(c, m, n, batch, dA, lda, stride_a));
-    const size_t abytes = batch_span(batch, stride_a, m, n, lda);
-    const size_t albytes = solve ? batch_span(batch, stride_alpha, n, 1, n) : 0;
+    Check a(c, "the batched QR");
+    a.require(m >= 0, 2, "m < 0");
+    a.require(n >= 0 && n <= m, 3, "need 0 <= n <= m");
+    a.require(n == 0 || m <= BQ_MAX_ELEMS / n, 3, "m * n exceeds batch_max_elems (%lld): factor a problem this large with dhqr_qr_f64",
+              (long long)BQ_MAX_ELEMS);
+    a.require(batch >= 0, 4, "batch < 0");
+    TRY(a);
+    a.require(batch * batched_geom(m, n).cs <= INT32_MAX, 4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
+    a.operand<double>(5, "A", dA, mat(m, n, lda, batch, stride_a), when(batch > 0 && n > 0, NEED) | ALIGN);
     const int o = solve ? 2 : 0;
-    if (solve) {
-        if (batch > 0 && n > 0 && !d_alpha) return set_err(-8, "null alpha");
-        TRY(check_elem_ptr<double>(d_alpha, -8, "alpha"));
-        if (spans_overlap(d_alpha, albytes, dA, abytes)) return set_err(-8, "alpha overlaps A");
-        if (batch > 1 && stride_alpha < n) return set_err(-9, "stride_alpha < n");
-    }
-    if (batch > 0 && n > 0 && nrhs > 0 && !d_b) return set_err(-8 - o, "null b");
-    TRY(check_elem_ptr<double>(d_b, -8 - o, "b"));
-    const size_t bbytes = batch_span(batch, stride_b, m, nrhs, ldb);
-    if (spans_overlap(d_b, bbytes, dA, abytes) || spans_overlap(d_b, bbytes, d_alpha, albytes))
-        return set_err(-8 - o, solve ? "b overlaps A or alpha" : "b overlaps A");
-    if (ldb < std::max<int64_t>(1, m)) return set_err(-9 - o, "ldb < max(1,m)");
-    if (batch > 1 && (__int128)stride_b < (__int128)ldb * nrhs) return set_err(-10 - o, "stride_b < ldb * nrhs");
-    if (nrhs < 0) return set_err(-11 - o, "nrhs < 0");
+    if (solve) a.operand<double>(8, "alpha", d_alpha, vec(n, batch, stride_alpha), when(batch > 0 && n > 0, NEED) | ALIGN | DISJOINT);
+    a.operand<double>(8 + o, "b", d_b, mat(m, nrhs, ldb, batch, stride_b), when(batch > 0 && n > 0 && nrhs > 0, NEED) | ALIGN | DISJOINT);
+    a.require(nrhs >= 0, 11 + o, "nrhs < 0");
+    TRY(a);
     if (batch == 0 || n == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     const BatchedGeom g = batched_geom(m, n);
@@ -2947,69 +2909,28 @@ static int tp_batched(dhqr_context* c, int64_t n, int64_t k, int64_t batch, doub
                       int64_t stride_alpha, double* dB, int64_t ldb, int64_t stride_b, double* d_vtop, int64_t stride_vtop, double* d_c,
                       int64_t ldc, int64_t stride_c, double* d_e, int64_t lde, int64_t stride_e, int nrhs, int64_t* d_info, bool hyp,
                       void* stream) {
-    const char* b = hyp ? "Z" : "B";
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the batched %s is single-GPU (the handle has %d ranks)", hyp ? "downdate" : "append", c->nranks);
-    if (n < 0) return set_err(-2, "n < 0");
-    if (k < 0) return set_err(-3, "k < 0");
     const int64_t ncol = n + std::max(nrhs, 0);
-    if (ncol > BQ_UPD_MAX_COLS)
-        return set_err(-3, "n + nrhs = %lld exceeds batch_update_max_cols (%d)", (long long)ncol, BQ_UPD_MAX_COLS);
-    if (ncol > 0 && k > BQ_MAX_ELEMS / ncol)
-        return set_err(-3, "k * (n + nrhs) exceeds batch_max_elems (%lld): split the block", (long long)BQ_MAX_ELEMS);
-    if (batch < 0) return set_err(-4, "batch < 0");
-    if (batch * batched_geom(k, ncol).cs > INT32_MAX) return set_err(-4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
     const bool work = batch > 0 && n > 0 && k > 0, rhs = work && nrhs > 0;
-    if (batch > 0 && n > 0 && !dR) return set_err(-5, "null R");
-    TRY(check_elem_ptr<double>(dR, -5, "R"));
-    if (ldr < std::max<int64_t>(1, n)) return set_err(-6, "ldr < max(1,n)");
-    if (batch > 1 && (__int128)stride_r < (__int128)ldr * n) return set_err(-7, "stride_r < ldr * n");
-    const size_t rbytes = batch_span(batch, stride_r, n, n, ldr), abytes = batch_span(batch, stride_alpha, n, 1, n);
-    if (batch > 0 && n > 0 && !d_alpha) return set_err(-8, "null alpha");
-    TRY(check_elem_ptr<double>(d_alpha, -8, "alpha"));
-    if (spans_overlap(d_alpha, abytes, dR, rbytes)) return set_err(-8, "alpha overlaps R");
-    if (batch > 1 && stride_alpha < n) return set_err(-9, "stride_alpha < n");
-    const size_t bbytes = work ? batch_span(batch, stride_b, k, n, ldb) : 0;
-    if (work && !dB) return set_err(-10, "null %s", b);
-    TRY(check_elem_ptr<double>(dB, -10, b));
-    if (spans_overlap(dB, bbytes, dR, rbytes) || spans_overlap(dB, bbytes, d_alpha, abytes)) return set_err(-10, "%s overlaps R or alpha", b);
-    if (ldb < std::max<int64_t>(1, k)) return set_err(-11, hyp ? "ldz < max(1,k)" : "ldb < max(1,k)");
-    if (batch > 1 && (__int128)stride_b < (__int128)ldb * n) return set_err(-12, hyp ? "stride_z < ldz * n" : "stride_b < ldb * n");
-    const size_t vbytes = work ? batch_span(batch, stride_vtop, n, 1, n) : 0;
-    if (work && !d_vtop) return set_err(-13, "null vtop");
-    TRY(check_elem_ptr<double>(d_vtop, -13, "vtop"));
-    if (spans_overlap(d_vtop, vbytes, dR, rbytes) || spans_overlap(d_vtop, vbytes, d_alpha, abytes) || spans_overlap(d_vtop, vbytes, dB, bbytes))
-        return set_err(-13, "vtop overlaps R, alpha or %s", b);
-    if (batch > 1 && stride_vtop < n) return set_err(-14, "stride_vtop < n");
-    size_t cbytes = 0, ebytes = 0;
+    Check a(c, hyp ? "the batched downdate" : "the batched append");
+    a.require(n >= 0, 2, "n < 0");
+    a.require(k >= 0, 3, "k < 0");
+    a.require(ncol <= BQ_UPD_MAX_COLS, 3, "n + nrhs = %lld exceeds batch_update_max_cols (%d)", (long long)ncol, BQ_UPD_MAX_COLS);
+    a.require(ncol == 0 || k <= BQ_MAX_ELEMS / ncol, 3, "k * (n + nrhs) exceeds batch_max_elems (%lld): split the block",
+              (long long)BQ_MAX_ELEMS);
+    a.require(batch >= 0, 4, "batch < 0");
+    TRY(a);
+    a.require(batch * batched_geom(k, ncol).cs <= INT32_MAX, 4, "batch too large for one grid (batch x CTAs per problem > 2^31 - 1)");
+    a.operand<double>(5, "R", dR, mat(n, n, ldr, batch, stride_r), when(batch > 0 && n > 0, NEED) | ALIGN);
+    a.operand<double>(8, "alpha", d_alpha, vec(n, batch, stride_alpha), when(batch > 0 && n > 0, NEED) | ALIGN | DISJOINT);
+    a.operand<double>(10, hyp ? "Z" : "B", dB, mat(k, n, ldb, batch, stride_b), when(work, NEED) | ALIGN | DISJOINT);
+    a.operand<double>(13, "vtop", d_vtop, vec(n, batch, stride_vtop), when(work, NEED | DISJOINT) | ALIGN);
     if (nrhs > 0) {
-        cbytes = rhs ? batch_span(batch, stride_c, n, nrhs, ldc) : 0;
-        if (rhs && !d_c) return set_err(-15, "null c");
-        TRY(check_elem_ptr<double>(d_c, -15, "c"));
-        if (spans_overlap(d_c, cbytes, dR, rbytes) || spans_overlap(d_c, cbytes, d_alpha, abytes) || spans_overlap(d_c, cbytes, dB, bbytes) ||
-            spans_overlap(d_c, cbytes, d_vtop, vbytes))
-            return set_err(-15, "c overlaps R, alpha, %s or vtop", b);
-        if (ldc < std::max<int64_t>(1, n)) return set_err(-16, "ldc < max(1,n)");
-        if (batch > 1 && (__int128)stride_c < (__int128)ldc * nrhs) return set_err(-17, "stride_c < ldc * nrhs");
-        ebytes = rhs ? batch_span(batch, stride_e, k, nrhs, lde) : 0;
-        if (rhs && !d_e) return set_err(-18, "null e");
-        TRY(check_elem_ptr<double>(d_e, -18, "e"));
-        if (spans_overlap(d_e, ebytes, dR, rbytes) || spans_overlap(d_e, ebytes, d_alpha, abytes) || spans_overlap(d_e, ebytes, dB, bbytes) ||
-            spans_overlap(d_e, ebytes, d_vtop, vbytes) || spans_overlap(d_e, ebytes, d_c, cbytes))
-            return set_err(-18, "e overlaps R, alpha, %s, vtop or c", b);
-        if (lde < std::max<int64_t>(1, k)) return set_err(-19, "lde < max(1,k)");
-        if (batch > 1 && (__int128)stride_e < (__int128)lde * nrhs) return set_err(-20, "stride_e < lde * nrhs");
+        a.operand<double>(15, "c", d_c, mat(n, nrhs, ldc, batch, stride_c), when(rhs, NEED | DISJOINT) | ALIGN);
+        a.operand<double>(18, "e", d_e, mat(k, nrhs, lde, batch, stride_e), when(rhs, NEED | DISJOINT) | ALIGN);
     }
-    if (nrhs < 0) return set_err(-21, "nrhs < 0");
-    if (hyp) {
-        const size_t ibytes = work ? (size_t)batch * 8 : 0;
-        if (work && !d_info) return set_err(-22, "null info");
-        TRY(check_elem_ptr<int64_t>(d_info, -22, "info"));
-        if (spans_overlap(d_info, ibytes, dR, rbytes) || spans_overlap(d_info, ibytes, d_alpha, abytes) ||
-            spans_overlap(d_info, ibytes, dB, bbytes) || spans_overlap(d_info, ibytes, d_vtop, vbytes) ||
-            spans_overlap(d_info, ibytes, d_c, cbytes) || spans_overlap(d_info, ibytes, d_e, ebytes))
-            return set_err(-22, "info overlaps R, alpha, Z, vtop, c or e");
-    }
+    a.require(nrhs >= 0, 21, "nrhs < 0");
+    if (hyp) a.operand<int64_t>(22, "info", d_info, vec(batch), when(work, NEED | DISJOINT) | ALIGN);
+    TRY(a);
     if (!work) return 0;
     CU(cudaSetDevice(c->device));
     const BatchedGeom g = batched_geom(k, ncol);
@@ -3039,27 +2960,16 @@ int dhqr_qr_downdate_batched_f64(dhqr_handle c, int64_t n, int64_t k, int64_t ba
 int dhqr_backsolve_batched_f64(dhqr_handle c, int64_t n, int64_t batch, const double* dR, int64_t ldr, int64_t stride_r,
                                const double* d_alpha, int64_t stride_alpha, double* d_b, int64_t ldb, int64_t stride_b, int nrhs,
                                void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (c->nranks != 1) return set_err(-1, "the batched back-substitution is single-GPU (the handle has %d ranks)", c->nranks);
-    if (n < 0) return set_err(-2, "n < 0");
-    if (n > BQ_UPD_MAX_COLS) return set_err(-2, "n = %lld exceeds batch_update_max_cols (%d)", (long long)n, BQ_UPD_MAX_COLS);
-    if (batch < 0) return set_err(-3, "batch < 0");
-    if (batch > INT32_MAX) return set_err(-3, "batch too large for one grid (> 2^31 - 1)");
-    if (batch > 0 && n > 0 && !dR) return set_err(-4, "null R");
-    TRY(check_elem_ptr<double>(dR, -4, "R"));
-    if (ldr < std::max<int64_t>(1, n)) return set_err(-5, "ldr < max(1,n)");
-    if (batch > 1 && (__int128)stride_r < (__int128)ldr * n) return set_err(-6, "stride_r < ldr * n");
-    const size_t rbytes = batch_span(batch, stride_r, n, n, ldr), abytes = batch_span(batch, stride_alpha, n, 1, n);
-    if (batch > 0 && n > 0 && !d_alpha) return set_err(-7, "null alpha");
-    TRY(check_elem_ptr<double>(d_alpha, -7, "alpha"));
-    if (batch > 1 && stride_alpha < n) return set_err(-8, "stride_alpha < n");
-    if (batch > 0 && n > 0 && nrhs > 0 && !d_b) return set_err(-9, "null b");
-    TRY(check_elem_ptr<double>(d_b, -9, "b"));
-    const size_t bbytes = batch_span(batch, stride_b, n, nrhs, ldb);
-    if (spans_overlap(d_b, bbytes, dR, rbytes) || spans_overlap(d_b, bbytes, d_alpha, abytes)) return set_err(-9, "b overlaps R or alpha");
-    if (ldb < std::max<int64_t>(1, n)) return set_err(-10, "ldb < max(1,n)");
-    if (batch > 1 && (__int128)stride_b < (__int128)ldb * nrhs) return set_err(-11, "stride_b < ldb * nrhs");
-    if (nrhs < 0) return set_err(-12, "nrhs < 0");
+    Check a(c, "the batched back-substitution");
+    a.require(n >= 0, 2, "n < 0");
+    a.require(n <= BQ_UPD_MAX_COLS, 2, "n = %lld exceeds batch_update_max_cols (%d)", (long long)n, BQ_UPD_MAX_COLS);
+    a.require(batch >= 0, 3, "batch < 0");
+    a.require(batch <= INT32_MAX, 3, "batch too large for one grid (> 2^31 - 1)");
+    a.operand<double>(4, "R", dR, mat(n, n, ldr, batch, stride_r), when(batch > 0 && n > 0, NEED) | ALIGN);
+    a.operand<double>(7, "alpha", d_alpha, vec(n, batch, stride_alpha), when(batch > 0 && n > 0, NEED) | ALIGN);
+    a.operand<double>(9, "b", d_b, mat(n, nrhs, ldb, batch, stride_b), when(batch > 0 && n > 0 && nrhs > 0, NEED) | ALIGN | DISJOINT);
+    a.require(nrhs >= 0, 12, "nrhs < 0");
+    TRY(a);
     if (batch == 0 || n == 0 || nrhs == 0) return 0;
     CU(cudaSetDevice(c->device));
     const int kc = (int)std::min<int64_t>({(int64_t)BQ_KC, BQ_SLAB / n, (int64_t)nrhs});
@@ -3130,10 +3040,12 @@ int dhqr_plan_host_upload(int64_t m, int64_t n, int nb, int chunk, int first, in
 }
 
 int dhqr_qr_host_f64(dhqr_handle c, int64_t m, int64_t n, double* hA, int64_t lda, double* h_alpha, int nb) {
-    TRY(check_common(c, m, n, 0, n, hA, lda));
-    if (n > 0 && !h_alpha) return set_err(-6, "null alpha");
-    if (c->nranks != 1) return set_err(-1, "host entry points are single-GPU");
-    if (nb != 0 && nb != 1 && (nb < 32 || nb > 128 || nb % 32)) return set_err(-9, "nb must be 0, 1 or a multiple of 32 in [32,128]");
+    Check a(c, "the host entry");   // hA, lda and h_alpha keep the codes of dA_local, lda and d_alpha of dhqr_qr_f64
+    column_block(a, m, n, 0, n);
+    a.operand<double>(6, "A", hA, mat(m, n, lda), when(n > 0, NEED));
+    a.operand<double>(6, "alpha", h_alpha, vec(n), when(n > 0, NEED));
+    a.require(nb == 0 || nb == 1 || (nb >= 32 && nb <= 128 && nb % 32 == 0), 9, "nb must be 0, 1 or a multiple of 32 in [32,128]");
+    TRY(a);
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     const int64_t ldd = rup(m, 32);                       // padded device leading dimension (aligned TMA sources)
@@ -3223,11 +3135,13 @@ int dhqr_qr_host_f64(dhqr_handle c, int64_t m, int64_t n, double* hA, int64_t ld
 
 int dhqr_ldiv_host_f64(dhqr_handle c, int64_t m, int64_t n, const double* hA, int64_t lda, const double* h_alpha,
                        const double* h_b, double* h_x) {
-    TRY(check_common(c, m, n, 0, n, hA, lda));
-    if (n > 0 && !h_alpha) return set_err(-6, "null alpha");
-    if (m > 0 && !h_b) return set_err(-7, "null b");
-    if (n > 0 && !h_x) return set_err(-8, "null x");
-    if (c->nranks != 1) return set_err(-1, "host entry points are single-GPU");
+    Check a(c, "the host entry");   // hA, lda and h_alpha keep the codes of dA_local, lda and d_alpha of dhqr_qr_f64
+    column_block(a, m, n, 0, n);
+    a.operand<double>(6, "A", hA, mat(m, n, lda), when(n > 0, NEED));
+    a.operand<double>(6, "alpha", h_alpha, vec(n), when(n > 0, NEED));
+    a.operand<double>(7, "b", h_b, vec(m), when(m > 0, NEED));
+    a.operand<double>(8, "x", h_x, vec(n), when(n > 0, NEED));
+    TRY(a);
     if (n == 0) return 0;
     CU(cudaSetDevice(c->device));
     const int64_t ldd = rup(m, 32);
@@ -3246,21 +3160,18 @@ int dhqr_ldiv_host_f64(dhqr_handle c, int64_t m, int64_t n, const double* hA, in
 }
 
 // ---- primitives ---------------------------------------------------------------------------------
-extern "C++" {   // as for form_q above
+extern "C++" {   // as for the adjoint solves above
 
 template <typename T>
 static int partialdot(dhqr_context* c, const void* d_a, const void* d_b, int64_t i0, int64_t i1, void* d_out, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (!d_a) return set_err(-2, "null a");
-    if (!d_b) return set_err(-3, "null b");
-    if (i0 < 0) return set_err(-4, "i0 < 0");
-    if (i1 < i0) return set_err(-5, "i1 < i0");
-    if (!d_out) return set_err(-6, "null out");
-    if (std::is_same<T, double2>::value) {                  // Float64 pointers are not checked for alignment here
-        TRY(check_elem_ptr<T>(d_a, -2, "a"));
-        TRY(check_elem_ptr<T>(d_b, -3, "b"));
-        TRY(check_elem_ptr<T>(d_out, -6, "out"));
-    }
+    const unsigned rules = NEED | when(std::is_same<T, double2>::value, ALIGN);   // Float64 pointers are not checked for alignment here
+    Check a(c);
+    a.operand<T>(2, "a", d_a, vec(i1), rules);
+    a.operand<T>(3, "b", d_b, vec(i1), rules);
+    a.require(i0 >= 0, 4, "i0 < 0");
+    a.require(i1 >= i0, 5, "i1 < i0");
+    a.operand<T>(6, "out", d_out, vec(1), rules);
+    TRY(a);
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     return launch(c, st, kname<T>("k_partialdot", "k_partialdot_c"), 0.0, [&](CwtSlot) {
@@ -3283,12 +3194,12 @@ int dhqr_partialdot_c64(dhqr_handle c, const void* d_a, const void* d_b, int64_t
 
 int dhqr_fill_uniform_f64(dhqr_handle c, uint64_t seed, int64_t i0, int64_t j0, int64_t m, int64_t n, double* dA,
                           int64_t lda, void* stream) {
-    if (!c) return set_err(-1, "null handle");
-    if (m < 0) return set_err(-5, "m < 0");
-    if (n < 0) return set_err(-6, "n < 0");
+    Check a(c);
+    a.require(m >= 0, 5, "m < 0");
+    a.require(n >= 0, 6, "n < 0");
+    TRY(a);
     if (m == 0 || n == 0) return 0;
-    if (!dA) return set_err(-7, "null matrix");
-    if (lda < m) return set_err(-8, "lda < m");
+    TRY(a.operand<double>(7, "A", dA, mat(m, n, lda), NEED));
     CU(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid((unsigned)std::min<int64_t>((m + 255) / 256, 1024), (unsigned)std::min<int64_t>(n, 4096));
